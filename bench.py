@@ -2,10 +2,10 @@
 """bench.py -- predict QPS of the route -> ensure-resident -> predict hot path on a Zipf
 multi-model mix (BASELINE.json metric), one process per GPU.
 
-Workload (config.workload): the per-GPU shard of BASELINE.json configs[2] -- the configuration the
-north_star target is quoted on: N GPUs serve 125*N per-tenant 3-layer MLPs (9216^4 fp32,
-1 019 326 464 B each), Zipf(alpha=1.0) request stream, ring replicas = min(2, N).  Per-GPU work is
-fixed as N grows (weak scaling); at N=8 it is exactly configs[2] (1000 models, replicas 2).
+Workload (config.workload): BASELINE.json configs[2] sized for an 80 GB H100: N GPUs serve 60*N
+per-tenant 3-layer MLPs (9216^4 fp32, 1 019 326 464 B each; 60 of them, 61 GB, stay resident in the
+HBM arena with room for activations and workspaces), Zipf(alpha=1.0) request stream, ring replicas =
+min(2, N).  Per-GPU work is fixed as N grows (weak scaling).
 
 A "step" is one batcher tick: `--tick` (default 1024) requests per GPU drawn from the seeded Zipf
 trace, routed with the consistent-hash ring, grouped per resident model and executed.
@@ -41,7 +41,7 @@ sys.path.insert(0, ROOT)
 
 DIMS = [9216, 9216, 9216, 9216]
 MODEL_BYTES = 1019326464
-MODELS_PER_GPU = 125
+MODELS_PER_GPU = 60
 IN_DIM, OUT_DIM = DIMS[0], DIMS[-1]
 
 
@@ -54,7 +54,7 @@ def parse_args():
     ap.add_argument("--tick", type=int, default=1024, help="requests per GPU per step")
     ap.add_argument("--clients", type=int, default=1024, help="closed-loop client threads per GPU (e2e)")
     ap.add_argument("--models-per-gpu", type=int, default=MODELS_PER_GPU)
-    ap.add_argument("--arena-gib", type=float, default=160.0)
+    ap.add_argument("--arena-gib", type=float, default=64.0)
     ap.add_argument("--host-gib", type=float, default=0.0, help="pinned host tier per GPU (0 = auto)")
     ap.add_argument("--e2e-steps", type=int, default=0, help="0 = same as --steps")
     ap.add_argument("--cpu-sample", type=int, default=48, help="requests in the cpu_baseline sample")
@@ -71,6 +71,8 @@ def parse_args():
                     help="clock samplers running during the timed regions (A/B their perturbation with 'none')")
     ap.add_argument("--replica-pick", default="balanced", choices=["balanced", "hot-spread", "random", "first", "hash"],
                     help="replica choice among the ring's GetN candidates (reference: random)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (rank 0)")
     return ap.parse_args()
 
 
@@ -172,7 +174,7 @@ def step_plan(wl, rank, step, tick_global):
 
 
 def pass_plan(rows, tc_min=9):
-    """Mirror of launch_dense (csrc/kernels.cu): groups of >= 9 rows take the tcgen05 path, 64 rows per
+    """Mirror of launch_dense (csrc/kernels.cu): groups of >= 9 rows take the wgmma path, 64 rows per
     pass; what is left (<= 8 rows) takes one SIMT streaming pass."""
     out, r = [], rows
     while tc_min > 0 and r >= tc_min:
@@ -344,9 +346,9 @@ def pin_to_gpu_numa(gpu_index):
 def workload_string(models_per_gpu, dims, replicas, pick_policy):
     """config.workload, identical for the b200 arm and the reference arm (same workload, two implementations)"""
     model_bytes = sum(dims[i] * dims[i + 1] * 4 + dims[i + 1] * 4 for i in range(len(dims) - 1))
-    return (f"BASELINE configs[2] per-GPU shard: {models_per_gpu} per-tenant 3-layer MLP "
+    return (f"BASELINE configs[2] per-GPU shard sized for 80 GB: {models_per_gpu} per-tenant 3-layer MLP "
             f"({'x'.join(map(str, dims))} fp32, {model_bytes} B) per GPU, Zipf alpha=1.0, ring replicas={replicas} "
-            f"(replica pick: {pick_policy}); at 8 GPUs = configs[2] (1000 models)")
+            f"(replica pick: {pick_policy})")
 
 
 def _peaks():
@@ -387,10 +389,37 @@ def graph_model_speed(kind, steps=30):
         torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / steps
     tfl = flop * rows / (ms * 1e-3) / 1e12
-    peak = _peaks().get("bf16_tflops_sustained", 1405.4)
+    peak = _peaks().get("bf16_tflops_sustained", 989.0)   # fallback: H100 SXM data sheet, dense BF16
     return {"batch": rows, "ms_per_batch": round(ms, 3), "items_per_s": round(rows / (ms * 1e-3), 1), "tflops": round(tfl, 2),
             "frac_of_bf16_sustained": round(tfl / peak, 4), "launches_per_batch": int(per_pass), "weights_bytes": man["weights_bytes"],
-            "note": "fp32 in/out, 3xTF32 tcgen05 GEMMs; device-resident inputs, one model, CUDA events"}
+            "note": "fp32 in/out, 3xTF32 wgmma GEMMs; device-resident inputs, one model, CUDA events"}
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, plan, x_dev, y_dev, xb_dev, yb_dev, out_dim):
+    """The rows the last timed step returned to its callers, in launch order, as <out_dir>/y.npy (float32), with the model
+    index of every row (model_ids.npy). Above DUMP_LIMIT_BYTES a fixed, seeded sample of rows is kept (rows.npy)."""
+    import torch
+    torch.cuda.synchronize()
+    ys, ids = [], []
+    for name, rows, _xp, yp in plan["launches"]:
+        base, buf = (y_dev, y_dev.data_ptr()) if y_dev.data_ptr() <= yp < y_dev.data_ptr() + y_dev.numel() * 4 else (yb_dev, yb_dev.data_ptr())
+        r0 = (yp - buf) // (out_dim * 4)
+        ys.append(base[r0:r0 + rows].cpu())
+        ids += [int(name.decode()[1:])] * rows
+    y = torch.cat(ys).numpy().astype(np.float32)
+    ids = np.asarray(ids, np.float64)
+    rows = np.arange(len(y), dtype=np.float64)
+    cap = DUMP_LIMIT_BYTES // (out_dim * 4 + 16)
+    if len(y) > cap:
+        keep = np.sort(np.random.default_rng(0).choice(len(y), cap, replace=False))
+        y, ids, rows = y[keep], ids[keep], rows[keep]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "y.npy"), y)
+    np.save(os.path.join(out_dir, "model_ids.npy"), ids)
+    np.save(os.path.join(out_dir, "rows.npy"), rows)
 
 
 def _phase(rank, t0, name):
@@ -413,7 +442,7 @@ def run_b200(args):
     if world != args.gpus:
         if world == 1 and args.gpus > 1:
             raise SystemExit("--gpus N>1 must be launched with torch.distributed.run (one rank per GPU)")
-    assert torch.cuda.is_available(), "bench.py needs a B200; the library has no CPU fallback"
+    assert torch.cuda.is_available(), "bench.py needs an H100; the library has no CPU fallback"
     torch.cuda.set_device(local)
     cpus_total = effective_cpus()          # before the NUMA pinning narrows the affinity mask
     numa = pin_to_gpu_numa(local)
@@ -476,11 +505,12 @@ def run_b200(args):
     sptr = stream.cuda_stream
     assert sptr != 0
     max_rows = args.tick * 4
+    torch.manual_seed(1234)   # the same inputs on every run with the same arguments (--dump-outputs comparisons)
     x_dev = torch.randn(max_rows, in_dim, device="cuda", dtype=torch.float32)
     y_dev = torch.empty(max_rows, out_dim, device="cuda", dtype=torch.float32)
     xb_dev = torch.empty(max_rows, in_dim, device="cuda", dtype=torch.float32)    # gathered batches (groups with forwarded rows)
     yb_dev = torch.empty(max_rows, out_dim, device="cuda", dtype=torch.float32)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -591,6 +621,8 @@ def run_b200(args):
     my_elapsed_ms, my_req = elapsed_ms, n_req
     launches = lib.tfsc_kernel_launches() - launches0
     st1 = srv.stats()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, plans[W + K - 1], x_dev, y_dev, xb_dev, yb_dev, out_dim)
 
     _phase(rank, t_start, "value region done")
     # ---- e2e: host buffers through the C ABI, closed-loop clients ----------------------------------------------
@@ -735,7 +767,7 @@ def run_b200(args):
     if "hbm_gbs" in peaks:
         peak, peak_src = peaks["hbm_gbs"], "MEASURED_PEAKS.json hbm_gbs (of measured)"
     else:
-        peak, peak_src = 6650.0, "B200_PROFILING.md fallback 6.65 TB/s (of fallback)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet 3.35 TB/s (not measured)"
     achieved = alg_bytes / (elapsed_ms * 1e-3) / 1e9  # this rank's dense launches are the whole timed region
     traffic = None
     tp = os.path.join(ROOT, "profiles", "dense_traffic.json")
@@ -759,7 +791,7 @@ def run_b200(args):
 
     roof = {"bound": "hbm", "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 4),
             "traffic": traffic,
-            "kernel": "dense_cluster_kernel<R> (<=8 rows, 2-CTA clusters, TMA ring, DSMEM K-fold, PDL) + dense_tc_kernel<RP> (9..64 rows, tcgen05 3xTF32, PDL): fused xW+b+ReLU",
+            "kernel": "dense_cluster_kernel<R> (<=8 rows, 2-CTA clusters, TMA ring, DSMEM K-fold, PDL) + dense_tc_kernel<RP> (9..64 rows, wgmma 3xTF32, PDL): fused xW+b+ReLU",
             "peak_source": peak_src, "launches_timed": int(n_dense), "avg_launch_us": round(elapsed_ms * 1e3 * world / max(1, n_dense), 2),
             "note": "per-GPU average algorithmic bytes / max-over-ranks device time; gather / scatter launches of forwarded rows are inside the timed region"}
     workload = workload_string(args.models_per_gpu, dims, wl["replicas"], wl["pick_policy"])
@@ -771,7 +803,7 @@ def run_b200(args):
             "ms_per_step": round(elapsed_ms / K, 3), "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f32", "data": "synthetic",
             "config": {"workload": workload,
-                       "models_total": wl["n_models"], "tick_requests_per_gpu": args.tick, "max_rows_per_pass": "8 (SIMT) / 64 (tcgen05 3xTF32)",
+                       "models_total": wl["n_models"], "tick_requests_per_gpu": args.tick, "max_rows_per_pass": "8 (SIMT) / 64 (wgmma 3xTF32)",
                        "l2": "inputs larger than L2 (>=1 GB of weights streamed per model pass); L2 flushed before timing",
                        "arena_gib": round(arena / 2**30, 1), "host_tier_gib": round(host_gib, 1), "cold_load_s": round(load_s, 1),
                        "preheat_s": args.preheat_s, "samplers": args.samplers, "cpu_affinity": numa},

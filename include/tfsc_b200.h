@@ -1,4 +1,4 @@
-/* tfsc_b200.h -- C ABI of libtfsc_b200.so, the B200-native replacement for the
+/* tfsc_b200.h -- C ABI of libtfsc_b200.so, the H100-native replacement for the
  * route -> ensure-resident -> predict path of mKaloer/TFServingCache.
  *
  * This is the drop-in boundary (SURVEY.md section 8b): plain C, plain pointers and sizes, no
@@ -12,7 +12,7 @@
  *     a too-small buffer yields TFSC_E_BUFFER.
  *   - buffers returned through `void**` are library-owned and released with tfsc_free().
  *   - there is NO CPU fallback: every compute entry fails with TFSC_E_NO_DEVICE when no
- *     sm_100-class device is usable.
+ *     sm_90 (H100) device is usable.
  */
 #ifndef TFSC_B200_H_
 #define TFSC_B200_H_
@@ -280,7 +280,7 @@ size_t tfsc_k_dense_workspace(int rows, int k, int n);
  * variant is bit-reproducible). */
 int tfsc_k_dense_variant(int variant, const float* x, const float* w, const float* b, float* y, int rows, int k, int n,
                          int relu, float* workspace, size_t workspace_bytes, void* stream);
-/* X3: the tcgen05/TMEM (3xTF32) path alone, rows <= 64, n % 32 == 0, k % 4 == 0. tfsc_k_dense picks it
+/* X3: the wgmma (3xTF32) path alone, rows <= 64, n % 32 == 0, k % 4 == 0. tfsc_k_dense picks it
  * automatically for more than 8 rows; this entry exists for parity tests and roofline timing. */
 int tfsc_k_dense_tc(const float* x, const float* w, const float* b, float* y, int rows, int k, int n, int relu,
                     float* workspace, size_t workspace_bytes, void* stream);
@@ -299,16 +299,16 @@ int tfsc_k_copy_segments(const tfsc_copy_seg* segs, int n, void* stream);
  * C[M,N] = act(A[M,K] (row stride lda) * B[K,N] + bias[N] (+ R[M,N])); bias / R may be NULL. */
 int tfsc_k_gemm(const float* a, const float* b, const float* bias, const float* r, float* c, int m, int n, int k, int lda,
                 int act, void* stream);
-/* the same GEMM on tcgen05 / TMEM (3xTF32, fp32-accurate): m >= 64, n >= 64, n % 32 == 0, k >= 32, lda % 4 == 0 */
+/* the same GEMM on the tensor cores (wgmma, 3xTF32, fp32-accurate): m >= 64, n >= 64, n % 32 == 0, k >= 32, lda % 4 == 0 */
 int tfsc_k_gemm_tc(const float* a, const float* b, const float* bias, const float* r, float* c, int m, int n, int k, int lda,
                    int act, void* stream);
-/* X4: implicit-GEMM convolution on tcgen05 / TMEM (3xTF32): y[B,OH,OW,cout] = act(conv2d(x[B,H,W,C] NHWC, w[KH,KW,C,cout] HWIO)
+/* X4: implicit-GEMM convolution on the tensor cores (wgmma, 3xTF32): y[B,OH,OW,cout] = act(conv2d(x[B,H,W,C] NHWC, w[KH,KW,C,cout] HWIO)
  * + bias (+ r)); the patch tiles are gathered from x by TMA im2col tensor maps, no patch matrix is materialised.
  * c % 32 == 0, cout >= 64 and % 32 == 0, batch*OH*OW >= 64. act: 0 none, 1 relu, 2 gelu, 3 tanh. */
 int tfsc_k_conv_tc(const float* x, const float* w, const float* bias, const float* r, float* y, int batch, int h, int wd, int c,
                    int kh, int kw, int stride, int pad, int cout, int act, void* stream);
-/* debugging aid: with TFSC_GT_TRACE=1 in the environment, 16 clock64 stamps of CTA 0 of the most recent persistent tcgen05
- * GEMM launch (entry, setup done, first TMA, first tile landed, converted, first MMA, per-tile commit / epilogue, exit) */
+/* debugging aid kept for ABI compatibility: the clock-trace timeline belonged to the persistent GEMM kernel, which the
+ * sm_90a build does not have; always returns TFSC_E_UNIMPLEMENTED and leaves out16 untouched */
 int tfsc_debug_gemm_trace(long long* out16);
 /* col[(b*OH+oh)*OW+ow][(kh*KW+kw)*C+c] patch matrix with row stride ldc >= KH*KW*C (zero padded) */
 int tfsc_k_im2col(const float* x, float* col, int batch, int h, int w, int c, int kh, int kw, int stride, int pad, int ldc,

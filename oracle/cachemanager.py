@@ -8,7 +8,7 @@ Follows:
   pkg/cachemanager/servingcontroller.go:29-54   ModelVersionStatus_State enum
   pkg/cachemanager/servingcontroller.go:159-187 createModelConfig (group by name, first seen)
 
-Tier mapping used by the B200 build (DESIGN.md): the reference's on-disk LRU
+Tier mapping used by the GPU build (DESIGN.md): the reference's on-disk LRU
 (``modelCache.size`` bytes) is the *pinned-host tier*; "loaded in TF-Serving"
 (``serving.maxConcurrentModels``) is the *HBM-resident tier*, additionally bounded by the HBM
 arena byte budget.  TF-Serving is restated as ``_Serving``: after a reload exactly the pushed

@@ -1,7 +1,7 @@
 """Numeric oracle for the executor the reference delegates to (TF-Serving, external and
 unpinned: deploy/docker-compose/docker-compose.yaml:22-37).  TEST INFRASTRUCTURE ONLY: nothing under
 tfservingcache_b200/ imports it.  numpy / torch-CPU restatement of the forward pass of each model
-template the B200 build executes, reading the same ``weights.bin`` blob + ``tfsc_model.json`` manifest
+template the GPU build executes, reading the same ``weights.bin`` blob + ``tfsc_model.json`` manifest
 the product pages into HBM (independent parse).
 
 Pin status: TF-Serving itself cannot run here or on the GPU box, so the only number that comes from it is

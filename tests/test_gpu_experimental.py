@@ -1,7 +1,6 @@
 """-m gpu: the dense-kernel variants and their programmatic-dependent-launch switch, each in its own process (TFSC_PDL /
-TFSC_DENSE_VARIANT are read once per process). Written at the end of round 1, validated on a B200 at the start of round 2
-(profiles/r2/dense_ab.jsonl): the cluster-pair kernel + PDL became the default for <= 8 rows; the other variants stay
-selectable for A/B runs, so they stay under test."""
+TFSC_DENSE_VARIANT are read once per process). The cluster-pair kernel + PDL is the default for <= 8 rows; the other
+variants stay selectable for A/B runs, so they stay under test."""
 import os
 import subprocess
 import sys

@@ -47,7 +47,7 @@ def test_k_gemm(m, n, k, lda, act):
                                         (1000, 3072, 768, 768), (512, 768, 3072, 3072), (6272, 128, 1152, 1152), (130, 96, 40, 44)])
 @pytest.mark.parametrize("act", [0, 1, 2, 3])
 def test_k_gemm_tc_matches_oracle(m, n, k, lda, act):
-    """tcgen05 / TMEM 3xTF32 GEMM (gemm_tc.cu) vs fp64; bias + residual + activation fused in the epilogue."""
+    """wgmma 3xTF32 GEMM (gemm_tc.cu) vs fp64; bias + residual + activation fused in the epilogue."""
     torch = _torch()
     rng = np.random.default_rng(m + n + k + act)
     a = rng.standard_normal((m, lda)).astype(np.float32)
@@ -105,7 +105,7 @@ def test_conv_as_im2col_gemm_matches_torch(h, c, kh, stride, pad, cout):
 @pytest.mark.parametrize("act,with_res", [(1, True), (0, False)])
 def test_implicit_gemm_conv_matches_torch(h, c, kh, stride, pad, cout, bsz, act, with_res):
     """X4: conv as implicit GEMM -- the A tiles come from TMA im2col tensor maps over the NHWC activations (padding = TMA
-    zero fill, stride = traversal stride), tcgen05 3xTF32, bias / residual / ReLU in the epilogue. vs torch conv2d fp64."""
+    zero fill, stride = traversal stride), wgmma 3xTF32, bias / residual / ReLU in the epilogue. vs torch conv2d fp64."""
     torch = _torch()
     rng = np.random.default_rng(h * 31 + c + kh + stride)
     x = rng.standard_normal((bsz, h, h, c)).astype(np.float32)

@@ -1,4 +1,4 @@
-"""-m gpu: X3, the tcgen05/TMEM 3xTF32 dense path (tfsc_k_dense_tc) vs the fp64 oracle; tolerance
+"""-m gpu: X3, the wgmma 3xTF32 dense path (tfsc_k_dense_tc) vs the fp64 oracle; tolerance
 1e-4 (north_star) although the split keeps it near 1e-5."""
 import ctypes as C
 

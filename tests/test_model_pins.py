@@ -1,7 +1,7 @@
 """Numeric parity pinned on INDEPENDENT implementations (VERDICT r1 'next' #1): torchvision's ResNet-50 and transformers'
 BERT-base define the two model families of BASELINE configs[1] / configs[3]; their own fp64 forward is the reference,
 their parameters are exported into the bundle format (tests/torch_export.py), and both the CPU oracle (here, not gpu) and
-the B200 executor (-m gpu) must reproduce it within north_star's 1e-4. Committed numbers: tests/golden/model_torch_golden.json
+the GPU executor (-m gpu) must reproduce it within north_star's 1e-4. Committed numbers: tests/golden/model_torch_golden.json
 (tests/golden/make_model_golden.py), required bit-for-bit-ish (1e-9) when the library versions match the recorded ones."""
 import os
 import sys
@@ -76,7 +76,7 @@ def test_oracle_matches_torchvision_and_transformers(name, golden):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["resnet_small", "resnet50", "bert_small", "bert_base"])
 def test_executor_matches_torchvision_and_transformers(name, golden, tmp_path):
-    """The B200 graph executor on bundles exported from the defining libraries, served from disk through the public
+    """The GPU graph executor on bundles exported from the defining libraries, served from disk through the public
     predict path (disk provider -> pinned host -> HBM arena -> kernels)."""
     import torch
     assert torch.cuda.is_available()

@@ -1,7 +1,7 @@
 """Independent numeric pins (test infrastructure): build the BASELINE configs[1] / configs[3] models with the
 libraries that DEFINE them -- torchvision.models.resnet50 and transformers.BertForSequenceClassification -- export
 their parameters into the product's bundle format, and let those libraries' own forward pass (fp64) be the reference.
-The oracle (oracle/models.py) and the B200 executor must both reproduce it within 1e-4, so a topology mistake shared by
+The oracle (oracle/models.py) and the GPU executor must both reproduce it within 1e-4, so a topology mistake shared by
 the oracle and the product manifests (same author) can no longer hide.
 
 TF-Serving itself (the reference's executor, deploy/docker-compose/docker-compose.yaml:22-37) is absent from this image and

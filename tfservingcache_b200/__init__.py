@@ -1,4 +1,4 @@
-"""tfservingcache_b200 -- B200-native route -> ensure-resident -> predict path with the API of
+"""tfservingcache_b200 -- H100-native route -> ensure-resident -> predict path with the API of
 mKaloer/TFServingCache.  The product is libtfsc_b200.so (C ABI: include/tfsc_b200.h); this
 package is the thin host-side mirror of the reference's Go interfaces over that ABI."""
 from . import _lib

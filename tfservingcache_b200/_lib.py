@@ -1,6 +1,6 @@
 """ctypes binding of libtfsc_b200.so (include/tfsc_b200.h).  There is no fallback: if the shared
 library is missing the import fails loudly, and every compute entry point returns
-TFSC_E_NO_DEVICE when no sm_100-class GPU is present."""
+TFSC_E_NO_DEVICE when no sm_90 GPU (H100) is present."""
 from __future__ import annotations
 
 import ctypes as C
@@ -12,7 +12,7 @@ LIB_PATH = os.path.join(_HERE, "libtfsc_b200.so")
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-        "or `make -C tfservingcache_b200/csrc` (nvcc, sm_100a). There is no CPU fallback.")
+        "or `make -C tfservingcache_b200/csrc` (nvcc, sm_90a). There is no CPU fallback.")
 
 lib = C.CDLL(LIB_PATH)
 

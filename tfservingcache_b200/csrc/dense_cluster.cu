@@ -1,6 +1,4 @@
 // X2, cluster-pair kernel of the fused dense pass: the DEFAULT for <= 8 rows per pass since round 2 (tfsc_k_dense_variant 0 / 5).
-// Measured on B200 (profiles/r2/dense_ab.jsonl, 300 back-to-back launches of one 9216x9216 layer, cold L2): 51.8 us at 8 rows,
-// 49.1 us at 1 row with programmatic dependent launch (55.5 / 53.2 us without) vs 61.1 / 54.1 us for dense_stream_kernel.
 //
 //   y[R,N] = act(x[R,K] W[K,N] + b),  R <= 8 rows per pass, fp32.
 //
@@ -14,7 +12,7 @@
 //     beyond N arrive as zeros), 4-stage mbarrier ring = 128 KB in flight per SM.
 //   * x: streamed too (a half of K does not fit beside the ring): chunks of 1024 k, R bulk copies each, double-buffered.
 //   * 16 consumer warps: lane = float4 column group of the strip, warp = k-lane (4 consecutive k rows of every stage,
-//     so one broadcast LDS.128 yields x[r][k..k+3]); packed FFMA2 accumulation; k-lane reduction through shared memory.
+//     so one broadcast LDS.128 yields x[r][k..k+3]); paired-column accumulation; k-lane reduction through shared memory.
 //   * programmatic dependent launch (TFSC_PDL=1): W streaming starts before griddepcontrol.wait, x after it.
 // Grid: 2 * ceil(N/128) CTAs (144 for N = 9216) in clusters of 2.
 #include <cuda.h>
@@ -59,9 +57,10 @@ __device__ __forceinline__ void cl_lds_2x64(uint32_t saddr, uint64_t& lo, uint64
   asm volatile("ld.shared.v2.b64 {%0,%1}, [%2];" : "=l"(lo), "=l"(hi) : "r"(saddr));
 }
 __device__ __forceinline__ void cl_ffma2(uint64_t& acc, float xs, uint64_t w2) {
-  uint64_t x2;
-  asm("mov.b64 %0, {%1, %1};" : "=l"(x2) : "f"(xs));
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(x2), "l"(w2));
+  float a0, a1, w0, w1;
+  asm("mov.b64 {%0, %1}, %2;" : "=f"(a0), "=f"(a1) : "l"(acc));
+  asm("mov.b64 {%0, %1}, %2;" : "=f"(w0), "=f"(w1) : "l"(w2));
+  asm("mov.b64 %0, {%1, %2};" : "=l"(acc) : "f"(fmaf(xs, w0, a0)), "f"(fmaf(xs, w1, a1)));
 }
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;

@@ -1,24 +1,21 @@
-// X3: tensor-core dense layer for batches of 9..64 rows, sm_100a only.
+// X3: tensor-core dense layer for batches of 9..64 rows, sm_90a (warpgroup MMA).
 //
 //   y[rows,N] = act(x[rows,K] W[K,N] + b),  fp32 in / fp32 out, |err| ~1e-6 (3xTF32 split)
 //
 // The weights are the big streamed operand (1 pass over W per launch, HBM-bound up to ~64 rows), so
 // W^T sits on the MMA "M" side: D[n, r] = sum_k W[k][n] x[r][k].
 //   * W tiles arrive by TMA (cp.async.bulk.tensor.3d over a 3-D tensor map {32 n, K, N/32}, boxes of 4 rows x
-//     8 slabs = 4 x 1 KB contiguous) into a 6-stage ring: 192 KB of W in flight per SM.
-//   * 8 converter warps move each tile into TMEM as the MMA "A" operand (lane = output column, column = k):
-//     W_hi = the raw fp32 bits (kind::tf32 ignores the low 13 mantissa bits) and W_lo = W - trunc_tf32(W)
-//     (tcgen05.st), and build B' = [x_hi ; x_lo] (K-major, SWIZZLE_128B) in shared memory from x.
-//     (An MN-major tf32 A operand read straight from shared memory -- layout SWIZZLE_128B_BASE32B, the only one
-//     UMMA accepts for it -- was measured at ~185 clk per MMA on B200; the TMEM path costs ~60.)
-//   * per 8-wide k step and 128-column tile: MMA1 D[:, 0:2R] += W_hi . [x_hi;x_lo]^T (N = 2R),
-//     MMA2 D[:, R:2R] += W_lo . x_hi^T (N = R); accumulators live in TMEM; y = D[:, :R] + D[:, R:2R]: the large
-//     term and the small correction terms are kept apart because the tensor core's fp32 accumulation truncates.
+//     8 slabs = 4 x 1 KB contiguous, SWIZZLE_128B) into a 6-stage ring: 192 KB of W in flight per SM.
+//   * 4 consumer warpgroups own 64 output columns each. A tf32 operand in shared memory must be K-major and W is
+//     N-major, so each warp reads its W fragments from the stage into registers (the wgmma A operand may come from
+//     registers in any layout): W_hi = trunc_tf32(W) and W_lo = W - W_hi. All consumers together build
+//     B' = [x_hi ; x_lo] (K-major, SWIZZLE_128B) in shared memory from x (double-buffered, one named barrier per k-block).
+//   * per 8-wide k step: acc_h += W_hi . x_hi, acc_s += W_hi . x_lo + W_lo . x_hi (N = rows padded to RP);
+//     y = acc_h + acc_s: the large term and the small correction terms are kept apart because the tensor core's fp32
+//     accumulation truncates.
 //   * split-K over CTAs (one CTA per SM), partials folded by the last CTA of a strip in fixed order
-//     (same deterministic scheme as dense_stream_kernel), bias + ReLU fused there. (A thread-block cluster per strip
-//     with a DSMEM fold, as in dense_cluster.cu, does not fit: 36 strips x 4 K-splits would need 36 clusters of 4 and
-//     B200 co-schedules at most 33 of them -- 132 of 148 SMs -- so the grid would take a second wave.)
-//   * programmatic dependent launch (round 2): the W ring fills (TMA) under the previous kernel's tail; x, the
+//     (same deterministic scheme as dense_stream_kernel), bias + ReLU fused there.
+//   * programmatic dependent launch: the W ring fills (TMA) under the previous kernel's tail; x, the
 //     split-K workspace and y are touched only after griddepcontrol.wait.
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -36,32 +33,20 @@ namespace tfsc {
 extern std::atomic<int64_t> g_launches_tc;
 std::atomic<int64_t> g_launches_tc{0};
 
-// Optional timeline trace of CTA (0,0) (debug builds only: -DTFSC_TC_TRACE): clock64 stamps per k-block
-#ifdef TFSC_TC_TRACE
-__device__ long long g_tc_trace[8][128];
-#define TC_TRACE(slot, kb) do { if (blockIdx.x == 0 && blockIdx.y == 0 && (kb) < 128) g_tc_trace[slot][kb] = clock64(); } while (0)
-#else
-#define TC_TRACE(slot, kb) do {} while (0)
-#endif
-
 namespace tc {
 constexpr int BK = 32;                     // k rows per stage = one 128-byte swizzle row of tf32
-constexpr int TILE_M = 128;                // output columns per MMA
-constexpr int TILES = 2;                   // MMA tiles per CTA
-constexpr int STRIP = TILE_M * TILES;      // 256 output columns per CTA
+constexpr int WG_COLS = 64;                // output columns per consumer warpgroup (wgmma M)
+constexpr int CONS_WG = 4;
+constexpr int STRIP = WG_COLS * CONS_WG;   // 256 output columns per CTA
 constexpr int SLABS = STRIP / 32;          // 8 slabs of 32 columns
-constexpr int SLAB_BYTES = BK * 128;       // 4 KB
-constexpr int W_BYTES = SLABS * SLAB_BYTES;  // 32 KB per stage
-constexpr int NUM_CONV_WARPS = 8;
-constexpr int THREADS = 64 + NUM_CONV_WARPS * 32;  // warp0 TMA, warp1 MMA, warps 2..9 convert + epilogue
+constexpr int W_BYTES = SLABS * BK * 128;  // 32 KB per stage
+constexpr int CONSUMERS = CONS_WG * 128;
+constexpr int CONS_WARPS = CONSUMERS / 32;
+constexpr int THREADS = CONSUMERS + 32;    // warps 0..15 consumers, warp 16 TMA producer
 }  // namespace tc
 
-// smem (dynamic, 1024-aligned): NS stages of W (32 KB each, TMA target, read by MMA1 and by the
-// converters), 2 buffers of B' = [x_hi ; x_lo] (2*RP rows x 128 B), then the mbarriers.
-// TMEM (512 columns): D tile t at columns [t*2RP, (t+1)*2RP): [0,RP) = W_hi.x_hi (main accumulator),
-// [RP,2RP) = W_hi.x_lo + W_lo.x_hi (small terms kept apart from the big one: the tensor core's fp32
-// accumulation truncates, so small terms must not be added into the large running sum);
-// A-operand buffers (W_hi raw bits | W_lo) at columns [256 + cb*128 + t*64, +64), cb = k-block parity.
+// smem (dynamic, 1024-aligned): NS stages of W (32 KB each, TMA target, layout [k/4][slab][k%4][32 n] with the
+// 128-byte swizzle), 2 buffers of B' = [x_hi ; x_lo] (2*RP rows x 128 B), then the mbarriers.
 template <int RP>
 struct TcSmem {
   static constexpr int NS = 6;
@@ -69,7 +54,6 @@ struct TcSmem {
   static constexpr int W_TOTAL = NS * tc::W_BYTES;
   static constexpr int TOTAL = W_TOTAL + 2 * B_BYTES + 256 + 1024;
 };
-constexpr uint32_t kAopCol = 256;  // A-operand staging: [cb][tile][hi 32 | lo 32] columns
 
 template <int RP>
 __global__ void __launch_bounds__(tc::THREADS, 1)
@@ -83,50 +67,34 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap wmap, const float* __restric
   uint8_t* bprime = smem + S::W_TOTAL;
   uint64_t* bars = reinterpret_cast<uint64_t*>(bprime + 2 * S::B_BYTES);
   uint64_t* full = bars;             // [NS] TMA landed the W stage
-  uint64_t* empty = bars + NS;       // [NS] MMAs finished reading the W stage
-  uint64_t* cfull = bars + 2 * NS;   // [2]  converters published B'[cb] and W_lo[cb]
-  uint64_t* cempty = cfull + 2;      // [2]  MMAs finished reading B'[cb] / W_lo[cb]
-  uint64_t* accum_full = cempty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_full + 1);
+  uint64_t* empty = bars + NS;       // [NS] every consumer warp holds its W fragments of the stage in registers
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // role from a broadcast warpgroup index: ptxas then knows the branch below is warpgroup-uniform and does not serialise
+  // the wgmma instructions behind compiler-inserted warpgroup barriers
+  const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
   const int strip = blockIdx.x, split = blockIdx.y;
   const int k_begin = split * chunk_k;
   const int k_end = min(K, k_begin + chunk_k);
   const int n_kblocks = (max(0, k_end - k_begin) + tc::BK - 1) / tc::BK;
-  constexpr int TMEM_COLS = 512;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int s = 0; s < NS; ++s) {
-        mbar_init(&full[s], 1);
-        mbar_init(&empty[s], tc::NUM_CONV_WARPS);  // the converters are the only readers of a W stage
-      }
-      for (int c = 0; c < 2; ++c) {
-        mbar_init(&cfull[c], tc::NUM_CONV_WARPS);
-        mbar_init(&cempty[c], 1);
-      }
-      mbar_init(accum_full, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < NS; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], tc::CONS_WARPS);
     }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // no-op without the PDL launch attribute
 
-  if (warp == 0) {
+  if (wg == tc::CONS_WG) {
     // ===================== TMA producer: keeps NS x 32 KB of W in flight =====================
     for (int kb = 0; kb < n_kblocks; ++kb) {
       const int s = kb % NS, it = kb / NS;
       if (lane == 0) {
         if (it > 0) mbar_wait(&empty[s], (it - 1) & 1);
-        TC_TRACE(0, kb);
         mbar_expect_tx(&full[s], tc::W_BYTES);
         // 8 boxes of {32 n, 4 k, 8 slabs}: every box covers 4 W rows x 1 KB contiguous, so the 128-byte
         // pieces of one DRAM row are requested close together; smem stage = [k/4][slab][k%4][32 n]
@@ -136,51 +104,17 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap wmap, const float* __restric
       }
       __syncwarp();
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc1 = make_idesc_ts(2 * RP);  // W_hi (TMEM) x [x_hi ; x_lo]
-    constexpr uint32_t idesc2 = make_idesc_ts(RP);      // W_lo (TMEM) x  x_hi
-    for (int kb = 0; kb < n_kblocks; ++kb) {
-      const int cb = kb & 1, cit = kb >> 1;
-      if (lane == 0) {
-        mbar_wait(&cfull[cb], cit & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        TC_TRACE(1, kb);
-        const uint32_t bp = smem_u32(bprime + cb * S::B_BYTES);
-#pragma unroll
-        for (int t = 0; t < tc::TILES; ++t) {
-          const uint32_t d = tmem_base + (uint32_t)(t * 2 * RP);
-          const uint32_t ahi = tmem_base + kAopCol + (uint32_t)(cb * 128 + t * 64);
-          const uint32_t alo = ahi + 32;
-#pragma unroll
-          for (int k8 = 0; k8 < tc::BK / 8; ++k8) {
-            // both A operands come from TMEM (an MN-major tf32 A operand read from shared memory costs ~185 clk
-            // per MMA on B200; the TMEM path does not). B' (K-major, SWIZZLE_128B): 8-row groups at SBO = 1 KB,
-            // k advances 32 B inside the swizzle row.
-            const uint64_t b = make_desc(bp + k8 * 32, 16, 1024, 2);
-            umma_tf32_ts(d, ahi + k8 * 8, b, idesc1, (kb | k8) ? 1u : 0u);
-            umma_tf32_ts(d + RP, alo + k8 * 8, b, idesc2, 1u);
-          }
-        }
-        umma_commit(&cempty[cb]);
-        TC_TRACE(2, kb);
-      }
-      __syncwarp();
-    }
-    if (lane == 0) umma_commit(accum_full);
-    __syncwarp();
   } else {
-    // ===================== converters: B' = [x_hi ; x_lo] (smem) and W_lo (TMEM) =====================
-    const int ct = threadIdx.x - 64;  // 0..255
-    const int q = warp & 3;           // TMEM lane quarter this warp may access
-    const int t = (warp - 2) >> 2;    // tile 0 for warps 2..5, tile 1 for warps 6..9
-    constexpr int XI = (RP * 8 + 255) / 256;  // x items (float4) per thread per k-block
-    float4 xr[2][XI];                         // register ring: x is fetched two k-blocks ahead (L2 latency)
+    // ===================== consumers: B' = [x_hi ; x_lo] (smem), W fragments (registers), wgmma =====================
+    const int ct = threadIdx.x;       // 0..511
+    const int wq = warp & 3, g = lane >> 2, t = lane & 3;
+    constexpr int XI = (RP * 8 + tc::CONSUMERS - 1) / tc::CONSUMERS;  // x items (float4) per thread per k-block
+    float4 xr[2][XI];                                                // register ring: x is fetched two k-blocks ahead
     auto load_x = [&](int kb, float4* dst) {
       const int k0 = k_begin + kb * tc::BK;
 #pragma unroll
       for (int j = 0; j < XI; ++j) {
-        const int idx = ct + j * 256;
+        const int idx = ct + j * tc::CONSUMERS;
         const int r = idx >> 3, c = idx & 7;
         float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
         const int kk = k0 + c * 4;
@@ -199,18 +133,23 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap wmap, const float* __restric
     asm volatile("griddepcontrol.wait;" ::: "memory");   // x is the previous kernel's output; W (TMA warp) never is
     if (n_kblocks > 0) load_x(0, xr[0]);
     if (n_kblocks > 1) load_x(1, xr[1]);
-    // shared address of this thread's column inside a W stage, before the per-row swizzle
-    const uint32_t w_col_base = smem_u32(smem) + (uint32_t)((t * 4 + q) * 512 + (lane & 7) * 4);
+    // this thread's A fragment columns: n0 = wg*64 + wq*16 + g and n0 + 8 (same 32-column slab), k % 4 == t always.
+    // Offset inside a 4-row k group of a stage: row = slab*4 + t (128 B), 16-byte chunk XOR (row % 8).
+    const int n0 = wg * tc::WG_COLS + wq * 16 + g, slab = n0 >> 5, row = slab * 4 + t;
+    auto w_off = [&](int n) { return (uint32_t)(row * 128 + ((((n & 31) >> 2) ^ (row & 7)) << 4) + (n & 3) * 4); };
+    const uint32_t w_base = smem_u32(smem);
+    const uint32_t off0 = w_off(n0), off1 = w_off(n0 + 8);
     const uint32_t bp_base = smem_u32(bprime);
+    float acc_h[RP / 2], acc_s[RP / 2];
+#pragma unroll
+    for (int i = 0; i < RP / 2; ++i) acc_h[i] = acc_s[i] = 0.f;
     auto body = [&](int kb, float4* xcur) {
-      const int s = kb % NS, it = kb / NS, cb = kb & 1, cit = kb >> 1;
-      if (ct == 0) TC_TRACE(3, kb);
-      if (cit > 0) mbar_wait(&cempty[cb], (cit - 1) & 1);
-      if (ct == 0) TC_TRACE(4, kb);
+      const int s = kb % NS, it = kb / NS, cb = kb & 1;
+      // B'[cb] was last read by the MMAs of k-block kb-2, which every consumer waited for before the barrier of kb-1
       const uint32_t bp = bp_base + cb * S::B_BYTES;
 #pragma unroll
       for (int j = 0; j < XI; ++j) {
-        const int idx = ct + j * 256;
+        const int idx = ct + j * tc::CONSUMERS;
         if (idx < RP * 8) {
           const int r = idx >> 3, c = idx & 7, rl = r + RP;
           const float4 v = xcur[j];
@@ -220,62 +159,58 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap wmap, const float* __restric
         }
       }
       if (kb + 2 < n_kblocks) load_x(kb + 2, xcur);
-      // W_lo[m][k] = W[k][m] - trunc_tf32(W[k][m]) -> TMEM (lane = output column m, column = k)
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // B' writes -> visible to the MMA (async proxy)
+      named_bar_sync(1, tc::CONSUMERS);
       mbar_wait(&full[s], it & 1);
-      if (ct == 0) TC_TRACE(5, kb);
-      const uint32_t wst = w_col_base + (uint32_t)(s * tc::W_BYTES);
-      uint32_t hi[32], lo[32];
+      const uint32_t wst = w_base + (uint32_t)(s * tc::W_BYTES);
+      uint32_t hi[tc::BK / 8][4], lo[tc::BK / 8][4];
 #pragma unroll
-      for (int k = 0; k < 32; ++k) {
-        const float v = lds_f32(wst + (k >> 2) * 4096 + (k & 3) * 128 + ((((lane >> 3) ^ (k & 3))) << 5));
-        hi[k] = __float_as_uint(v);  // kind::tf32 ignores the low 13 mantissa bits: W_hi = trunc_tf32(W)
-        lo[k] = __float_as_uint(tf32_lo(v));
-      }
+      for (int k8 = 0; k8 < tc::BK / 8; ++k8)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {   // a[j]: column n0 + 8*(j&1), k = 8*k8 + t + 4*(j>>1)
+          const float v = lds_f32(wst + (uint32_t)((k8 * 2 + (j >> 1)) * 4096) + ((j & 1) ? off1 : off0));
+          hi[k8][j] = tf32_hi_bits(v);
+          lo[k8][j] = __float_as_uint(tf32_lo(v));
+        }
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty[s]);  // this warp is done with the W stage: TMA may refill it
-      const uint32_t aop = tmem_base + ((uint32_t)(q * 32) << 16) + kAopCol + (uint32_t)(cb * 128 + t * 64);
-      tmem_st32(aop, hi);
-      tmem_st32(aop + 32, lo);
-      asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // B' writes -> visible to the MMA (async proxy)
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (ct == 0) TC_TRACE(6, kb);
-      if (lane == 0) mbar_arrive(&cfull[cb]);
+      if constexpr (RP <= 32) {   // fragments final before the warpgroup fence; at 48 / 64 rows it costs spills instead
+        fence_regs(hi);
+        fence_regs(lo);
+      }
+      fence_regs(acc_h);
+      fence_regs(acc_s);
+      wgmma_fence();
+#pragma unroll
+      for (int k8 = 0; k8 < tc::BK / 8; ++k8) {
+        const uint64_t bh = gmma_desc_sw128(bp + k8 * 32), bl = gmma_desc_sw128(bp + RP * 128 + k8 * 32);
+        wgmma_tf32_rs<RP>(acc_h, hi[k8], bh);
+        wgmma_tf32_rs<RP>(acc_s, hi[k8], bl);
+        wgmma_tf32_rs<RP>(acc_s, lo[k8], bh);
+      }
+      wgmma_commit();
+      wgmma_wait_all();
+      fence_regs(acc_h);
+      fence_regs(acc_s);
     };
     for (int kb = 0; kb < n_kblocks; kb += 2) {
       body(kb, xr[0]);
       if (kb + 1 < n_kblocks) body(kb + 1, xr[1]);
     }
-    // ===================== epilogue: TMEM -> split-K partials =====================
-    mbar_wait(accum_full, 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int ncol = t * tc::TILE_M + q * 32 + lane;  // column within the strip
+    // ===================== epilogue: accumulators -> split-K partials =====================
     float* my_partial = partials + ((size_t)(strip * splits + split) * RP) * tc::STRIP;
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(t * 2 * RP);
-    if (n_kblocks > 0) {
 #pragma unroll
-      for (int c = 0; c < RP; c += 16) {
-        float hi[16], sm[16];
-        tmem_ld16(taddr + c, hi);
-        tmem_ld16(taddr + RP + c, sm);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) my_partial[(size_t)(c + i) * tc::STRIP + ncol] = hi[i] + sm[i];
-      }
-    } else {
-      for (int r = 0; r < RP; ++r) my_partial[(size_t)r * tc::STRIP + ncol] = 0.f;
+    for (int i = 0; i < RP / 2; ++i) {
+      const int ncol = n0 + 8 * ((i >> 1) & 1), r = 8 * (i >> 2) + 2 * t + (i & 1);
+      my_partial[(size_t)r * tc::STRIP + ncol] = acc_h[i] + acc_s[i];
     }
   }
 
-  // ---- teardown + deterministic split-K fold by the last CTA of the strip ----
+  // ---- deterministic split-K fold by the last CTA of the strip ----
   __shared__ unsigned int s_last;
   asm volatile("griddepcontrol.wait;" ::: "memory");   // workspace counters / y: every thread observes the prerequisite grid
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __threadfence();
   __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
-  }
   if (threadIdx.x == 0) {
     const unsigned int prev = atomicAdd(&counters[strip], 1u);
     s_last = (prev == (unsigned)splits - 1) ? 1u : 0u;
@@ -339,7 +274,7 @@ static bool get_wmap(const float* w, int k, int n, CUtensorMap* out) {
   const cuuint32_t box[3] = {32, 4, (cuuint32_t)tc::SLABS};
   const cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = enc(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(w), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return false;
   if (cache.size() > 4096) cache.clear();
@@ -348,19 +283,13 @@ static bool get_wmap(const float* w, int k, int n, CUtensorMap* out) {
   return true;
 }
 
-#ifdef TFSC_TC_TRACE
-extern "C" int tfsc_tc_trace_read(long long* out) {
-  return cudaMemcpyFromSymbol(out, g_tc_trace, sizeof(long long) * 8 * 128) == cudaSuccess ? 0 : -1;
-}
-#endif
-
 struct TcPlan {
   int strips, splits, chunk_k;
 };
 static TcPlan plan_tc(int k, int n) {
   TcPlan p;
   p.strips = (n + tc::STRIP - 1) / tc::STRIP;
-  int splits = 148 / p.strips;
+  int splits = device_sm_count() / p.strips;
   if (splits < 1) splits = 1;
   int max_splits = (k + 4 * tc::BK - 1) / (4 * tc::BK);  // keep >= 4 k-blocks per CTA
   if (splits > max_splits) splits = max_splits;

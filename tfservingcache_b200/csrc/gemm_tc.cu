@@ -1,25 +1,27 @@
-// tcgen05 GEMM for the graph executor (conv-as-GEMM, transformer dense layers), sm_100a only:
+// Warpgroup-MMA GEMM for the graph executor (conv-as-GEMM, transformer dense layers), sm_90a:
 //
 //   C[M,N] = act(A[M,K] * B[K,N] + bias[N] (+ R[M,N])),  fp32 in / out, 3xTF32 split (fp32-accurate)
 //
-// Round 2: both MMA operands come from shared memory (SS mode) and the A tile can be gathered by the TMA unit itself.
 //   * A (activations) is K-major: TMA lands the tile [128 m][32 k] (SWIZZLE_128B) either from a row-major matrix (2-D tiled
 //     map: dense layers, 1x1 stride-1 convs) or -- IMPLICIT GEMM, no im2col buffer -- straight from the NHWC activation
 //     tensor with an im2col tensor map (cuTensorMapEncodeIm2col): the 128 rows are 128 consecutive output pixels, the 32
 //     columns are 32 channels of one filter tap (kh, kw); padding arrives as zeros, strided convs through the map's
-//     traversal stride. The raw fp32 bits are A_hi (kind::tf32 ignores the low 13 mantissa bits).
-//   * B (weights [K,N] row-major) is MN-major: TMA 3-D map {32 n, K, N/32} -> SWIZZLE_128B_ATOM_32B slabs.
-//   * 8 converter warps write A_lo = A - trunc_tf32(A) and B_lo = B - trunc_tf32(B) next to the TMA tiles, elementwise at
-//     the same (swizzled) offsets, so no layout knowledge is needed: B' = [B_hi | B_lo] is one operand of N = 2*BN.
-//     (Round 1 moved A through TMEM with tcgen05.st; the A-from-TMEM read costs ~64 clk per MMA and needed a second
-//     barrier pair.)
-//   * per 8-wide k step: MMA1 D[:, 0:2BN] += A_hi . B'  (hh | hl), MMA2 D[:, BN:2BN] += A_lo . B_hi (lh): the large term
-//     and the small corrections have separate TMEM accumulators (the tensor core's fp32 accumulate truncates).
-//   * epilogue: tcgen05.ld, C = hh + small + bias (+ residual), ReLU / GELU(erf) / tanh, row-contiguous stores.
+//     traversal stride. The raw fp32 bits are A_hi (the tensor core ignores the low 13 mantissa bits); the consumers write
+//     A_lo = A - trunc_tf32(A) next to it, elementwise at the same (swizzled) offsets.
+//   * B (weights [K,N] row-major) is N-major, which a tf32 wgmma operand in shared memory cannot be. So the MMA computes
+//     the transposed tile, C^T = B^T A^T: B^T is the register ("A") operand -- each warp reads its fragments from the TMA
+//     tile (3-D map {32 n, K, N/32}, SWIZZLE_128B slabs) and splits them into B_hi / B_lo -- and the activation tile is the
+//     shared-memory ("B") operand, K-major as it lands.
+//   * per 8-wide k step: acc_h += B_hi . A_hi, acc_s += B_hi . A_lo + B_lo . A_hi: the large term and the small corrections
+//     have separate accumulators (the tensor core's fp32 accumulate truncates).
+//   * two consumer warpgroups: for BN = 128 each owns 64 columns x 128 rows (wgmma N = 128), for BN = 64 each owns the 64
+//     columns x 64 rows. The epilogue parks the tile in shared memory and stores it row-contiguous with bias (+ residual)
+//     and ReLU / GELU(erf) / tanh.
 // One CTA per 128 x BN output tile; small grids (late ResNet stages: M = 392, K = 4608; BERT's K = 3072 projection) split K
 // over a thread-block cluster of 2 / 4 / 8 CTAs along grid.z: every CTA parks its partial tile in its own shared memory
 // and each CTA folds 128/S rows of the tile over distributed shared memory in fixed rank order (deterministic), then
-// applies bias / residual / activation. warp 0 TMA producer, warp 1 MMA issuer, warps 2..9 converters + epilogue.
+// applies bias / residual / activation. Warpgroups 0..1 consumers, warpgroup 2 producer (warp 8 issues the TMA); the producer
+// warpgroup hands its registers to the consumers with setmaxnreg.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -39,7 +41,12 @@ extern std::atomic<int64_t> g_launches_nn;
 namespace gt {
 constexpr int BM = 128, BK = 32;
 constexpr int A_BYTES = BM * BK * 4;  // 16 KB per A tile (hi or lo)
-constexpr int THREADS = 320;
+constexpr int CONSUMERS = 256;        // two warpgroups
+constexpr int CONS_WARPS = CONSUMERS / 32;
+constexpr int THREADS = CONSUMERS + 128;   // + a producer warpgroup (warp 8 issues the TMA)
+// register split (setmaxnreg): each 16K register-file quarter holds one producer warp and two consumer warps:
+// 40 + 2 * 232 = 504 registers per lane (the BN = 128 accumulators alone take 128)
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 }  // namespace gt
 
 // geometry of an implicit-GEMM conv (A tile = TMA im2col gather from the NHWC activations)
@@ -49,24 +56,16 @@ struct ConvGeom {
 
 template <int BN>
 struct GtSmem {
-  static constexpr int STAGES = BN == 128 ? 3 : 4;
+  static constexpr int STAGES = 4;
   static constexpr int SLABS = BN / 32;                 // 32-column slabs of the B tile
-  static constexpr int KG_BYTES = 2 * SLABS * 512;      // one 4-row k group: hi slabs then lo slabs, 512 B each
-  static constexpr int B_BYTES = (gt::BK / 4) * KG_BYTES;  // 8 k groups: 2*BN*32*4 bytes
-  static constexpr int STAGE_BYTES = 2 * gt::A_BYTES + B_BYTES;   // A_hi | A_lo | B'
+  static constexpr int KG_BYTES = SLABS * 512;          // one 4-row k group of B: [slab][k%4][32 n]
+  static constexpr int B_BYTES = (gt::BK / 4) * KG_BYTES;
+  static constexpr int STAGE_BYTES = 2 * gt::A_BYTES + B_BYTES;   // A_hi | A_lo | B
   static constexpr int TOTAL = STAGES * STAGE_BYTES + 256 + 1024;
-  static constexpr int TOTAL_PERSIST = TOTAL + 4 * 32 * 36 * 4;   // + the epilogue's transpose staging (4 warps x 32 rows x 36 floats)
-  static constexpr int TMEM_COLS = 2 * BN;              // D: [0, BN) main, [BN, 2BN) corrections (power of two >= 32)
+  static constexpr int WM = BN == 128 ? 128 : 64;       // tile rows per consumer warpgroup (wgmma N)
+  static_assert(gt::BM * (BN + 4) * 4 <= STAGES * STAGE_BYTES, "the parked tile overlays the stages");
 };
 
-__device__ __forceinline__ void umma_tf32_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(0u), "r"(0u), "r"(0u), "r"(0u)
-      : "memory");
-}
 // TMA im2col gather: coordinates {c, w, h, n} of the base pixel (input space), offsets {kw, kh} of the filter tap
 __device__ __forceinline__ void tma_load_im2col_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c, int w, int h, int n,
                                                    uint16_t woff, uint16_t hoff) {
@@ -78,11 +77,6 @@ __device__ __forceinline__ void tma_load_im2col_4d(void* dst, const CUtensorMap*
 }
 
 __device__ __forceinline__ float gelu_erf_tc(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f)); }
-// activation selected at COMPILE time inside the store loops: with a run-time `act` the compiler if-converts the chain and
-// every element pays for erff and tanhf (~200 instructions per float4) whatever the activation is -- the timeline showed the
-// epilogue store phase at ~300 clk per 512-byte store because of it
-template <int ACT>
-__device__ __forceinline__ float4 apply_act(float4 v);
 // run-time activation with REAL branches (noinline bodies cannot be if-converted into the caller's store loop)
 __device__ __noinline__ float4 act_gelu4(float4 v) { return make_float4(gelu_erf_tc(v.x), gelu_erf_tc(v.y), gelu_erf_tc(v.z), gelu_erf_tc(v.w)); }
 __device__ __noinline__ float4 act_tanh4(float4 v) { return make_float4(tanhf(v.x), tanhf(v.y), tanhf(v.z), tanhf(v.w)); }
@@ -92,31 +86,22 @@ __device__ __forceinline__ float4 apply_act_rt(float4 v, int act) {
   if (act == 3) return act_tanh4(v);
   return v;
 }
-template <int ACT>
-__device__ __forceinline__ float4 apply_act(float4 v) {
-  if (ACT == 1) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
-  else if (ACT == 2) { v.x = gelu_erf_tc(v.x); v.y = gelu_erf_tc(v.y); v.z = gelu_erf_tc(v.z); v.w = gelu_erf_tc(v.w); }
-  else if (ACT == 3) { v.x = tanhf(v.x); v.y = tanhf(v.y); v.z = tanhf(v.z); v.w = tanhf(v.w); }
-  return v;
-}
-
 template <int BN, bool IM2COL>
 __global__ void __launch_bounds__(gt::THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
                const float* __restrict__ bias, const float* __restrict__ R, float* __restrict__ C, int M, int N, int K, int act,
                ConvGeom cg) {
   using S = GtSmem<BN>;
-  constexpr int NS = S::STAGES;
+  constexpr int NS = S::STAGES, WM = S::WM;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NS * S::STAGE_BYTES);
-  uint64_t* full = bars;            // [NS] TMA landed A_hi and B_hi
-  uint64_t* conv = bars + NS;       // [NS] converters published A_lo and B_lo
-  uint64_t* empty = bars + 2 * NS;  // [NS] MMAs finished reading the stage
-  uint64_t* accum_full = bars + 3 * NS;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_full + 1);
+  uint64_t* full = bars;            // [NS] TMA landed A_hi and B
+  uint64_t* empty = bars + NS;      // [NS] every consumer warp's MMAs on the stage have completed
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // role from a broadcast warpgroup index: the consumer branch is then provably warpgroup-uniform for ptxas
+  const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
   const int m0 = blockIdx.y * gt::BM, n0 = blockIdx.x * BN;
   // split-K: grid.z = cluster size S; this CTA (cluster rank = blockIdx.z) takes k blocks [kb0, kb0 + n_kblocks)
   const int splits = (int)gridDim.z, split = (int)blockIdx.z;
@@ -124,36 +109,26 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
   const int per_split = (total_kblocks + splits - 1) / splits;
   const int kb0 = split * per_split;
   const int n_kblocks = max(0, min(total_kblocks, kb0 + per_split) - kb0);
-  constexpr int TMEM_COLS = S::TMEM_COLS;
-  constexpr int PSTRIDE = BN + 4;   // partial tile [128][BN + 4] fp32 (padded: conflict-free float4 stores, one row per lane)
+  constexpr int PSTRIDE = BN + 4;   // parked tile [128][BN + 4] fp32 (padded: conflict-free fragment stores)
 
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int s = 0; s < NS; ++s) {
-        mbar_init(&full[s], 1);
-        mbar_init(&conv[s], 8);
-        mbar_init(&empty[s], 1);
-      }
-      mbar_init(accum_full, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&amap) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&bmap) : "memory");
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < NS; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], gt::CONS_WARPS);
     }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&amap) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&bmap) : "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  // programmatic dependent launch: successors may begin their setup; this kernel (split-K path, few CTAs) simply waits for its
-  // predecessor here -- its own setup above already ran under the predecessor's tail
+  // programmatic dependent launch: successors may begin their setup; this kernel waits for its predecessor here -- its
+  // own setup above already ran under the predecessor's tail
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   asm volatile("griddepcontrol.wait;" ::: "memory");
 
-  if (warp == 0) {
+  if (wg == gt::CONSUMERS / 128) {
     // ===================== TMA producer =====================
+    regs_release<gt::PRODUCER_REGS>();
     int pn = 0, ph = 0, pw = 0;  // im2col: base pixel of the tile's first row, input space
     if (IM2COL) {
       const int per_img = cg.OH * cg.OW;
@@ -162,6 +137,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
       ph = (rem / cg.OW) * cg.stride - cg.pad;
       pw = (rem % cg.OW) * cg.stride - cg.pad;
     }
+    if (warp == gt::CONS_WARPS)
     for (int kb = 0; kb < n_kblocks; ++kb) {
       const int s = kb % NS, it = kb / NS;
       if (lane == 0) {
@@ -176,126 +152,96 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
           tma_load_2d(stage, &amap, &full[s], (kb0 + kb) * gt::BK, m0);  // A: [128 m][32 k], 128 B rows, SW128
         }
 #pragma unroll
-        for (int g = 0; g < gt::BK / 4; ++g)                              // B_hi: k group g -> slabs [0, SLABS) of the group
+        for (int g = 0; g < gt::BK / 4; ++g)                              // B: k group g -> slabs [0, SLABS) of the group
           tma_load_3d(stage + 2 * gt::A_BYTES + g * S::KG_BYTES, &bmap, &full[s], 0, (kb0 + kb) * gt::BK + g * 4, n0 / 32);
       }
       __syncwarp();
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc1 = make_idesc_ts_b(2 * BN, 1);  // A_hi (K-major smem) x [B_hi | B_lo] (MN-major)
-    constexpr uint32_t idesc2 = make_idesc_ts_b(BN, 1);      // A_lo x B_hi
-    for (int kb = 0; kb < n_kblocks; ++kb) {
-      const int s = kb % NS, it = kb / NS;
-      if (lane == 0) {
-        mbar_wait(&conv[s], it & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t ahi = smem_u32(smem + s * S::STAGE_BYTES);
-        const uint32_t alo = ahi + gt::A_BYTES;
-        const uint32_t bsm = ahi + 2 * gt::A_BYTES;
-#pragma unroll
-        for (int k8 = 0; k8 < gt::BK / 8; ++k8) {
-          // A (K-major, SWIZZLE_128B): 8-row groups SBO = 1 KB apart, k advances 32 B inside the swizzle row.
-          // B' (MN-major tf32, SWIZZLE_128B_BASE32B): atoms of 4 k rows x 128 B; slabs LBO = 512 B apart, consecutive
-          // 4-row k groups SBO = KG_BYTES apart; one MMA (K = 8) spans two k groups
-          const uint64_t b = make_desc(bsm + k8 * 2 * S::KG_BYTES, 512, S::KG_BYTES, 1);
-          umma_tf32_ss(tmem_base, make_desc(ahi + k8 * 32, 16, 1024, 2), b, idesc1, (kb | k8) ? 1u : 0u);
-          umma_tf32_ss(tmem_base + BN, make_desc(alo + k8 * 32, 16, 1024, 2), b, idesc2, 1u);
-        }
-        umma_commit(&empty[s]);
-      }
-      __syncwarp();
-    }
-    if (lane == 0 && n_kblocks > 0) umma_commit(accum_full);
-    __syncwarp();
   } else {
-    const int ct = threadIdx.x - 64;   // 0..255
-    const int q = warp & 3;            // TMEM lane quarter of this warp
-    // ===================== converters (warps 2..9): X_lo = X - trunc_tf32(X), elementwise at the same offsets =========
+    // ===================== consumers: A_lo, B fragments, wgmma =====================
+    regs_acquire<gt::CONSUMER_REGS>();
+    const int ct = threadIdx.x;  // 0..255
+    const int wq = warp & 3, g = lane >> 2, t = lane & 3;
+    const int n_off = BN == 128 ? wg * 64 : 0, m_off = BN == 128 ? 0 : wg * 64;
+    // this thread's B^T fragment columns n and n + 8 (same 32-column slab); k % 4 == t always
+    const int nf = n_off + wq * 16 + g, row = (nf >> 5) * 4 + t;
+    auto b_off = [&](int n) { return (uint32_t)(row * 128 + ((((n & 31) >> 2) ^ (row & 7)) << 4) + (n & 3) * 4); };
+    const uint32_t off0 = b_off(nf), off1 = b_off(nf + 8);
+    float acc_h[WM / 2], acc_s[WM / 2];
+#pragma unroll
+    for (int i = 0; i < WM / 2; ++i) acc_h[i] = acc_s[i] = 0.f;
     for (int kb = 0; kb < n_kblocks; ++kb) {
       const int s = kb % NS, it = kb / NS;
-      mbar_wait(&full[s], it & 1);     // the stage itself is free: the producer waited on empty[s] before refilling
+      mbar_wait(&full[s], it & 1);
       const uint32_t ast = smem_u32(smem + s * S::STAGE_BYTES);
 #pragma unroll
-      for (int i = 0; i < gt::A_BYTES / 16 / 256; ++i) {          // A tile: 1024 float4, 4 per thread
-        const uint32_t src = ast + (uint32_t)((ct + i * 256) * 16);
+      for (int i = 0; i < gt::A_BYTES / 16 / gt::CONSUMERS; ++i) {   // A tile: 1024 float4, 4 per thread
+        const uint32_t src = ast + (uint32_t)((ct + i * gt::CONSUMERS) * 16);
         const float4 v = lds_f4(src);
         sts_f4(src + gt::A_BYTES, make_float4(tf32_lo(v.x), tf32_lo(v.y), tf32_lo(v.z), tf32_lo(v.w)));
       }
-      const uint32_t bsm = ast + 2 * gt::A_BYTES;
-      // hi part of k group g: bytes [g*KG, g*KG + SLABS*512); lo part right behind it
-      constexpr int F4_PER_GROUP = S::SLABS * 512 / 16;
-      for (int idx = ct; idx < (gt::BK / 4) * F4_PER_GROUP; idx += 256) {
-        const int g = idx / F4_PER_GROUP, o = idx - g * F4_PER_GROUP;
-        const uint32_t src = bsm + (uint32_t)(g * S::KG_BYTES + o * 16);
-        const float4 v = lds_f4(src);
-        sts_f4(src + S::SLABS * 512, make_float4(tf32_lo(v.x), tf32_lo(v.y), tf32_lo(v.z), tf32_lo(v.w)));
-      }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the MMA (async proxy)
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&conv[s]);
-    }
-    // ===================== epilogue: all 8 warps, 4 lane quarters x 2 column halves =====================
-    if (n_kblocks > 0) {
-      mbar_wait(accum_full, 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
-    const int half = (warp - 2) >> 2;                  // warps 2..5 -> columns [0, BN/2), warps 6..9 -> [BN/2, BN)
-    const int gm = m0 + q * 32 + lane;
-    const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-    float* part = reinterpret_cast<float*>(smem) + (size_t)(q * 32 + lane) * PSTRIDE;   // split-K: this thread's row of the partial
+      const uint32_t bsm = ast + 2 * gt::A_BYTES;
+      uint32_t hi[gt::BK / 8][4], lo[gt::BK / 8][4];
 #pragma unroll
-    for (int c = half * (BN / 2); c < (half + 1) * (BN / 2); c += 16) {
-      float hh[16], sm[16];
-      if (n_kblocks > 0) {
-        tmem_ld16(taddr + c, hh);
-        tmem_ld16(taddr + BN + c, sm);
-      } else {
+      for (int k8 = 0; k8 < gt::BK / 8; ++k8)
 #pragma unroll
-        for (int j = 0; j < 16; ++j) hh[j] = sm[j] = 0.f;
-      }
-      if (splits > 1) {
-        // every MMA of this CTA has completed (accum_full), so the stages are idle: the partial tile overlays them
-#pragma unroll
-        for (int j = 0; j < 16; j += 4)
-          *reinterpret_cast<float4*>(part + c + j) = make_float4(hh[j] + sm[j], hh[j + 1] + sm[j + 1], hh[j + 2] + sm[j + 2], hh[j + 3] + sm[j + 3]);
-      } else if (gm < M) {
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          const int gn = n0 + c + j;
-          if (gn >= N) continue;
-          float4 v = make_float4(hh[j] + sm[j], hh[j + 1] + sm[j + 1], hh[j + 2] + sm[j + 2], hh[j + 3] + sm[j + 3]);
-          if (bias) {
-            const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + gn));
-            v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w;
-          }
-          if (R) {
-            const float4 rv = __ldg(reinterpret_cast<const float4*>(R + (size_t)gm * N + gn));
-            v.x += rv.x; v.y += rv.y; v.z += rv.z; v.w += rv.w;
-          }
-          v = apply_act_rt(v, act);
-          *reinterpret_cast<float4*>(C + (size_t)gm * N + gn) = v;
+        for (int j = 0; j < 4; ++j) {   // a[j]: column nf + 8*(j&1), k = 8*k8 + t + 4*(j>>1)
+          const float v = lds_f32(bsm + (uint32_t)((k8 * 2 + (j >> 1)) * S::KG_BYTES) + ((j & 1) ? off1 : off0));
+          hi[k8][j] = tf32_hi_bits(v);
+          lo[k8][j] = __float_as_uint(tf32_lo(v));
         }
+      named_bar_sync(1, gt::CONSUMERS);   // every consumer has written its share of A_lo
+      fence_regs(hi);   // fragments and accumulators are final before the warpgroup fence
+      fence_regs(lo);
+      fence_regs(acc_h);
+      fence_regs(acc_s);
+      wgmma_fence();
+      const uint32_t ahi = ast + (uint32_t)(m_off * 128), alo = ahi + gt::A_BYTES;
+#pragma unroll
+      for (int k8 = 0; k8 < gt::BK / 8; ++k8) {
+        const uint64_t dh = gmma_desc_sw128(ahi + k8 * 32), dl = gmma_desc_sw128(alo + k8 * 32);
+        wgmma_tf32_rs<WM>(acc_h, hi[k8], dh);
+        wgmma_tf32_rs<WM>(acc_s, hi[k8], dl);
+        wgmma_tf32_rs<WM>(acc_s, lo[k8], dh);
       }
+      wgmma_commit();
+      wgmma_wait_all();
+      fence_regs(acc_h);
+      fence_regs(acc_s);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);
+    }
+    // ===================== park the tile: every MMA of this CTA has completed, the stages are idle =====================
+    named_bar_sync(1, gt::CONSUMERS);
+    float* part = reinterpret_cast<float*>(smem);
+#pragma unroll
+    for (int i = 0; i < WM / 2; ++i) {
+      const int n = nf + 8 * ((i >> 1) & 1), m = m_off + 8 * (i >> 2) + 2 * t + (i & 1);
+      part[m * PSTRIDE + n] = acc_h[i] + acc_s[i];
     }
   }
 
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
+  // ---- the K slices meet in distributed shared memory: rank r folds rows [r*128/S, (r+1)*128/S) of the tile ----
   if (splits > 1) {
-    // ---- the K slices meet in distributed shared memory: rank r folds rows [r*128/S, (r+1)*128/S) of the tile ----
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");      // every CTA of the cluster parked its partial
-    const int rows_per = gt::BM / splits;
-    const uint32_t part_s = smem_u32(smem);
-    constexpr int V4 = BN / 4;
-    for (int idx = threadIdx.x; idx < rows_per * V4; idx += gt::THREADS) {
-      const int r = split * rows_per + idx / V4, c = (idx % V4) * 4;
-      const int gm = m0 + r, gn = n0 + c;
-      if (gm >= M || gn >= N) continue;
-      const uint32_t off = part_s + (uint32_t)((r * PSTRIDE + c) * 4);
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+  } else {
+    __syncthreads();
+  }
+  const int rows_per = gt::BM / splits;
+  const uint32_t part_s = smem_u32(smem);
+  constexpr int V4 = BN / 4;
+  for (int idx = threadIdx.x; idx < rows_per * V4; idx += gt::THREADS) {
+    const int r = split * rows_per + idx / V4, c = (idx % V4) * 4;
+    const int gm = m0 + r, gn = n0 + c;
+    if (gm >= M || gn >= N) continue;
+    const uint32_t off = part_s + (uint32_t)((r * PSTRIDE + c) * 4);
+    float4 v;
+    if (splits == 1) {
+      v = lds_f4(off);
+    } else {
+      v = make_float4(0.f, 0.f, 0.f, 0.f);
       for (int s2 = 0; s2 < splits; ++s2) {                                   // fixed rank order: bit-reproducible
         uint32_t raddr;
         asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(off), "r"((uint32_t)s2));
@@ -303,303 +249,22 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__
         asm volatile("ld.shared::cluster.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(t.x), "=f"(t.y), "=f"(t.z), "=f"(t.w) : "r"(raddr) : "memory");
         v.x += t.x; v.y += t.y; v.z += t.z; v.w += t.w;
       }
-      if (bias) {
-        const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + gn));
-        v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w;
-      }
-      if (R) {
-        const float4 rv = __ldg(reinterpret_cast<const float4*>(R + (size_t)gm * N + gn));
-        v.x += rv.x; v.y += rv.y; v.z += rv.z; v.w += rv.w;
-      }
-      v = apply_act_rt(v, act);
-      *reinterpret_cast<float4*>(C + (size_t)gm * N + gn) = v;
     }
+    if (bias) {
+      const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + gn));
+      v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w;
+    }
+    if (R) {
+      const float4 rv = __ldg(reinterpret_cast<const float4*>(R + (size_t)gm * N + gn));
+      v.x += rv.x; v.y += rv.y; v.z += rv.z; v.w += rv.w;
+    }
+    v = apply_act_rt(v, act);
+    *reinterpret_cast<float4*>(C + (size_t)gm * N + gn) = v;
+  }
+  if (splits > 1) {
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");      // peers may still be reading this CTA's partial
   }
-}
-
-// ------------------------------------------------------------------------------- persistent variant ----
-// One CTA per SM walks the output tiles (tile = blockIdx.x + i * gridDim.x). Against the kernel above it pays the TMEM
-// allocation, barrier setup and descriptor prefetch once, keeps the TMA ring full across tile boundaries, and overlaps the
-// epilogue of tile i (4 dedicated warps, tcgen05.ld -> bias / residual / activation -> global) with the main loop of tile
-// i+1 through two TMEM accumulators. The graph models are made of many small GEMMs (ResNet-50: 53 convs, K = 64..4608): with
-// one tile per CTA the fixed per-tile cost (~6 us) was several times the MMA time of the small-K layers.
-// Roles: warp 0 TMA producer, warp 1 MMA issuer, warps 2..9 converters (A_lo / B_lo), warps 10..13 epilogue.
-namespace gt {
-constexpr int P_THREADS = 64 + 256 + 128;
-}
-
-#define GT_TRACE(slot) do { if (trace && blockIdx.x == 0) trace[slot] = clock64(); } while (0)
-// epilogue of one tile for one epilogue warp (persistent kernel): TMEM -> staging rows -> coalesced stores, see the kernel
-template <int BN, int ACT>
-__device__ __forceinline__ void persist_epilogue_tile(uint32_t taddr, uint32_t stg_s, const float* __restrict__ bias,
-                                                      const float* __restrict__ R, float* __restrict__ C, int M, int N, int m0, int n0,
-                                                      int q, int lane, int prow, int pcol, long long* __restrict__ trace, int i, int warp) {
-  constexpr int EST = 36;
-      // bias of every chunk up front: its L2 latency must not sit between the TMEM loads and the stores of a chunk
-      float4 bvs[BN / 32];
-#pragma unroll
-      for (int cc = 0; cc < BN / 32; ++cc) {
-        const int gnb = n0 + cc * 32 + pcol;
-        bvs[cc] = (bias && gnb < N) ? __ldg(reinterpret_cast<const float4*>(bias + gnb)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-#pragma unroll
-      for (int cc = 0; cc < BN / 32; ++cc) {
-        const int c = cc * 32;
-        const int gn = n0 + c + pcol;
-        const float4 bv = bvs[cc];
-        {
-          uint32_t hh[32], sm[32];
-          tmem_ld32_nowait(taddr + c, hh);            // both loads in flight, one wait
-          tmem_ld32_nowait(taddr + BN + c, sm);
-          tmem_wait_ld();
-          if (i == 0 && cc == 0 && warp == 10 && lane == 0) GT_TRACE(13);
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            sts_f4(stg_s + (uint32_t)((lane * EST + j) * 4),
-                   make_float4(__uint_as_float(hh[j]) + __uint_as_float(sm[j]), __uint_as_float(hh[j + 1]) + __uint_as_float(sm[j + 1]),
-                               __uint_as_float(hh[j + 2]) + __uint_as_float(sm[j + 2]), __uint_as_float(hh[j + 3]) + __uint_as_float(sm[j + 3])));
-        }
-        __syncwarp();
-        if (i == 0 && cc == 0 && warp == 10 && lane == 0) GT_TRACE(14);
-#pragma unroll
-        for (int r4 = 0; r4 < 32; r4 += 4) {
-          const int row = r4 + prow, gm = m0 + q * 32 + row;
-          float4 v = lds_f4(stg_s + (uint32_t)((row * EST + pcol) * 4));
-          if (gm < M && gn < N) {
-            v.x += bv.x; v.y += bv.y; v.z += bv.z; v.w += bv.w;
-            if (R) {
-              const float4 rv = __ldg(reinterpret_cast<const float4*>(R + (size_t)gm * N + gn));
-              v.x += rv.x; v.y += rv.y; v.z += rv.z; v.w += rv.w;
-            }
-            v = apply_act<ACT>(v);
-            *reinterpret_cast<float4*>(C + (size_t)gm * N + gn) = v;
-          }
-        }
-        __syncwarp();   // the staging rows are rewritten by the next chunk
-        if (i == 0 && cc == 0 && warp == 10 && lane == 0) GT_TRACE(15);
-      }
-}
-
-// optional timeline of CTA 0 (TFSC_GT_TRACE=1: the launcher passes a device buffer, tfsc_debug_gemm_trace reads it back)
-
-template <int BN, bool IM2COL>
-__global__ void __launch_bounds__(gt::P_THREADS, 1)
-gemm_tc_persist_kernel(const __grid_constant__ CUtensorMap amap, const __grid_constant__ CUtensorMap bmap,
-                       const float* __restrict__ bias, const float* __restrict__ R, float* __restrict__ C, int M, int N, int K,
-                       int act, ConvGeom cg, int tiles_n, int tiles_total, long long* __restrict__ trace) {
-  using S = GtSmem<BN>;
-  constexpr int NS = S::STAGES;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NS * S::STAGE_BYTES);
-  uint64_t* full = bars;                 // [NS] TMA landed A_hi and B_hi
-  uint64_t* conv = bars + NS;            // [NS] converters published A_lo and B_lo
-  uint64_t* empty = bars + 2 * NS;       // [NS] MMAs finished reading the stage
-  uint64_t* accum_full = bars + 3 * NS;  // [2]  all MMAs of a tile have completed into accumulator ab
-  uint64_t* accum_empty = accum_full + 2;  // [2] the epilogue has read accumulator ab
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_empty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_kblocks = (K + gt::BK - 1) / gt::BK;
-  constexpr int TMEM_COLS = 4 * BN;      // two accumulators of 2*BN columns (512 for BN = 128: the whole TMEM)
-  if (threadIdx.x == 0) GT_TRACE(0);
-
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int s = 0; s < NS; ++s) {
-        mbar_init(&full[s], 1);
-        mbar_init(&conv[s], 8);
-        mbar_init(&empty[s], 1);
-      }
-      for (int a = 0; a < 2; ++a) {
-        mbar_init(&accum_full[a], 1);
-        mbar_init(&accum_empty[a], 4);
-      }
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&amap) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(&bmap) : "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  if (threadIdx.x == 0) GT_TRACE(1);
-  // programmatic dependent launch: the next kernel of the stream may start its own setup / weight prefetch on SMs this grid
-  // has left; everything that depends on the PREVIOUS kernel (A tiles, residual, C) is touched only after griddepcontrol.wait
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-
-  if (warp == 0) {
-    // ===================== TMA producer: the ring does not drain at tile boundaries =====================
-    int g = 0;  // k blocks issued so far by this CTA (all tiles)
-    bool waited = false;
-    for (int tile = blockIdx.x; tile < tiles_total; tile += gridDim.x) {
-      const int m0 = (tile / tiles_n) * gt::BM, n0 = (tile % tiles_n) * BN;
-      int pn = 0, ph = 0, pw = 0;
-      if (IM2COL) {
-        const int per_img = cg.OH * cg.OW;
-        pn = m0 / per_img;
-        const int rem = m0 - pn * per_img;
-        ph = (rem / cg.OW) * cg.stride - cg.pad;
-        pw = (rem % cg.OW) * cg.stride - cg.pad;
-      }
-      auto load_a = [&](int kb, int s) {
-        uint8_t* stage = smem + s * S::STAGE_BYTES;
-        if (IM2COL) {
-          const int k0 = kb * gt::BK, tap = k0 / cg.C, c0 = k0 - tap * cg.C;
-          tma_load_im2col_4d(stage, &amap, &full[s], c0, pw, ph, pn, (uint16_t)(tap % cg.KW), (uint16_t)(tap / cg.KW));
-        } else {
-          tma_load_2d(stage, &amap, &full[s], kb * gt::BK, m0);
-        }
-      };
-      auto load_b = [&](int kb, int s) {
-        uint8_t* stage = smem + s * S::STAGE_BYTES;
-#pragma unroll
-        for (int gq = 0; gq < gt::BK / 4; ++gq)
-          tma_load_3d(stage + 2 * gt::A_BYTES + gq * S::KG_BYTES, &bmap, &full[s], 0, kb * gt::BK + gq * 4, n0 / 32);
-      };
-      int kb = 0;
-      if (!waited) {
-        // first stages of the first tile: the WEIGHT tiles never depend on the previous kernel -> in flight before the wait
-        const int pre = n_kblocks < NS ? n_kblocks : NS;
-        if (lane == 0) {
-          GT_TRACE(2);
-          for (int p = 0; p < pre; ++p) {
-            mbar_expect_tx(&full[p], gt::A_BYTES + BN * gt::BK * 4);
-            load_b(p, p);
-          }
-        }
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-        if (lane == 0)
-          for (int p = 0; p < pre; ++p) load_a(p, p);
-        __syncwarp();
-        waited = true;
-        kb = pre;
-        g = pre;
-      }
-      for (; kb < n_kblocks; ++kb, ++g) {
-        const int s = g % NS, it = g / NS;
-        if (lane == 0) {
-          if (it > 0) mbar_wait(&empty[s], (it - 1) & 1);
-          mbar_expect_tx(&full[s], gt::A_BYTES + BN * gt::BK * 4);
-          load_a(kb, s);
-          load_b(kb, s);
-        }
-        __syncwarp();
-      }
-    }
-    if (!waited) asm volatile("griddepcontrol.wait;" ::: "memory");
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc1 = make_idesc_ts_b(2 * BN, 1);
-    constexpr uint32_t idesc2 = make_idesc_ts_b(BN, 1);
-    int g = 0, i = 0;
-    for (int tile = blockIdx.x; tile < tiles_total; tile += gridDim.x, ++i) {
-      const int ab = i & 1, n = i >> 1;
-      const uint32_t dacc = tmem_base + (uint32_t)(ab * 2 * BN);
-      if (lane == 0 && n > 0) {
-        mbar_wait(&accum_empty[ab], (n - 1) & 1);   // the epilogue drained this accumulator (tile i - 2)
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      }
-      for (int kb = 0; kb < n_kblocks; ++kb, ++g) {
-        const int s = g % NS, it = g / NS;
-        if (lane == 0) {
-          mbar_wait(&conv[s], it & 1);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          if (g == 0) GT_TRACE(5);
-          const uint32_t ahi = smem_u32(smem + s * S::STAGE_BYTES);
-          const uint32_t alo = ahi + gt::A_BYTES;
-          const uint32_t bsm = ahi + 2 * gt::A_BYTES;
-#pragma unroll
-          for (int k8 = 0; k8 < gt::BK / 8; ++k8) {
-            const uint64_t b = make_desc(bsm + k8 * 2 * S::KG_BYTES, 512, S::KG_BYTES, 1);
-            umma_tf32_ss(dacc, make_desc(ahi + k8 * 32, 16, 1024, 2), b, idesc1, (kb | k8) ? 1u : 0u);
-            umma_tf32_ss(dacc + BN, make_desc(alo + k8 * 32, 16, 1024, 2), b, idesc2, 1u);
-          }
-          umma_commit(&empty[s]);
-        }
-        __syncwarp();
-      }
-      if (lane == 0) {
-        umma_commit(&accum_full[ab]);
-        if (i < 2) GT_TRACE(6 + 3 * i);
-      }
-      __syncwarp();
-    }
-  } else if (warp < 10) {
-    // ===================== converters (warps 2..9) =====================
-    const int ct = threadIdx.x - 64;   // 0..255
-    int g = 0;
-    for (int tile = blockIdx.x; tile < tiles_total; tile += gridDim.x) {
-      for (int kb = 0; kb < n_kblocks; ++kb, ++g) {
-        const int s = g % NS, it = g / NS;
-        mbar_wait(&full[s], it & 1);
-        if (g == 0 && ct == 0) GT_TRACE(3);
-        const uint32_t ast = smem_u32(smem + s * S::STAGE_BYTES);
-#pragma unroll
-        for (int j = 0; j < gt::A_BYTES / 16 / 256; ++j) {
-          const uint32_t src = ast + (uint32_t)((ct + j * 256) * 16);
-          const float4 v = lds_f4(src);
-          sts_f4(src + gt::A_BYTES, make_float4(tf32_lo(v.x), tf32_lo(v.y), tf32_lo(v.z), tf32_lo(v.w)));
-        }
-        const uint32_t bsm = ast + 2 * gt::A_BYTES;
-        constexpr int F4_PER_GROUP = S::SLABS * 512 / 16;
-        for (int idx = ct; idx < (gt::BK / 4) * F4_PER_GROUP; idx += 256) {
-          const int gq = idx / F4_PER_GROUP, o = idx - gq * F4_PER_GROUP;
-          const uint32_t src = bsm + (uint32_t)(gq * S::KG_BYTES + o * 16);
-          const float4 v = lds_f4(src);
-          sts_f4(src + S::SLABS * 512, make_float4(tf32_lo(v.x), tf32_lo(v.y), tf32_lo(v.z), tf32_lo(v.w)));
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&conv[s]);
-        if (g == 0 && ct == 0) GT_TRACE(4);
-      }
-    }
-  } else {
-    // ===================== epilogue (warps 10..13), TMEM lane quarter = warp % 4 =====================
-    // A thread owns one accumulator row in TMEM, but 16-byte stores from 32 different rows are 32 half-filled sectors and
-    // the per-row bias / residual loads sat on the critical path (timeline: 7.7k clk per 128 x 64 tile against a 2.6k clk
-    // main loop). So the tile is transposed through shared memory in 32-column chunks: phase A thread = row (tcgen05.ld ->
-    // padded staging rows, conflict-free float4 stores), phase B 8 lanes = one 128-byte row segment (bias / residual /
-    // activation, full-sector coalesced loads and stores). A warp only ever reads back the 32 rows it staged itself.
-    asm volatile("griddepcontrol.wait;" ::: "memory");   // C / R may be buffers the previous kernel of the stream still uses
-    const int q = warp & 3;
-    constexpr int EST = 36;                                       // staging row stride in floats (32 + 4 pad)
-    float* stg = reinterpret_cast<float*>(smem + NS * S::STAGE_BYTES + 256) + (size_t)(warp - 10) * 32 * EST;
-    const uint32_t stg_s = smem_u32(stg);
-    const int prow = lane >> 3, pcol = (lane & 7) * 4;            // phase B: row within a group of 4, column within the chunk
-    int i = 0;
-    for (int tile = blockIdx.x; tile < tiles_total; tile += gridDim.x, ++i) {
-      const int ab = i & 1, n = i >> 1;
-      const int m0 = (tile / tiles_n) * gt::BM, n0 = (tile % tiles_n) * BN;
-      mbar_wait(&accum_full[ab], n & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (i < 2 && warp == 10 && lane == 0) GT_TRACE(7 + 3 * i);
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(ab * 2 * BN);
-      switch (act) {   // uniform: one instantiation of the tile epilogue per activation
-        case 1: persist_epilogue_tile<BN, 1>(taddr, stg_s, bias, R, C, M, N, m0, n0, q, lane, prow, pcol, trace, i, warp); break;
-        case 2: persist_epilogue_tile<BN, 2>(taddr, stg_s, bias, R, C, M, N, m0, n0, q, lane, prow, pcol, trace, i, warp); break;
-        case 3: persist_epilogue_tile<BN, 3>(taddr, stg_s, bias, R, C, M, N, m0, n0, q, lane, prow, pcol, trace, i, warp); break;
-        default: persist_epilogue_tile<BN, 0>(taddr, stg_s, bias, R, C, M, N, m0, n0, q, lane, prow, pcol, trace, i, warp); break;
-      }
-      // the accumulator may be overwritten once every epilogue warp has pulled its rows out of TMEM
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&accum_empty[ab]);
-      if (i < 2 && warp == 10 && lane == 0) GT_TRACE(8 + 3 * i);
-    }
-  }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
-  if (threadIdx.x == 0) GT_TRACE(12);
 }
 
 // --------------------------------------------------------------------------------- host side ----
@@ -638,21 +303,6 @@ bool gemm_tc_supported(const float* A, const float* B, const float* bias, const 
          (!bias || al16(bias)) && (!R || al16(R)) && tc_encode_fn() != nullptr;
 }
 
-static long long* gt_trace_buffer() {  // TFSC_GT_TRACE=1: 16 clock64 stamps of CTA 0 of the most recent persistent launch
-  static long long* buf = [] {
-    const char* e = getenv("TFSC_GT_TRACE");
-    long long* p = nullptr;
-    if (e && atoi(e) != 0 && cudaMalloc(&p, 16 * sizeof(long long)) == cudaSuccess) cudaMemset(p, 0, 16 * sizeof(long long));
-    return p;
-  }();
-  return buf;
-}
-int gemm_trace_read(long long* out16) {
-  long long* p = gt_trace_buffer();
-  if (!p) return -1;
-  return cudaMemcpy(out16, p, 16 * sizeof(long long), cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
-}
-
 template <int BN, bool IM2COL>
 static cudaError_t launch_gt(const CUtensorMap& am, const CUtensorMap& bm, const float* bias, const float* R, float* C, int M,
                              int N, int K, int act, const ConvGeom& cg, cudaStream_t s) {
@@ -666,9 +316,10 @@ static cudaError_t launch_gt(const CUtensorMap& am, const CUtensorMap& bm, const
   }
   const int tiles = ((N + BN - 1) / BN) * ((M + gt::BM - 1) / gt::BM);
   const int kblocks = (K + gt::BK - 1) / gt::BK;
-  // split-K over a cluster when the tile grid alone leaves most of the 148 SMs idle and K is long enough to share
+  // split-K over a cluster when the tile grid alone leaves most of the SMs idle and K is long enough to share
+  const int sms = device_sm_count();
   int splits = 1;
-  while (splits < 8 && tiles * splits * 2 <= 148 && kblocks / (splits * 2) >= 6) splits *= 2;
+  while (splits < 8 && tiles * splits * 2 <= sms && kblocks / (splits * 2) >= 6) splits *= 2;
   static const int force = [] {
     const char* e = getenv("TFSC_GEMM_SPLITK");   // 0 = never split (A/B), 2 / 4 / 8 = force where K allows
     return e ? atoi(e) : -1;
@@ -677,40 +328,6 @@ static cudaError_t launch_gt(const CUtensorMap& am, const CUtensorMap& bm, const
   else if (force > 0) {
     splits = 1;
     while (splits < force && splits < 8 && kblocks / (splits * 2) >= 1) splits *= 2;
-  }
-  static const bool persist = [] {
-    const char* e = getenv("TFSC_GEMM_PERSIST");   // 0 = one tile per CTA (the non-persistent kernel), for A/B runs
-    return !e || atoi(e) != 0;
-  }();
-  if (splits == 1 && persist) {
-    static bool pattr[64] = {};
-    static int sms[64] = {};
-    if (!pattr[dev & 63]) {
-      cudaError_t e = cudaFuncSetAttribute(gemm_tc_persist_kernel<BN, IM2COL>, cudaFuncAttributeMaxDynamicSharedMemorySize, GtSmem<BN>::TOTAL_PERSIST);
-      if (e != cudaSuccess) return e;
-      if (cudaDeviceGetAttribute(&sms[dev & 63], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms[dev & 63] <= 0) sms[dev & 63] = 148;
-      pattr[dev & 63] = true;
-    }
-    const int tiles_n = (N + BN - 1) / BN;
-    const int grid = tiles < sms[dev & 63] ? tiles : sms[dev & 63];
-    static const bool pdl = [] {
-      const char* e = getenv("TFSC_PDL");
-      return !e || atoi(e) != 0;
-    }();
-    cudaLaunchConfig_t pc = {};
-    pc.gridDim = dim3(grid);
-    pc.blockDim = dim3(gt::P_THREADS);
-    pc.dynamicSmemBytes = GtSmem<BN>::TOTAL_PERSIST;
-    pc.stream = s;
-    cudaLaunchAttribute pa[1];
-    pa[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    pa[0].val.programmaticStreamSerializationAllowed = 1;
-    pc.attrs = pa;
-    pc.numAttrs = pdl ? 1 : 0;
-    cudaError_t pe = cudaLaunchKernelEx(&pc, gemm_tc_persist_kernel<BN, IM2COL>, am, bm, bias, R, C, M, N, K, act, cg, tiles_n, tiles,
-                                        gt_trace_buffer());
-    g_launches_nn++;
-    return pe != cudaSuccess ? pe : cudaGetLastError();
   }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((N + BN - 1) / BN, (M + gt::BM - 1) / gt::BM, splits);
@@ -726,11 +343,11 @@ static cudaError_t launch_gt(const CUtensorMap& am, const CUtensorMap& bm, const
     at[na].val.clusterDim.z = splits;
     ++na;
   }
-  static const bool pdl2 = [] {
+  static const bool pdl = [] {   // programmatic dependent launch is on unless TFSC_PDL=0
     const char* e = getenv("TFSC_PDL");
     return !e || atoi(e) != 0;
   }();
-  if (pdl2) {
+  if (pdl) {
     at[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[na].val.programmaticStreamSerializationAllowed = 1;
     ++na;
@@ -744,7 +361,7 @@ static cudaError_t launch_gt(const CUtensorMap& am, const CUtensorMap& bm, const
 
 static int pick_bn(int M, int N) {
   if (N % 128 != 0 && N <= 128) return 64;
-  // small problems: 128 x 64 tiles double the CTA count (BERT's N = 768 projections: 48 -> 96 CTAs on 148 SMs)
+  // small problems: 128 x 64 tiles double the CTA count (BERT's N = 768 projections: 48 -> 96 CTAs on 132 SMs)
   const long tiles128 = (long)((N + 127) / 128) * ((M + gt::BM - 1) / gt::BM);
   return tiles128 < 120 && N % 64 == 0 ? 64 : 128;
 }
@@ -757,7 +374,7 @@ static bool weight_map(const float* B, int K, int N, int BN, CUtensorMap* bm) {
     const cuuint32_t box[3] = {32, 4, (cuuint32_t)(BN / 32)};
     const cuuint32_t estr[3] = {1, 1, 1};
     return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(B), gdim, gstride, box, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
   }, bm);
 }

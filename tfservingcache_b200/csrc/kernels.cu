@@ -1,4 +1,4 @@
-// Executor kernels for sm_100a (B200). fp32 SIMT: the per-tenant models of the Zipf mix are run
+// Executor kernels for sm_90a (H100). fp32 SIMT: the per-tenant models of the Zipf mix are run
 // at batch <= 8 rows per pass, where y = xW + b is bound by streaming W from HBM once
 // (intensity rows/2 FLOP/B, far below the fp32 ridge) -- so the design goal is HBM-rate
 // streaming: 128-bit coalesced loads, >= 64 KB in flight per SM, one CTA per SM-sized grid,
@@ -17,6 +17,18 @@ extern std::atomic<int64_t> g_launches_tc;
 extern std::atomic<int64_t> g_launches_nn;
 extern std::atomic<int64_t> g_launches_cl;
 int64_t kernel_launch_count() { return g_launches.load() + g_launches_tc.load() + g_launches_nn.load() + g_launches_cl.load(); }
+
+int device_sm_count() {
+  static std::atomic<int> cache[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  int n = cache[dev & 63].load();
+  if (n <= 0) {
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+    cache[dev & 63].store(n);
+  }
+  return n;
+}
 
 // ------------------------------------------------------------------------------------ X1 ----
 __global__ void __launch_bounds__(256) affine_kernel(const float* __restrict__ x, float* __restrict__ y, int64_t n,
@@ -44,7 +56,7 @@ cudaError_t launch_affine(const float* x, float* y, int64_t n, const float* a, c
   if (n <= 0) return cudaSuccess;
   int64_t blocks = (n / 4 + 255) / 256;
   if (blocks < 1) blocks = 1;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
   affine_kernel<<<(unsigned)blocks, 256, 0, s>>>(x, y, n, a, b);
   g_launches++;
   return cudaGetLastError();
@@ -55,7 +67,7 @@ cudaError_t launch_affine(const float* x, float* y, int64_t n, const float* a, c
 // DRAM bursts) and one of `splits` K-chunks. 512 threads = 128 float4 columns x 4 k-lanes; every
 // thread keeps kUnroll independent 16-byte loads in flight (64 KB per CTA).
 constexpr int kThreads = 512;
-constexpr int kColsPerThread = 8;                          // one 256-bit load (LDG.E.256, new on sm_100)
+constexpr int kColsPerThread = 8;                          // two adjacent 128-bit loads (32 contiguous bytes)
 constexpr int kColGroups = 64;                             // 32-byte column groups per strip
 constexpr int kStripCols = kColGroups * kColsPerThread;    // 512
 constexpr int kKLanes = kThreads / kColGroups;             // 8
@@ -67,10 +79,14 @@ struct __align__(32) float8 { float v[8]; };
 // streaming 32-byte load: no L1 allocation, L2 evict-first (W is read exactly once per pass)
 __device__ __forceinline__ float8 ld_stream(const float8* p) {
   float8 r;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3]), "=f"(r.v[4]), "=f"(r.v[5]), "=f"(r.v[6]),
-                 "=f"(r.v[7])
-               : "l"(p));
+  uint64_t pol;
+  asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f32 {%0,%1,%2,%3}, [%4], %5;"
+               : "=f"(r.v[0]), "=f"(r.v[1]), "=f"(r.v[2]), "=f"(r.v[3])
+               : "l"(p), "l"(pol));
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f32 {%0,%1,%2,%3}, [%4+16], %5;"
+               : "=f"(r.v[4]), "=f"(r.v[5]), "=f"(r.v[6]), "=f"(r.v[7])
+               : "l"(p), "l"(pol));
   return r;
 }
 
@@ -236,8 +252,7 @@ dense_stream_kernel(const float* __restrict__ x, const float* __restrict__ w, co
 // row segment into a ring of kBulkStages x 32 KB shared-memory stages guarded by full / empty mbarriers, so the bytes in
 // flight per SM (~128 KB) are not bounded by registers. 16 consumer warps = 64 column groups x 8 k-lanes; a thread owns
 // the float4 column groups cg and cg + 64 of the strip (both LDS.128 conflict-free) and accumulates with packed
-// `fma.rn.f32x2` (FFMA2: two columns per issue slot, x broadcast from a scalar register), which halves the issue
-// pressure that bounded the first version of this kernel (profiles/r1_summary.md).
+// register pairs (two adjacent columns per 64-bit shared load, x broadcast from a scalar register).
 constexpr int kBulkStageRows = 16;
 constexpr int kBulkStages = 5;
 constexpr int kBulkColGroups = kStripCols / 8;    // 64 threads across a strip, 2 x float4 each
@@ -257,9 +272,10 @@ __device__ __forceinline__ void lds_2x64(uint32_t saddr, uint64_t& lo, uint64_t&
   asm volatile("ld.shared.v2.b64 {%0,%1}, [%2];" : "=l"(lo), "=l"(hi) : "r"(saddr));
 }
 __device__ __forceinline__ void ffma2(uint64_t& acc, float xs, uint64_t w2) {
-  uint64_t x2;
-  asm("mov.b64 %0, {%1, %1};" : "=l"(x2) : "f"(xs));
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(x2), "l"(w2));
+  float a0, a1, w0, w1;
+  asm("mov.b64 {%0, %1}, %2;" : "=f"(a0), "=f"(a1) : "l"(acc));
+  asm("mov.b64 {%0, %1}, %2;" : "=f"(w0), "=f"(w1) : "l"(w2));
+  asm("mov.b64 %0, {%1, %2};" : "=l"(acc) : "f"(fmaf(xs, w0, a0)), "f"(fmaf(xs, w1, a1)));
 }
 
 template <int R>
@@ -469,8 +485,8 @@ struct DensePlan {
 static DensePlan plan_dense(int k, int n) {
   DensePlan p;
   p.strips = (n + kStripCols - 1) / kStripCols;
-  // fill ~one CTA per SM (148 on B200); each chunk must fit the smem x stage
-  int splits = 148 / p.strips;
+  // fill ~one CTA per SM; each chunk must fit the smem x stage
+  int splits = device_sm_count() / p.strips;
   if (splits < 1) splits = 1;
   int min_splits = (k + kMaxChunkK - 1) / kMaxChunkK;
   if (splits < min_splits) splits = min_splits;

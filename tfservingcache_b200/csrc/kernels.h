@@ -1,4 +1,4 @@
-// Device kernels of the executor (SURVEY.md section 8a row X). All fp32, sm_100a.
+// Device kernels of the executor (SURVEY.md section 8a row X). All fp32, sm_90a.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -22,7 +22,7 @@ cudaError_t launch_dense(const float* x, const float* w, const float* bias, floa
 // 2 / 4 bulk-copy (TMA) ring for the <= 8-row passes (tensor cores above, as in auto), 3 tensor cores for every row count,
 // 5 cluster-pair kernel for the <= 8-row passes (experimental)
 
-// X3: tcgen05/TMEM 3xTF32 path for 9..64 rows per pass (dense_tc.cu)
+// X3: wgmma 3xTF32 path for 9..64 rows per pass (dense_tc.cu)
 bool dense_tc_supported(int rows, int k, int n, const float* w, const float* x, const float* bias, const float* y);
 size_t dense_tc_workspace_bytes(int k, int n);
 cudaError_t launch_dense_tc(const float* x, const float* w, const float* bias, float* y, int rows, int k, int n,
@@ -49,7 +49,7 @@ cudaError_t launch_layernorm(const float* x, const float* res, const int* ids, c
 cudaError_t launch_attention(const float* qkv, const int* ids, float* ctx, int Bn, int S, int H, int heads, cudaStream_t s);
 size_t attention_smem_bytes(int S, int H, int heads);
 
-// tcgen05 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
+// wgmma 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
 bool gemm_tc_supported(const float* A, const float* B, const float* bias, const float* R, const float* C, int M, int N, int K,
                        int lda);
 cudaError_t launch_gemm_tc(const float* A, const float* B, const float* bias, const float* R, float* C, int M, int N, int K,
@@ -65,15 +65,16 @@ struct CopySeg {
 };
 cudaError_t launch_copy_segments(const CopySeg* segs, int n, cudaStream_t s);
 
-// X4: implicit-GEMM convolution on tcgen05 (gemm_tc.cu): y[B,OH,OW,N] = act(conv(x[B,H,W,C], w[KH,KW,C,N]) + bias (+ R)); the A
+// X4: implicit-GEMM convolution on the tensor cores (gemm_tc.cu): y[B,OH,OW,N] = act(conv(x[B,H,W,C], w[KH,KW,C,N]) + bias (+ R)); the A
 // tiles are gathered from the NHWC activations by TMA im2col tensor maps -- no patch matrix in HBM. C % 32 == 0, N % 32 == 0.
 bool conv_tc_supported(const float* x, const float* w, const float* bias, const float* R, const float* y, int Bn, int H, int W,
                        int C, int KH, int KW, int stride, int pad, int OH, int OW, int N);
 cudaError_t launch_conv_tc(const float* x, const float* w, const float* bias, const float* R, float* y, int Bn, int H, int W, int C,
                            int KH, int KW, int stride, int pad, int OH, int OW, int N, int act, cudaStream_t s);
 
-int gemm_trace_read(long long* out16);  // debugging aid (TFSC_GT_TRACE=1): clock64 timeline of CTA 0 of the last persistent GEMM
-
 int64_t kernel_launch_count();
+
+// streaming multiprocessors of the current device (132 on an H100 SXM), queried once per device
+int device_sm_count();
 
 }  // namespace tfsc

@@ -1,9 +1,9 @@
-// Dense-net building blocks for the graph executor (SURVEY.md 8a rows X4 / X5), fp32, sm_100a:
+// Dense-net building blocks for the graph executor (SURVEY.md 8a rows X4 / X5), fp32, sm_90a:
 //   gemm_f32      C[M,N] = act(A[M,K] B[K,N] + bias[N] (+ R[M,N]))   register-tiled FFMA GEMM (exact fp32)
 //   im2col_nhwc   NHWC activations -> [B*OH*OW, KH*KW*C (padded to x4)] patch matrix (conv = im2col + GEMM with
 //                 the TF HWIO kernel flattened to [KH*KW*Cin, Cout]; 1x1/stride-1 convs skip it)
 //   maxpool / global average pool (NHWC), embedding gather + LayerNorm, residual LayerNorm, attention
-// launch_gemm dispatches to the tcgen05 3xTF32 GEMM of gemm_tc.cu when the shape allows (M >= 64, N % 32 == 0,
+// launch_gemm dispatches to the wgmma 3xTF32 GEMM of gemm_tc.cu when the shape allows (M >= 64, N % 32 == 0,
 // K >= 32); gemm_f32_kernel (CUDA-core FFMA, exact fp32) covers the rest (small M, N = 1000 / 2 heads, conv1's K).
 #include <cuda_runtime.h>
 
@@ -183,7 +183,7 @@ im2col_nhwc_kernel(const float* __restrict__ x, float* __restrict__ col, int Bn,
 __global__ void __launch_bounds__(1024)
 im2col_rows_kernel(const float* __restrict__ x, float* __restrict__ col, int Bn, int H, int W, int C, int KH, int KW,
                    int stride, int pad, int OH, int OW, int ldc) {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tcgen05 GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tensor-core GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
   const int Kreal = KH * KW * C;
   const int64_t rows = (int64_t)Bn * OH * OW;
   for (int kk = threadIdx.x; kk < ldc; kk += blockDim.x) {
@@ -208,7 +208,7 @@ cudaError_t launch_im2col(const float* x, float* col, int Bn, int H, int W, int 
   const int bx = ldc >= 256 ? 256 : (ldc + 31) / 32 * 32;
   const int by = 1024 / bx >= 1 ? (1024 / bx > 8 ? 8 : 1024 / bx) : 1;
   int64_t blocks = (rows + by - 1) / by;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > device_sm_count() * 8) blocks = device_sm_count() * 8;
   im2col_rows_kernel<<<(unsigned)blocks, dim3(bx, by), 0, s>>>(x, col, Bn, H, W, C, KH, KW, stride, pad, OH, OW, ldc);
   g_launches_nn++;
   return cudaGetLastError();
@@ -218,7 +218,7 @@ cudaError_t launch_im2col(const float* x, float* col, int Bn, int H, int W, int 
 __global__ void __launch_bounds__(256)
 maxpool_nhwc_kernel(const float* __restrict__ x, float* __restrict__ y, int Bn, int H, int W, int C, int KH, int KW, int stride,
                     int pad, int OH, int OW) {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tcgen05 GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tensor-core GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
   const int64_t total = (int64_t)Bn * OH * OW * C;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
     const int c = (int)(idx % C);
@@ -238,7 +238,7 @@ cudaError_t launch_maxpool(const float* x, float* y, int Bn, int H, int W, int C
   const int64_t total = (int64_t)Bn * OH * OW * C;
   if (total <= 0) return cudaSuccess;
   int64_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > device_sm_count() * 16) blocks = device_sm_count() * 16;
   maxpool_nhwc_kernel<<<(unsigned)blocks, 256, 0, s>>>(x, y, Bn, H, W, C, KH, KW, stride, pad, OH, OW);
   g_launches_nn++;
   return cudaGetLastError();
@@ -247,7 +247,7 @@ cudaError_t launch_maxpool(const float* x, float* y, int Bn, int H, int W, int C
 // y[b][c] = mean over H*W of x[b][h][w][c]; sequential fp32 sum per (b,c): deterministic
 __global__ void __launch_bounds__(256)
 avgpool_nhwc_kernel(const float* __restrict__ x, float* __restrict__ y, int Bn, int HW, int C) {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tcgen05 GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tensor-core GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= Bn * C) return;
   const int c = idx % C, b = idx / C;
@@ -297,7 +297,7 @@ layernorm_kernel(const float* __restrict__ x, const float* __restrict__ res, con
                  const float* __restrict__ word, const float* __restrict__ pos, const float* __restrict__ type,
                  const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ y, int S, int H,
                  int vocab, float eps) {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tcgen05 GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tensor-core GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
   __shared__ float2 sh[8];
   extern __shared__ float row[];
   const int token = blockIdx.x;
@@ -405,7 +405,7 @@ attention_kernel(const float* __restrict__ qkv, const int* __restrict__ ids, flo
 template <int KPL>
 __global__ void __launch_bounds__(128)
 attention_tile_kernel(const float* __restrict__ qkv, const int* __restrict__ ids, float* __restrict__ ctx, int S, int H, int heads) {
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tcgen05 GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tensor-core GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
   extern __shared__ __align__(16) float sm[];
   constexpr int SP = 32 * KPL;           // padded key count
   const int d = H / heads, ds = d + 4;   // d % 4 == 0

@@ -132,8 +132,8 @@ static tfsc_server* server_create_impl(const char* config_json) {
       fail(TFSC_E_NO_DEVICE, "gpu.devices: device %d not present", d);
       return nullptr;
     }
-    if (prop.major < 10) {
-      fail(TFSC_E_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_100a (B200) only", d, prop.major,
+    if (prop.major != 9 || prop.minor != 0) {
+      fail(TFSC_E_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a (H100) only", d, prop.major,
            prop.minor);
       return nullptr;
     }
@@ -1367,7 +1367,6 @@ int tfsc_k_conv_tc(const float* x, const float* w, const float* bias, const floa
   cudaError_t e = launch_conv_tc(x, w, bias, r, y, batch, h, wd, c, kh, kw, stride, pad, oh, ow, cout, act, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "conv_tc: %s", cudaGetErrorString(e));
 }
-int tfsc_debug_gemm_trace(long long* out16) { return gemm_trace_read(out16) == 0 ? 0 : fail(TFSC_E_INVALID, "set TFSC_GT_TRACE=1"); }
 int tfsc_k_im2col(const float* x, float* col, int batch, int h, int w, int c, int kh, int kw, int stride, int pad, int ldc,
                   void* stream) {
   if (int rc = check_device()) return rc;
@@ -1385,6 +1384,9 @@ int tfsc_k_avgpool(const float* x, float* y, int batch, int hw, int c, void* str
   if (int rc = check_device()) return rc;
   cudaError_t e = launch_avgpool(x, y, batch, hw, c, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "avgpool: %s", cudaGetErrorString(e));
+}
+int tfsc_debug_gemm_trace(long long*) {
+  return fail(TFSC_E_UNIMPLEMENTED, "no GEMM clock trace: the persistent GEMM kernel it timed is not part of the sm_90a build");
 }
 
 }  // extern "C"
