@@ -280,6 +280,9 @@ size_t tfsc_k_dense_workspace(int rows, int k, int n);
  * variant is bit-reproducible). */
 int tfsc_k_dense_variant(int variant, const float* x, const float* w, const float* b, float* y, int rows, int k, int n,
                          int relu, float* workspace, size_t workspace_bytes, void* stream);
+/* Grid of the <= 8-row cluster-pair kernel on the current device: the number of co-resident 2-CTA clusters (the grid never
+ * exceeds it, so a pass runs in one wave) and the strip width in columns it uses for n output columns. */
+int tfsc_k_dense_cluster_grid(int rows, int n, int* active_clusters, int* strip_cols);
 /* X3: the wgmma (3xTF32) path alone, rows <= 64, n % 32 == 0, k % 4 == 0. tfsc_k_dense picks it
  * automatically for more than 8 rows; this entry exists for parity tests and roofline timing. */
 int tfsc_k_dense_tc(const float* x, const float* w, const float* b, float* y, int rows, int k, int n, int relu,

@@ -126,6 +126,7 @@ _sig("tfsc_k_affine", C.c_int, vp, vp, i64, vp, vp, vp)
 _sig("tfsc_k_dense", C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, sz, vp)
 _sig("tfsc_k_dense_workspace", sz, C.c_int, C.c_int, C.c_int)
 _sig("tfsc_k_dense_variant", C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, sz, vp)
+_sig("tfsc_k_dense_cluster_grid", C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int))
 _sig("tfsc_k_dense_tc", C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, sz, vp)
 _sig("tfsc_k_gemm", C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp)
 _sig("tfsc_k_gemm_tc", C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp)

@@ -1,20 +1,24 @@
-// X2, cluster-pair kernel of the fused dense pass: the DEFAULT for <= 8 rows per pass since round 2 (tfsc_k_dense_variant 0 / 5).
+// X2, cluster-pair kernel of the fused dense pass: the DEFAULT for <= 8 rows per pass (tfsc_k_dense_variant 0 / 5).
 //
 //   y[R,N] = act(x[R,K] W[K,N] + b),  R <= 8 rows per pass, fp32.
 //
 // What it changes against dense_stream_kernel / dense_bulk_kernel (kernels.cu): the split-K tail. Those kernels split K
 // eight ways across independent CTAs and fold the partials through an L2 workspace (partials -> fence -> atomic counter
 // -> last CTA of the strip re-reads 8 partials), a serial tail of several microseconds that grows with R. Here a
-// thread-block CLUSTER of two CTAs (one TPC) owns a 128-column strip, each CTA streams one half of K, and the two halves
-// meet in distributed shared memory: no workspace, no atomics, no second pass -- rank 0 reads rank 1's [R,128] result
+// thread-block CLUSTER of two CTAs (one TPC) owns a column strip, each CTA streams one half of K, and the two halves
+// meet in distributed shared memory: no workspace, no atomics, no second pass -- rank 0 reads rank 1's [R,strip] result
 // with ld.shared::cluster, adds it in fixed order (bit-reproducible), applies bias / ReLU and stores y.
-//   * W: one 2-D TMA box {128 n, 64 k} = 32 KB per stage (tensor map over W[K,N], no swizzle; rows beyond K and columns
-//     beyond N arrive as zeros), 4-stage mbarrier ring = 128 KB in flight per SM.
+//   * grid: one wave. The launch never has more clusters than cudaOccupancyMaxActiveClusters reports for it (66 two-CTA
+//     clusters on a 132-SM H100, one CTA per SM), and the strip width is sized from N and that count: a multiple of 16
+//     columns, at most 144 (N = 9216: 64 strips of 144 columns, 128 CTAs). A 128-column strip would give 72 clusters, and
+//     the last 6 would run as a second wave on 12 SMs. When N needs more than 66 strips of 144, a cluster loops over them.
+//   * W: one 2-D TMA box {strip, 64 k} (36 KB at 144 columns) per stage (tensor map over W[K,N], no swizzle; rows beyond K
+//     and columns beyond N arrive as zeros), 4-stage mbarrier ring = up to 144 KB in flight per SM.
 //   * x: streamed too (a half of K does not fit beside the ring): chunks of 1024 k, R bulk copies each, double-buffered.
-//   * 16 consumer warps: lane = float4 column group of the strip, warp = k-lane (4 consecutive k rows of every stage,
-//     so one broadcast LDS.128 yields x[r][k..k+3]); paired-column accumulation; k-lane reduction through shared memory.
+//   * 576 consumer threads = 16 k-lanes x 36 float4 column groups: k-lane = 4 consecutive k rows of every stage (one
+//     broadcast LDS.128 yields x[r][k..k+3]), paired-column accumulation, k-lane reduction through shared memory in k-lane
+//     order. The K split and the k-lane rows do not depend on the strip width, so every column sums in the same order.
 //   * programmatic dependent launch (TFSC_PDL=1): W streaming starts before griddepcontrol.wait, x after it.
-// Grid: 2 * ceil(N/128) CTAs (144 for N = 9216) in clusters of 2.
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -31,21 +35,24 @@ namespace tfsc {
 std::atomic<int64_t> g_launches_cl{0};
 
 namespace cl {
-constexpr int STRIP = 128;             // columns per cluster
+constexpr int STRIP_MAX = 144;         // columns per cluster strip (runtime width: a multiple of 16, at most this)
+constexpr int GROUPS = STRIP_MAX / 4;  // float4 column groups of the widest strip
 constexpr int SK = 64;                 // k rows per W stage
 constexpr int STAGES = 4;
-constexpr int STAGE_BYTES = STRIP * SK * 4;   // 32 KB
+constexpr int STAGE_MAX_BYTES = STRIP_MAX * SK * 4;   // 36 KB
 constexpr int XC = 1024;               // k per x chunk
-constexpr int CONSUMERS = 512;         // 32 column groups x 16 k-lanes
+constexpr int KLANES = 16;             // 4 consecutive k rows of every stage each
+constexpr int CONSUMERS = GROUPS * KLANES;   // 576: thread = (k-lane, column group)
+constexpr int CONS_WARPS = CONSUMERS / 32;   // 18
 constexpr int THREADS = CONSUMERS + 32;
-constexpr int KLANES = CONSUMERS / 32;
 }  // namespace cl
 
 template <int R>
 struct ClSmem {
-  static constexpr int RING = cl::STAGES * cl::STAGE_BYTES;      // 128 KB
+  static constexpr int RING = cl::STAGES * cl::STAGE_MAX_BYTES;  // 144 KB
   static constexpr int XS = 2 * R * cl::XC * 4;                  // double-buffered x chunks
   static constexpr int TOTAL = RING + XS + 1024;                 // + alignment slack
+  static_assert((cl::KLANES + 1) * R * cl::STRIP_MAX * 4 <= RING, "the k-lane reduction overlays the ring");
 };
 
 __device__ __forceinline__ void cl_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
@@ -79,14 +86,16 @@ __device__ __forceinline__ float4 ld_dsmem_f4(uint32_t local_saddr, uint32_t cta
   return v;
 }
 
+// Grid: one wave of clusters (gridDim.x / 2 <= the co-resident cluster count); cluster c owns strips c, c + clusters, ...
+// of `sw` columns each.
 template <int R>
 __global__ void __launch_bounds__(cl::THREADS, 1)
 dense_cluster_kernel(const __grid_constant__ CUtensorMap wmap, const float* __restrict__ x, const float* __restrict__ bias,
-                     float* __restrict__ y, int rows, int K, int N, int relu, int k_half) {
+                     float* __restrict__ y, int rows, int K, int N, int relu, int k_half, int sw) {
   using S = ClSmem<R>;
   extern __shared__ __align__(1024) uint8_t cl_smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(cl_smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* ring = smem;                                        // [STAGES][SK][STRIP] fp32
+  uint8_t* ring = smem;                                        // [STAGES][SK][sw] fp32
   float* xs = reinterpret_cast<float*>(smem + S::RING);        // [2][R][XC]
   __shared__ __align__(8) uint64_t full[cl::STAGES];
   __shared__ __align__(8) uint64_t empty[cl::STAGES];
@@ -95,7 +104,10 @@ dense_cluster_kernel(const __grid_constant__ CUtensorMap wmap, const float* __re
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint32_t rank = cluster_ctarank();                     // 0 / 1: which half of K
-  const int strip = blockIdx.x >> 1;
+  const int clusters = (int)gridDim.x >> 1;
+  const int strips = (N + sw - 1) / sw;
+  const int stage_bytes = sw * cl::SK * 4;
+  const int groups = sw >> 2;                                  // float4 column groups of a strip
   const int k_begin = (int)rank * k_half;
   const int k_end = min(K, k_begin + k_half);
   const int kc = max(0, k_end - k_begin);
@@ -107,155 +119,169 @@ dense_cluster_kernel(const __grid_constant__ CUtensorMap wmap, const float* __re
 #pragma unroll
     for (int s = 0; s < cl::STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], cl::KLANES);
+      mbar_init(&empty[s], cl::CONS_WARPS);
     }
     mbar_init(&xfull[0], 1);
     mbar_init(&xfull[1], 1);
-    mbar_init(&xempty[0], cl::KLANES);
-    mbar_init(&xempty[1], cl::KLANES);
+    mbar_init(&xempty[0], cl::CONS_WARPS);
+    mbar_init(&xempty[1], cl::CONS_WARPS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&wmap) : "memory");
   }
-  // x buffers start as zeros: rows >= `rows` are never copied, and the tail of the last chunk meets W rows that the
-  // tensor map zero-fills -- 0 * stale must not be NaN
+  // x buffers start as zeros: rows >= `rows` are never copied
   for (int i = tid; i < 2 * R * cl::XC; i += cl::THREADS) xs[i] = 0.f;
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   __syncthreads();
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // no-op without the PDL launch attribute
 
-  uint64_t acc[R][2];
+  // consumer thread = (k-lane, column group): k-lane kl takes k rows 4*kl .. 4*kl+3 of every stage (as with 16 warps of
+  // 32 column groups), so every output column sums in the same order whatever the strip width
+  const int kl = tid / cl::GROUPS, grp = tid - kl * cl::GROUPS;
+  // ring / x-chunk barrier phases run on across the strips of this cluster
+  int it_base = 0, c_base = 0;
+  for (int strip = (int)blockIdx.x >> 1; strip < strips; strip += clusters) {
+    uint64_t acc[R][2];
 #pragma unroll
-  for (int r = 0; r < R; ++r) acc[r][0] = acc[r][1] = 0ull;
+    for (int r = 0; r < R; ++r) acc[r][0] = acc[r][1] = 0ull;
 
-  if (warp == cl::KLANES) {
-    // ===================== producer: W stages (TMA 2-D boxes) and x chunks (bulk copies) =====================
-    auto issue_x_chunk = [&](int c) {
-      const int bsel = c & 1, k0 = c * cl::XC, len = min(cl::XC, kc - k0);
-      if (c >= 2) mbar_wait(&xempty[bsel], ((c >> 1) - 1) & 1);   // consumers finished chunk c-2 (same buffer)
-      if (lane == 0) mbar_expect_tx(&xfull[bsel], (uint32_t)(rows * len * 4));
-      __syncwarp();
-      if (lane < rows)
-        cl_bulk_g2s(xs + ((size_t)bsel * R + lane) * cl::XC, x + (size_t)lane * K + k_begin + k0, (uint32_t)(len * 4), &xfull[bsel]);
-    };
-    const int primed = min(cl::STAGES, n_stage) - 1;             // stage index after which the ring is full
-    for (int it = 0; it < n_stage; ++it) {
-      const int s = it % cl::STAGES;
-      if (it >= cl::STAGES) mbar_wait(&empty[s], ((it / cl::STAGES) - 1) & 1);
-      if (lane == 0) {
-        mbar_expect_tx(&full[s], cl::STAGE_BYTES);
-        tma_load_2d(ring + s * cl::STAGE_BYTES, &wmap, &full[s], strip * cl::STRIP, k_begin + it * cl::SK);
-      }
-      __syncwarp();
-      if (it == primed) {
-        // W never depends on the previous kernel of the stream, x (its output) does: with programmatic dependent launch
-        // the ring fills under the previous kernel's tail and only the first x chunk waits for it
-        asm volatile("griddepcontrol.wait;" ::: "memory");
-        issue_x_chunk(0);
-      }
-      // chunk c >= 1 is requested while chunk c-1 is being consumed (at its 5th stage)
-      if ((it % STAGES_PER_CHUNK) == cl::STAGES && it / STAGES_PER_CHUNK + 1 < n_chunk) issue_x_chunk(it / STAGES_PER_CHUNK + 1);
-    }
-    if (n_stage == 0) asm volatile("griddepcontrol.wait;" ::: "memory");
-  } else {
-    // ===================== consumers: warp = k-lane (rows 4*warp .. 4*warp+3 of every stage), lane = column group =====
-    const uint32_t ring_s = smem_u32(ring) + (uint32_t)lane * 16u + (uint32_t)(warp * 4 * cl::STRIP * 4);
-    const uint32_t xs_s = smem_u32(xs);
-    for (int it = 0; it < n_stage; ++it) {
-      const int s = it % cl::STAGES;
-      const int c = it / STAGES_PER_CHUNK, b = c & 1;
-      if ((it % STAGES_PER_CHUNK) == 0) mbar_wait(&xfull[b], (c >> 1) & 1);
-      const int kq = (it % STAGES_PER_CHUNK) * cl::SK + warp * 4;   // this warp's k offset inside the chunk
-      if (it == n_stage - 1) {
-        // last stage: x positions beyond the valid length meet W rows the tensor map zero-filled; make them zeros too
-        // (stale data from an earlier chunk could hold Inf / NaN). Each warp only ever reads its own offsets.
-        const int valid = kc - c * cl::XC;
-        if (kq + 4 > valid && lane < R) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            if (kq + j >= valid) xs[((size_t)b * R + lane) * cl::XC + kq + j] = 0.f;
+    if (warp == cl::CONS_WARPS) {
+      // ===================== producer: W stages (TMA 2-D boxes) and x chunks (bulk copies) =====================
+      auto issue_x_chunk = [&](int c) {
+        const int gc = c_base + c, bsel = gc & 1, k0 = c * cl::XC, len = min(cl::XC, kc - k0);
+        if (gc >= 2) mbar_wait(&xempty[bsel], ((gc >> 1) - 1) & 1);   // consumers finished chunk gc-2 (same buffer)
+        if (lane == 0) mbar_expect_tx(&xfull[bsel], (uint32_t)(rows * len * 4));
+        __syncwarp();
+        if (lane < rows)
+          cl_bulk_g2s(xs + ((size_t)bsel * R + lane) * cl::XC, x + (size_t)lane * K + k_begin + k0, (uint32_t)(len * 4), &xfull[bsel]);
+      };
+      const int primed = min(cl::STAGES, n_stage) - 1;             // stage index after which the ring is full
+      for (int it = 0; it < n_stage; ++it) {
+        const int gi = it_base + it, s = gi % cl::STAGES;
+        if (gi >= cl::STAGES) mbar_wait(&empty[s], ((gi / cl::STAGES) - 1) & 1);
+        if (lane == 0) {
+          mbar_expect_tx(&full[s], (uint32_t)stage_bytes);
+          tma_load_2d(ring + s * stage_bytes, &wmap, &full[s], strip * sw, k_begin + it * cl::SK);
         }
         __syncwarp();
+        if (it == primed) {
+          // W never depends on the previous kernel of the stream, x (its output) does: with programmatic dependent launch
+          // the ring fills under the previous kernel's tail and only the first x chunk waits for it
+          asm volatile("griddepcontrol.wait;" ::: "memory");
+          issue_x_chunk(0);
+        }
+        // chunk c >= 1 is requested while chunk c-1 is being consumed (at its 5th stage)
+        if ((it % STAGES_PER_CHUNK) == cl::STAGES && it / STAGES_PER_CHUNK + 1 < n_chunk) issue_x_chunk(it / STAGES_PER_CHUNK + 1);
       }
-      mbar_wait(&full[s], (it / cl::STAGES) & 1);
-      const uint32_t wbase = ring_s + (uint32_t)(s * cl::STAGE_BYTES);
-      const uint32_t xk = xs_s + (uint32_t)((b * R * cl::XC + kq) * 4);
-      uint64_t w[4][2];
+      if (n_stage == 0) asm volatile("griddepcontrol.wait;" ::: "memory");
+    } else {
+      // ===================== consumers =====================
+      const bool active = grp < groups;
+      const uint32_t ring_s = smem_u32(ring) + (uint32_t)grp * 16u + (uint32_t)(kl * 4 * sw * 4);
+      const uint32_t xs_s = smem_u32(xs);
+      // one stage: x positions at or beyond `valid` (last stage only) meet W rows the tensor map zero-filled; they count as
+      // zeros (stale x from an earlier chunk could hold Inf / NaN)
+      auto consume = [&](int it, bool tail) {
+        const int gi = it_base + it, s = gi % cl::STAGES;
+        const int c = it / STAGES_PER_CHUNK, b = (c_base + c) & 1;
+        if ((it % STAGES_PER_CHUNK) == 0) mbar_wait(&xfull[b], ((c_base + c) >> 1) & 1);
+        const int kq = (it % STAGES_PER_CHUNK) * cl::SK + kl * 4;   // this k-lane's k offset inside the chunk
+        mbar_wait(&full[s], (gi / cl::STAGES) & 1);
+        if (active) {
+          const uint32_t wbase = ring_s + (uint32_t)(s * stage_bytes);
+          const uint32_t xk = xs_s + (uint32_t)((b * R * cl::XC + kq) * 4);
+          const int valid = kc - c * cl::XC - kq;
+          uint64_t w[4][2];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) cl_lds_2x64(wbase + (uint32_t)(j * cl::STRIP * 4), w[j][0], w[j][1]);
+          for (int j = 0; j < 4; ++j) cl_lds_2x64(wbase + (uint32_t)(j * sw * 4), w[j][0], w[j][1]);
 #pragma unroll
-      for (int r = 0; r < R; ++r) {
-        const float4 xv = lds_f4(xk + (uint32_t)(r * cl::XC * 4));   // x[r][k..k+3], broadcast
-        cl_ffma2(acc[r][0], xv.x, w[0][0]); cl_ffma2(acc[r][1], xv.x, w[0][1]);
-        cl_ffma2(acc[r][0], xv.y, w[1][0]); cl_ffma2(acc[r][1], xv.y, w[1][1]);
-        cl_ffma2(acc[r][0], xv.z, w[2][0]); cl_ffma2(acc[r][1], xv.z, w[2][1]);
-        cl_ffma2(acc[r][0], xv.w, w[3][0]); cl_ffma2(acc[r][1], xv.w, w[3][1]);
-      }
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&empty[s]);
-        if ((it % STAGES_PER_CHUNK) == STAGES_PER_CHUNK - 1 || it == n_stage - 1) mbar_arrive(&xempty[b]);
-      }
+          for (int r = 0; r < R; ++r) {
+            float4 xv = lds_f4(xk + (uint32_t)(r * cl::XC * 4));   // x[r][k..k+3]
+            if (tail) {
+              if (valid < 4) xv.w = 0.f;
+              if (valid < 3) xv.z = 0.f;
+              if (valid < 2) xv.y = 0.f;
+              if (valid < 1) xv.x = 0.f;
+            }
+            cl_ffma2(acc[r][0], xv.x, w[0][0]); cl_ffma2(acc[r][1], xv.x, w[0][1]);
+            cl_ffma2(acc[r][0], xv.y, w[1][0]); cl_ffma2(acc[r][1], xv.y, w[1][1]);
+            cl_ffma2(acc[r][0], xv.z, w[2][0]); cl_ffma2(acc[r][1], xv.z, w[2][1]);
+            cl_ffma2(acc[r][0], xv.w, w[3][0]); cl_ffma2(acc[r][1], xv.w, w[3][1]);
+          }
+        }
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&empty[s]);
+          if ((it % STAGES_PER_CHUNK) == STAGES_PER_CHUNK - 1 || it == n_stage - 1) mbar_arrive(&xempty[b]);
+        }
+      };
+      for (int it = 0; it + 1 < n_stage; ++it) consume(it, false);
+      if (n_stage > 0) consume(n_stage - 1, true);
     }
-  }
+    it_base += n_stage;
+    c_base += n_chunk;
 
-  // ---- k-lane reduction through shared memory (the ring is idle: every full barrier was waited on) ----
-  __syncthreads();
-  // every thread that is about to write y observes the completion of the prerequisite grid itself (y may be a buffer
-  // the previous kernel of the stream still read); long satisfied by now, no-op without the PDL launch attribute
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  float* red = reinterpret_cast<float*>(ring);                     // [KLANES][R][STRIP]   (64 KB at R = 8)
-  float* res = red + cl::KLANES * R * cl::STRIP;                   // [R][STRIP]           (4 KB at R = 8)
-  if (warp < cl::KLANES) {
+    // ---- k-lane reduction through shared memory (the ring is idle: every full barrier was waited on) ----
+    __syncthreads();
+    // every thread that is about to write y observes the completion of the prerequisite grid itself (y may be a buffer
+    // the previous kernel of the stream still read); long satisfied by now, no-op without the PDL launch attribute
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    float* red = reinterpret_cast<float*>(ring);                     // [KLANES][R][sw]
+    float* res = red + cl::KLANES * R * sw;                          // [R][sw]
+    if (warp < cl::CONS_WARPS && grp < groups) {
 #pragma unroll
-    for (int r = 0; r < R; ++r)
-      *reinterpret_cast<ulonglong2*>(red + ((size_t)(warp * R + r) * cl::STRIP) + lane * 4) = make_ulonglong2(acc[r][0], acc[r][1]);
-  }
-  __syncthreads();
-  constexpr int ITEMS = R * (cl::STRIP / 4);                       // float4 items of the [R, 128] result
-  for (int idx = tid; idx < ITEMS; idx += cl::THREADS) {
-    const int r = idx / (cl::STRIP / 4), c4 = idx - r * (cl::STRIP / 4);
-    float4 sacc = *reinterpret_cast<const float4*>(red + (size_t)r * cl::STRIP + c4 * 4);
+      for (int r = 0; r < R; ++r)
+        *reinterpret_cast<ulonglong2*>(red + ((size_t)(kl * R + r) * sw) + grp * 4) = make_ulonglong2(acc[r][0], acc[r][1]);
+    }
+    __syncthreads();
+    const int items = R * groups;                                    // float4 items of the [R, sw] result
+    for (int idx = tid; idx < items; idx += cl::THREADS) {
+      const int r = idx / groups, c4 = idx - r * groups;
+      float4 sacc = *reinterpret_cast<const float4*>(red + (size_t)r * sw + c4 * 4);
 #pragma unroll
-    for (int l = 1; l < cl::KLANES; ++l) {
-      const float4 t = *reinterpret_cast<const float4*>(red + ((size_t)(l * R + r) * cl::STRIP) + c4 * 4);
-      sacc.x += t.x; sacc.y += t.y; sacc.z += t.z; sacc.w += t.w;
+      for (int l = 1; l < cl::KLANES; ++l) {
+        const float4 t = *reinterpret_cast<const float4*>(red + ((size_t)(l * R + r) * sw) + c4 * 4);
+        sacc.x += t.x; sacc.y += t.y; sacc.z += t.z; sacc.w += t.w;
+      }
+      *reinterpret_cast<float4*>(res + (size_t)r * sw + c4 * 4) = sacc;
     }
-    *reinterpret_cast<float4*>(res + (size_t)r * cl::STRIP + c4 * 4) = sacc;
-  }
-  // ---- the two halves of K meet in distributed shared memory ----
-  cluster_sync_all();                                              // both CTAs published `res`
-  if (rank == 0) {
-    const uint32_t res_s = smem_u32(res);
-    for (int idx = tid; idx < ITEMS; idx += cl::THREADS) {
-      const int r = idx / (cl::STRIP / 4), c4 = idx - r * (cl::STRIP / 4);
-      const int col = strip * cl::STRIP + c4 * 4;
-      if (r >= rows || col >= N) continue;
-      float4 a = *reinterpret_cast<const float4*>(res + (size_t)r * cl::STRIP + c4 * 4);
-      const float4 o = ld_dsmem_f4(res_s + (uint32_t)((r * cl::STRIP + c4 * 4) * 4), 1u);
-      const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + col));
-      a.x = a.x + o.x + bv.x; a.y = a.y + o.y + bv.y; a.z = a.z + o.z + bv.z; a.w = a.w + o.w + bv.w;
-      if (relu) { a.x = fmaxf(a.x, 0.f); a.y = fmaxf(a.y, 0.f); a.z = fmaxf(a.z, 0.f); a.w = fmaxf(a.w, 0.f); }
-      *reinterpret_cast<float4*>(y + (size_t)r * N + col) = a;
+    // ---- the two halves of K meet in distributed shared memory ----
+    cluster_sync_all();                                              // both CTAs published `res`
+    if (rank == 0) {
+      const uint32_t res_s = smem_u32(res);
+      for (int idx = tid; idx < items; idx += cl::THREADS) {
+        const int r = idx / groups, c4 = idx - r * groups;
+        const int col = strip * sw + c4 * 4;
+        if (r >= rows || col >= N) continue;
+        float4 a = *reinterpret_cast<const float4*>(res + (size_t)r * sw + c4 * 4);
+        const float4 o = ld_dsmem_f4(res_s + (uint32_t)((r * sw + c4 * 4) * 4), 1u);
+        const float4 bv = __ldg(reinterpret_cast<const float4*>(bias + col));
+        a.x = a.x + o.x + bv.x; a.y = a.y + o.y + bv.y; a.z = a.z + o.z + bv.z; a.w = a.w + o.w + bv.w;
+        if (relu) { a.x = fmaxf(a.x, 0.f); a.y = fmaxf(a.y, 0.f); a.z = fmaxf(a.z, 0.f); a.w = fmaxf(a.w, 0.f); }
+        *reinterpret_cast<float4*>(y + (size_t)r * N + col) = a;
+      }
     }
+    // rank 1's shared memory stays alive until rank 0 has read it; the ring is reused by the next strip after this
+    cluster_sync_all();
   }
-  cluster_sync_all();                                              // rank 1's shared memory stays alive until rank 0 has read it
 }
 
 // --------------------------------------------------------------------------------- host side ----
 struct ClKey {
   const void* w;
-  int k, n;
-  bool operator==(const ClKey& o) const { return w == o.w && k == o.k && n == o.n; }
+  int k, n, sw;
+  bool operator==(const ClKey& o) const { return w == o.w && k == o.k && n == o.n && sw == o.sw; }
 };
 struct ClKeyHash {
-  size_t operator()(const ClKey& m) const { return std::hash<const void*>()(m.w) ^ ((size_t)m.k * 1315423911u) ^ ((size_t)m.n << 20); }
+  size_t operator()(const ClKey& m) const {
+    return std::hash<const void*>()(m.w) ^ ((size_t)m.k * 1315423911u) ^ ((size_t)m.n << 20) ^ ((size_t)m.sw << 44);
+  }
 };
 
-static bool get_cl_map(const float* w, int k, int n, CUtensorMap* out) {
+static bool get_cl_map(const float* w, int k, int n, int sw, CUtensorMap* out) {
   static std::mutex mu;
   static std::unordered_map<ClKey, CUtensorMap, ClKeyHash> cache;
   std::lock_guard<std::mutex> lk(mu);
-  auto it = cache.find({w, k, n});
+  auto it = cache.find({w, k, n, sw});
   if (it != cache.end()) {
     *out = it->second;
     return true;
@@ -265,13 +291,13 @@ static bool get_cl_map(const float* w, int k, int n, CUtensorMap* out) {
   CUtensorMap m;
   const cuuint64_t gdim[2] = {(cuuint64_t)n, (cuuint64_t)k};
   const cuuint64_t gstride[1] = {(cuuint64_t)n * 4};
-  const cuuint32_t box[2] = {(cuuint32_t)cl::STRIP, (cuuint32_t)cl::SK};
+  const cuuint32_t box[2] = {(cuuint32_t)sw, (cuuint32_t)cl::SK};
   const cuuint32_t estr[2] = {1, 1};
   if (enc(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(w), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
           CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
     return false;
   if (cache.size() > 4096) cache.clear();
-  cache[{w, k, n}] = m;
+  cache[{w, k, n, sw}] = m;
   *out = m;
   return true;
 }
@@ -282,29 +308,20 @@ bool dense_cluster_supported(int rows, int k, int n, const float* w, const float
          tc_encode_fn() != nullptr;
 }
 
-template <int R>
-static cudaError_t launch_cl_r(const CUtensorMap& map, const float* x, const float* bias, float* y, int rows, int k, int n, bool relu,
-                               cudaStream_t s) {
-  static bool attr[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (!attr[dev & 63]) {
-    cudaError_t e = cudaFuncSetAttribute(dense_cluster_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, ClSmem<R>::TOTAL);
-    if (e != cudaSuccess) return e;
-    attr[dev & 63] = true;
-  }
-  static const bool pdl = [] {  // programmatic dependent launch is on unless TFSC_PDL=0
+static bool pdl_on() {  // programmatic dependent launch is on unless TFSC_PDL=0
+  static const bool pdl = [] {
     const char* e = getenv("TFSC_PDL");
     return !e || atoi(e) != 0;
   }();
-  const int strips = (n + cl::STRIP - 1) / cl::STRIP;
-  int k_half = ((k + 1) / 2 + cl::SK - 1) / cl::SK * cl::SK;   // rank 0 takes [0, k_half), rank 1 the rest
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2 * strips);
+  return pdl;
+}
+
+static void cl_config(cudaLaunchConfig_t& cfg, cudaLaunchAttribute (&at)[2], int R_smem, int clusters, cudaStream_t s) {
+  cfg = {};
+  cfg.gridDim = dim3(2 * clusters);
   cfg.blockDim = dim3(cl::THREADS);
-  cfg.dynamicSmemBytes = ClSmem<R>::TOTAL;
+  cfg.dynamicSmemBytes = R_smem;
   cfg.stream = s;
-  cudaLaunchAttribute at[2];
   at[0].id = cudaLaunchAttributeClusterDimension;
   at[0].val.clusterDim.x = 2;
   at[0].val.clusterDim.y = 1;
@@ -312,20 +329,84 @@ static cudaError_t launch_cl_r(const CUtensorMap& map, const float* x, const flo
   at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
-  cfg.numAttrs = pdl ? 2 : 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, dense_cluster_kernel<R>, map, x, bias, y, rows, k, n, relu ? 1 : 0, k_half);
+  cfg.numAttrs = pdl_on() ? 2 : 1;
+}
+
+// Per device and row template: the smem attribute is set and the number of 2-CTA clusters that are co-resident
+// (cudaOccupancyMaxActiveClusters for this exact launch configuration; 66 on a 132-SM H100) is cached. The grid never
+// exceeds it, so every pass runs in one wave.
+template <int R>
+static cudaError_t cl_active_clusters(int* out) {
+  static int cached[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (cached[dev & 63] > 0) {
+    *out = cached[dev & 63];
+    return cudaSuccess;
+  }
+  cudaError_t e = cudaFuncSetAttribute(dense_cluster_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, ClSmem<R>::TOTAL);
+  if (e != cudaSuccess) return e;
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute at[2];
+  cl_config(cfg, at, ClSmem<R>::TOTAL, 1, 0);
+  cfg.numAttrs = 1;   // the cluster shape alone decides co-residency
+  int n = 0;
+  e = cudaOccupancyMaxActiveClusters(&n, dense_cluster_kernel<R>, &cfg);
+  if (e != cudaSuccess) return e;
+  if (n < 1) return cudaErrorLaunchOutOfResources;
+  cached[dev & 63] = n;
+  *out = n;
+  return cudaSuccess;
+}
+
+// Strip width for N columns over `clusters` co-resident clusters: the narrowest multiple of 16 that covers N in one strip
+// per cluster, capped at STRIP_MAX (wider N: clusters loop over several strips). N = 9216 on 66 clusters: 144 columns,
+// 64 strips.
+static int cl_strip_width(int n, int clusters) {
+  int sw = ((n + clusters - 1) / clusters + 15) / 16 * 16;
+  if (sw > cl::STRIP_MAX) sw = cl::STRIP_MAX;
+  if (sw < 16) sw = 16;
+  return sw;
+}
+
+template <int R>
+static cudaError_t launch_cl_r(const float* w, const float* x, const float* bias, float* y, int rows, int k, int n, bool relu,
+                               cudaStream_t s) {
+  int active = 0;
+  cudaError_t e = cl_active_clusters<R>(&active);
+  if (e != cudaSuccess) return e;
+  const int sw = cl_strip_width(n, active);
+  CUtensorMap map;
+  if (!get_cl_map(w, k, n, sw, &map)) return cudaErrorNotSupported;
+  const int strips = (n + sw - 1) / sw;
+  const int clusters = strips < active ? strips : active;
+  int k_half = ((k + 1) / 2 + cl::SK - 1) / cl::SK * cl::SK;   // rank 0 takes [0, k_half), rank 1 the rest
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute at[2];
+  cl_config(cfg, at, ClSmem<R>::TOTAL, clusters, s);
+  e = cudaLaunchKernelEx(&cfg, dense_cluster_kernel<R>, map, x, bias, y, rows, k, n, relu ? 1 : 0, k_half, sw);
   g_launches_cl++;
   return e != cudaSuccess ? e : cudaGetLastError();
 }
 
+cudaError_t dense_cluster_grid(int rows, int n, int* active_clusters, int* strip_cols) {
+  int active = 0;
+  cudaError_t e = rows == 1 ? cl_active_clusters<1>(&active)
+                  : rows == 2 ? cl_active_clusters<2>(&active)
+                  : rows <= 4 ? cl_active_clusters<4>(&active)
+                              : cl_active_clusters<8>(&active);
+  if (e != cudaSuccess) return e;
+  *active_clusters = active;
+  *strip_cols = cl_strip_width(n, active);
+  return cudaSuccess;
+}
+
 cudaError_t launch_dense_cluster(const float* x, const float* w, const float* bias, float* y, int rows, int k, int n, bool relu,
                                  cudaStream_t s) {
-  CUtensorMap map;
-  if (!get_cl_map(w, k, n, &map)) return cudaErrorNotSupported;
-  if (rows == 1) return launch_cl_r<1>(map, x, bias, y, rows, k, n, relu, s);
-  if (rows == 2) return launch_cl_r<2>(map, x, bias, y, rows, k, n, relu, s);
-  if (rows <= 4) return launch_cl_r<4>(map, x, bias, y, rows, k, n, relu, s);
-  return launch_cl_r<8>(map, x, bias, y, rows, k, n, relu, s);
+  if (rows == 1) return launch_cl_r<1>(w, x, bias, y, rows, k, n, relu, s);
+  if (rows == 2) return launch_cl_r<2>(w, x, bias, y, rows, k, n, relu, s);
+  if (rows <= 4) return launch_cl_r<4>(w, x, bias, y, rows, k, n, relu, s);
+  return launch_cl_r<8>(w, x, bias, y, rows, k, n, relu, s);
 }
 
 }  // namespace tfsc

@@ -28,11 +28,13 @@ size_t dense_tc_workspace_bytes(int k, int n);
 cudaError_t launch_dense_tc(const float* x, const float* w, const float* bias, float* y, int rows, int k, int n,
                             bool relu, void* workspace, size_t workspace_bytes, cudaStream_t s);
 
-// X2, cluster-pair variant (dense_cluster.cu, EXPERIMENTAL, variant 5): two CTAs of a cluster split K and meet in
+// X2, cluster-pair kernel (dense_cluster.cu, default for <= 8 rows): two CTAs of a cluster split K and meet in
 // distributed shared memory -- no split-K workspace, no atomics. rows <= 8, n % 4 == 0, k % 4 == 0, k >= 128.
 bool dense_cluster_supported(int rows, int k, int n, const float* w, const float* x, const float* bias, const float* y);
 cudaError_t launch_dense_cluster(const float* x, const float* w, const float* bias, float* y, int rows, int k, int n, bool relu,
                                  cudaStream_t s);
+// grid of the cluster kernel on the current device: co-resident 2-CTA clusters and the strip width chosen for n columns
+cudaError_t dense_cluster_grid(int rows, int n, int* active_clusters, int* strip_cols);
 
 // X4/X5 building blocks (nn_kernels.cu): act 0 none / 1 relu / 2 gelu(erf)
 cudaError_t launch_gemm(const float* A, const float* B, const float* bias, const float* R, float* C, int M, int N, int K,

@@ -1335,6 +1335,13 @@ int tfsc_k_dense_variant(int variant, const float* x, const float* w, const floa
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "dense(variant %d): %s", variant, cudaGetErrorString(e));
 }
 
+int tfsc_k_dense_cluster_grid(int rows, int n, int* active_clusters, int* strip_cols) {
+  if (int rc = check_device()) return rc;
+  if (rows < 1 || rows > 8 || n < 1 || !active_clusters || !strip_cols) return fail(TFSC_E_INVALID, "dense_cluster_grid: rows in 1..8, n >= 1");
+  cudaError_t e = dense_cluster_grid(rows, n, active_clusters, strip_cols);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "dense_cluster_grid: %s", cudaGetErrorString(e));
+}
+
 int tfsc_k_dense_tc(const float* x, const float* w, const float* b, float* y, int rows, int k, int n, int relu,
                     float* workspace, size_t workspace_bytes, void* stream) {
   if (int rc = check_device()) return rc;
