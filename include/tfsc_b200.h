@@ -318,6 +318,16 @@ int tfsc_k_im2col(const float* x, float* col, int batch, int h, int w, int c, in
                   void* stream);
 int tfsc_k_maxpool(const float* x, float* y, int batch, int h, int w, int c, int kh, int kw, int stride, int pad, void* stream);
 int tfsc_k_avgpool(const float* x, float* y, int batch, int hw, int c, void* stream);
+/* X5 building blocks of the transformer graphs. Multi-head self-attention: qkv[batch, seq, 3*hidden] (q | k | v of every
+ * token), ctx[batch, seq, hidden]; head width d = hidden / heads, scores scaled by 1/sqrt(d). ids[batch, seq] may be NULL;
+ * a key whose id is 0 ([PAD]) gets the additive mask -10000 unless every key of its sequence is [PAD]. Every seq runs for
+ * d % 4 == 0 and d <= 128 on 16-byte aligned qkv / ctx; other head widths while the row kernel's K / V fit in shared
+ * memory. TFSC_E_INVALID for shapes no kernel can run. */
+int tfsc_k_attention(const float* qkv, const int* ids, float* ctx, int batch, int seq, int hidden, int heads, void* stream);
+/* y[t] = LayerNorm(x[t] (+ res[t])) * gamma + beta over rows of hidden floats (two-pass fp32 mean / variance); res may be
+ * NULL; hidden in 1..12272. */
+int tfsc_k_layernorm(const float* x, const float* res, const float* gamma, const float* beta, float* y, int tokens, int hidden,
+                     float eps, void* stream);
 
 #ifdef __cplusplus
 }

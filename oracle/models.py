@@ -245,6 +245,31 @@ def bert_ops(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30522, 
     return ops
 
 
+def layer_norm_ref(v, gamma, beta, eps):
+    """LayerNorm over the last axis of the torch tensor v, in v's dtype: two-pass mean and (biased) variance,
+    (v - mean) / sqrt(var + eps) * gamma + beta."""
+    import torch
+    mean = v.mean(dim=-1, keepdim=True)
+    var = ((v - mean) ** 2).mean(dim=-1, keepdim=True)
+    return (v - mean) / torch.sqrt(var + eps) * gamma + beta
+
+
+def attention_ref(qkv, ids, heads: int):
+    """BERT multi-head self-attention (google-research/bert modeling.py attention_layer) on a torch tensor
+    qkv[B, S, 3H] = q | k | v, in qkv's dtype: per head softmax(q k^T / sqrt(d) + mask) v with d = H / heads, where the
+    additive mask is -10000 on every key whose token id is 0 ([PAD]); ids[B, S] or None (no mask). Returns ctx[B, S, H]."""
+    import torch
+    Bn, S, C3 = qkv.shape
+    Hd = C3 // 3
+    dh = Hd // heads
+    q, k, v = (qkv[..., i * Hd:(i + 1) * Hd].reshape(Bn, S, heads, dh).permute(0, 2, 1, 3) for i in range(3))
+    sc = q @ k.transpose(-1, -2) / math.sqrt(dh)
+    if ids is not None:
+        sc = sc + ((torch.as_tensor(ids) == 0).to(qkv.dtype) * -10000.0)[:, None, None, :]
+    p = torch.softmax(sc, dim=-1)
+    return (p @ v).permute(0, 2, 1, 3).reshape(Bn, S, Hd)
+
+
 def graph_forward(man: dict, blob: np.ndarray, x: np.ndarray, dtype=np.float64) -> np.ndarray:
     """Interpreter of a graph bundle with torch-CPU functional ops (conv2d / max_pool2d) in `dtype`; NHWC in and
     out, NCHW inside."""
@@ -264,10 +289,8 @@ def graph_forward(man: dict, blob: np.ndarray, x: np.ndarray, dtype=np.float64) 
         return torch.from_numpy(blob[off // 4: off // 4 + n]).to(td)
 
     def layer_norm(v, o):  # v: [B, C, S, 1]
-        mean = v.mean(dim=1, keepdim=True)
-        var = ((v - mean) ** 2).mean(dim=1, keepdim=True)
-        g, bta = vec(o["w_offset"], o["c"]).view(1, -1, 1, 1), vec(o["b_offset"], o["c"]).view(1, -1, 1, 1)
-        return (v - mean) / torch.sqrt(var + o.get("eps", 1e-12)) * g + bta
+        g, bta = vec(o["w_offset"], o["c"]), vec(o["b_offset"], o["c"])
+        return layer_norm_ref(v.permute(0, 2, 3, 1), g, bta, o.get("eps", 1e-12)).permute(0, 3, 1, 2)
 
     for o in man["ops"]:
         src = bufs[o["src"]]
@@ -282,15 +305,8 @@ def graph_forward(man: dict, blob: np.ndarray, x: np.ndarray, dtype=np.float64) 
             v = src + (bufs[o["res"]] if o.get("res", -100) != -100 else 0)
             y = layer_norm(v, o)
         elif o["op"] == "attention":
-            Bn, C3, S, _ = src.shape
-            Hd, nh = C3 // 3, o["heads"]
-            dh = Hd // nh
             qkv = src.squeeze(-1).permute(0, 2, 1)                                    # [B, S, 3H]
-            q, k, v = (qkv[..., i * Hd:(i + 1) * Hd].reshape(Bn, S, nh, dh).permute(0, 2, 1, 3) for i in range(3))
-            sc = q @ k.transpose(-1, -2) / math.sqrt(dh)
-            mask = (bufs[-1] == 0).to(td) * -10000.0                                  # [B, S] additive, [PAD] = 0
-            p = torch.softmax(sc + mask[:, None, None, :], dim=-1)
-            ctx = (p @ v).permute(0, 2, 1, 3).reshape(Bn, S, Hd)
+            ctx = attention_ref(qkv, bufs[-1] if is_ids else None, o["heads"])         # the mask comes from the request's ids
             y = ctx.permute(0, 2, 1).unsqueeze(-1)
         elif o["op"] in ("conv", "dense"):
             kh, kw, c, cout = o.get("kh", 1), o.get("kw", 1), o["c"], o["cout"]

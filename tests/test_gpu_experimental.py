@@ -63,3 +63,62 @@ def test_cluster_pair_dense_kernel(pdl):
     run = subprocess.run([sys.executable, "-c", PDL_SCRIPT], capture_output=True, text=True, timeout=600, env=env, cwd=ROOT)
     assert run.returncode == 0, (run.stdout + run.stderr)[-3000:]
     assert "WORST" in run.stdout
+
+
+BATCH_SCRIPT = r"""
+import sys
+import numpy as np, torch
+import tfservingcache_b200 as t
+lib = t._lib.lib
+out = {}
+rng = np.random.default_rng(0)
+for (K, N) in [(1024, 520), (4096, 4096), (9216, 9216)]:
+    w = torch.from_numpy((rng.standard_normal((K, N)) / K ** 0.5).astype(np.float32)).cuda()
+    b = torch.from_numpy(rng.standard_normal(N).astype(np.float32)).cuda()
+    for rows in (65, 72, 73, 128, 219):
+        x = torch.from_numpy(rng.standard_normal((rows, K)).astype(np.float32)).cuda()
+        ws_bytes = lib.tfsc_k_dense_workspace(rows, K, N); ws = torch.zeros(ws_bytes // 4 + 64, device="cuda")
+        y = torch.full((rows, N), float("nan"), device="cuda")
+        for _ in range(3):   # back to back on one stream and one workspace
+            t._lib.check(lib.tfsc_k_dense(x.data_ptr(), w.data_ptr(), b.data_ptr(), y.data_ptr(), rows, K, N, 1, ws.data_ptr(),
+                                          ws_bytes, None))
+        torch.cuda.synchronize()
+        out[f"k{K}_n{N}_r{rows}"] = y.cpu().numpy()
+dims = [9216, 9216, 9216, 9216]
+cfg = {"modelProvider.type": "synthetic", "modelProvider.synthetic.dims": dims, "modelProvider.synthetic.count": 2,
+       "gpu.devices": [0], "gpu.arenaBytes": 3 << 30, "modelCache.size": 4 << 30}
+stream = torch.cuda.Stream()
+with t.Server(cfg) as srv:
+    srv.ensure(0, "m1", 1)
+    x = torch.from_numpy(rng.standard_normal((219, dims[0])).astype(np.float32)).cuda()
+    ys = {r: torch.full((r, dims[-1]), float("nan"), device="cuda") for r in (219, 70)}
+    for r, y in ys.items():   # the two groups back to back on one stream, as a bench step issues them
+        srv.predict_device(0, "m1", 1, x.data_ptr(), r, y.data_ptr(), stream.cuda_stream)
+    stream.synchronize()
+    for r, y in ys.items():
+        out[f"model_r{r}"] = y.cpu().numpy()
+np.savez(sys.argv[1], **out)
+print("SAVED", len(out))
+"""
+
+
+def test_programmatic_dependent_launch_is_bit_identical_above_64_rows(tmp_path):
+    """Batches above 64 rows run as several dense passes back to back, each allowed to start under the previous one's
+    tail (PDL, on by default). PDL does not change the summation order, so TFSC_PDL=0 must give the same bits: a
+    difference means a pass read x, the workspace or its counters before the previous pass was done with them."""
+    import numpy as np
+    res = {}
+    for pdl in ("default", "0"):
+        env = dict(os.environ, PYTHONPATH=ROOT)
+        env.pop("TFSC_PDL", None)
+        env.pop("TFSC_DENSE_VARIANT", None)
+        if pdl == "0":
+            env["TFSC_PDL"] = "0"
+        path = str(tmp_path / f"pdl_{pdl}.npz")
+        run = subprocess.run([sys.executable, "-c", BATCH_SCRIPT, path], capture_output=True, text=True, timeout=900, env=env, cwd=ROOT)
+        assert run.returncode == 0, (run.stdout + run.stderr)[-3000:]
+        res[pdl] = dict(np.load(path))
+    assert sorted(res["default"]) == sorted(res["0"])
+    for key, y in res["default"].items():
+        assert not np.isnan(y).any(), key
+        assert np.array_equal(y, res["0"][key]), key

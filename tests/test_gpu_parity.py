@@ -67,9 +67,11 @@ def _dense(x, w, b, relu, variant=None):
     return yd.cpu().numpy()
 
 
-@pytest.mark.parametrize("rows", [1, 2, 3, 4, 5, 7, 8, 9, 16, 19])
+@pytest.mark.parametrize("rows", [1, 2, 3, 4, 5, 7, 8, 9, 16, 19, 65, 72, 73, 128, 219])
 @pytest.mark.parametrize("k,n", [(64, 64), (100, 512), (577, 1032), (1024, 520), (9216, 1024), (33, 8), (5000, 4096)])
 def test_k_dense_matches_oracle(rows, k, n):
+    """above 64 rows tfsc_k_dense runs several passes back to back on one split-K workspace: 219 rows = tensor-core passes
+    of 64, 64, 64, 27; 65 / 72 rows = one of 64 and a <= 8-row pass; 73 = 64 + 9"""
     rng = np.random.default_rng(rows * 7919 + k + n)
     x = rng.standard_normal((rows, k)).astype(np.float32)
     w = (rng.standard_normal((k, n)) / np.sqrt(k)).astype(np.float32)
@@ -372,3 +374,29 @@ def test_full_size_tenant_model_matches_oracle():
     ref = _oracle_mlp(3, x, dims, np.float64)
     assert y.shape == (8, 9216) and _close(y, ref) <= TOL
     assert _close(y1, ref[:1]) <= TOL
+
+
+@pytest.mark.parametrize("rows", [219, 70])
+def test_full_size_tenant_model_device_batches_match_oracle(rows):
+    """bench.py's value path: one model group of a step in one tfsc_predict_device call. With Zipf(1) over 60 models and
+    1024 requests the hottest group is ~219 rows (tensor-core passes 64, 64, 64, 27 per layer, programmatic dependent launch
+    between them); 70 rows end in a tensor-core pass followed by a cluster-kernel pass."""
+    torch = _torch()
+    dims = [9216, 9216, 9216, 9216]
+    cfg = {"modelProvider.type": "synthetic", "modelProvider.synthetic.dims": dims, "modelProvider.synthetic.count": 8,
+           "gpu.devices": [0], "gpu.arenaBytes": 3 << 30, "serving.maxConcurrentModels": 2, "modelCache.size": 4 << 30}
+    x = np.random.default_rng(rows).standard_normal((rows, dims[0])).astype(np.float32)
+    stream = torch.cuda.Stream()
+    with t.Server(cfg) as srv:
+        srv.ensure(0, "m5", 1)
+        xd = torch.from_numpy(x).cuda()
+        outs = []
+        for _ in range(2):
+            yd = torch.full((rows, dims[-1]), float("nan"), device="cuda")
+            torch.cuda.synchronize()
+            srv.predict_device(0, "m5", 1, xd.data_ptr(), rows, yd.data_ptr(), stream.cuda_stream)
+            stream.synchronize()
+            outs.append(yd.cpu().numpy())
+    assert np.array_equal(outs[0], outs[1])
+    ref = _oracle_mlp(5, x, dims, np.float64)
+    assert outs[0].shape == ref.shape and not np.isnan(outs[0]).any() and _close(outs[0], ref) <= TOL

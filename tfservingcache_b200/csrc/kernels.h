@@ -5,6 +5,8 @@
 #include <cstddef>
 #include <cstdint>
 
+#include "nn_limits.h"
+
 namespace tfsc {
 
 constexpr int kMaxRowsPerLaunch = 8;  // rows handled by one streaming pass over W (SIMT path)
@@ -48,8 +50,9 @@ cudaError_t launch_avgpool(const float* x, float* y, int Bn, int HW, int C, cuda
 cudaError_t launch_layernorm(const float* x, const float* res, const int* ids, const float* word, const float* pos,
                              const float* type, const float* gamma, const float* beta, float* y, int tokens, int S, int H,
                              int vocab, float eps, cudaStream_t s);
+// multi-head self-attention: qkv[B, S, 3H] (q | k | v), ctx[B, S, H], ids[B, S] ([PAD] = 0 masks a key) or nullptr.
+// Both launchers return cudaErrorInvalidValue for shapes outside attention_supported / layernorm_supported (nn_limits.h).
 cudaError_t launch_attention(const float* qkv, const int* ids, float* ctx, int Bn, int S, int H, int heads, cudaStream_t s);
-size_t attention_smem_bytes(int S, int H, int heads);
 
 // wgmma 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
 bool gemm_tc_supported(const float* A, const float* B, const float* bias, const float* R, const float* C, int M, int N, int K,

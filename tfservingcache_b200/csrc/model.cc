@@ -2,15 +2,19 @@
 
 #include <algorithm>
 
+#include "nn_limits.h"
+
 namespace tfsc {
 
 static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 size_t ModelDesc::scratch_bytes(int64_t rows) const {
   if (tmpl == Template::Mlp) return 2 * (((size_t)rows * (size_t)(max_width > 0 ? max_width : 1) * 4 + 255) & ~(size_t)255);
-  if (tmpl == Template::Graph) return ((size_t)rows * (size_t)(n_buffers * buf_elems + col_elems) * 4 + 255) & ~(size_t)255;
+  if (tmpl == Template::Graph) return (size_t)n_buffers * graph_buf_bytes(rows) + align256((size_t)rows * (size_t)col_elems * 4);
   return 256;
 }
+
+size_t ModelDesc::graph_buf_bytes(int64_t rows) const { return align256((size_t)rows * (size_t)buf_elems * 4); }
 
 static void finish(ModelDesc* d) {
   if (d->tmpl == Template::Graph) {
@@ -195,12 +199,24 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         o.oh = o.h;
         o.ow = o.w;
         o.cout = o.c;
+        if (!layernorm_supported(o.c)) {
+          *err = "graph manifest: no LayerNorm kernel for hidden " + std::to_string(o.c) + " (at most 12272)";
+          return false;
+        }
       } else if (o.kind == OpKind::Attention) {
         o.oh = o.h;
         o.ow = o.w;
         o.cout = o.c / 3;
         if (o.c % 3 || o.heads < 1 || o.cout % o.heads || o.w != 1) {
           *err = "graph manifest: attention expects a packed [S,1,3H] qkv source";
+          return false;
+        }
+        // the executor's scratch buffers are 256-byte aligned (graph_buf_bytes); the request input (src -1) and the response
+        // (dst -2) may be any caller pointer, so an op that reads or writes those must run without the aligned kernels
+        if (!attention_supported(o.h, o.cout, o.heads, o.src >= 0 && o.dst >= 0)) {
+          *err = "graph manifest: no attention kernel for S = " + std::to_string(o.h) + ", hidden " + std::to_string(o.cout) + ", " +
+                 std::to_string(o.heads) + " heads (head width d % 4 == 0 and d <= 128 runs at every S; other widths only while"
+                 " K and V of a head fit in shared memory)";
           return false;
         }
       } else if (o.kind == OpKind::AvgPool) {

@@ -66,6 +66,9 @@ struct ModelDesc {
   int input_dtype = TFSC_DT_FLOAT;    // TFSC_DT_INT32 for token-id inputs (BERT)
   // bytes of executor scratch (activation buffers + im2col) for `rows` images / batch rows
   size_t scratch_bytes(int64_t rows) const;
+  // stride of the graph activation buffers in that scratch: rounded up to 256 bytes, so every buffer (and the im2col
+  // matrix after them) starts 256-byte aligned whatever rows * buf_elems is
+  size_t graph_buf_bytes(int64_t rows) const;
 };
 
 bool parse_manifest(const Json& j, ModelDesc* d, std::string* err);

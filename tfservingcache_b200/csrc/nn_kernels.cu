@@ -334,14 +334,29 @@ cudaError_t launch_layernorm(const float* x, const float* res, const int* ids, c
                              const float* type, const float* gamma, const float* beta, float* y, int tokens, int S, int H,
                              int vocab, float eps, cudaStream_t s) {
   if (tokens <= 0) return cudaSuccess;
+  if (!layernorm_supported(H)) return cudaErrorInvalidValue;
   layernorm_kernel<<<tokens, 256, (size_t)H * sizeof(float), s>>>(x, res, ids, word, pos, type, gamma, beta, y, S, H, vocab, eps);
   g_launches_nn++;
   return cudaGetLastError();
 }
 
+// Additive BERT mask of sequence b: keys whose token id is 0 ([PAD]) get -10000. When every key of the sequence is [PAD]
+// the same constant is added to every score and softmax is invariant to it, so no key is masked: adding -10000 in fp32
+// would round each score to a multiple of 2^-10 and shift the weights by up to 5e-4. Call from every thread of the CTA.
+__device__ __forceinline__ bool attention_all_pad(const int* __restrict__ ids, int b, int S) {
+  int real = 0;
+  if (ids)
+    for (int j = threadIdx.x; j < S && !real; j += blockDim.x) real = __ldg(ids + (size_t)b * S + j) != 0;
+  return ids && !__syncthreads_or(real);
+}
+__device__ __forceinline__ float attention_mask(const int* __restrict__ ids, int b, int S, int j, bool all_pad) {
+  return (ids && !all_pad && __ldg(ids + (size_t)b * S + j) == 0) ? -10000.f : 0.f;
+}
+
 // Multi-head self-attention on a packed qkv buffer [B, S, 3H] (q | k | v), one CTA per (batch, head): K and V of
 // the head are staged in shared memory, each warp owns query rows; softmax with warp shuffles; keys whose token
-// id is 0 ([PAD]) get the BERT additive mask -10000. ctx[B, S, H].
+// id is 0 ([PAD]) get the BERT additive mask -10000. ctx[B, S, H]. Serves head widths the tiled kernels do not take
+// (d % 4 != 0, d > 128) while S·(2d+10)+8d floats fit in shared memory.
 __global__ void __launch_bounds__(256)
 attention_kernel(const float* __restrict__ qkv, const int* __restrict__ ids, float* __restrict__ ctx, int S, int H, int heads) {
   extern __shared__ float sm[];
@@ -358,7 +373,8 @@ attention_kernel(const float* __restrict__ qkv, const int* __restrict__ ids, flo
     Ks[j * (d + 1) + c] = __ldg(base + (size_t)j * 3 * H + H + hd * d + c);
     Vs[j * d + c] = __ldg(base + (size_t)j * 3 * H + 2 * H + hd * d + c);
   }
-  for (int j = threadIdx.x; j < S; j += blockDim.x) Ms[j] = (ids && __ldg(ids + (size_t)b * S + j) == 0) ? -10000.f : 0.f;
+  const bool all_pad = attention_all_pad(ids, b, S);
+  for (int j = threadIdx.x; j < S; j += blockDim.x) Ms[j] = attention_mask(ids, b, S, j, all_pad);
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float scale = rsqrtf((float)d);
@@ -433,8 +449,8 @@ attention_tile_kernel(const float* __restrict__ qkv, const int* __restrict__ ids
     if (q0 + r < S) qv = __ldg(reinterpret_cast<const float4*>(base + (size_t)(q0 + r) * 3 * H + hd * d + c));
     *reinterpret_cast<float4*>(Qs + r * d + c) = qv;
   }
-  for (int j = threadIdx.x; j < SP; j += 128)
-    Ms[j] = j >= S ? -FLT_MAX : ((ids && __ldg(ids + (size_t)b * S + j) == 0) ? -10000.f : 0.f);
+  const bool all_pad = attention_all_pad(ids, b, S);
+  for (int j = threadIdx.x; j < SP; j += 128) Ms[j] = j >= S ? -FLT_MAX : attention_mask(ids, b, S, j, all_pad);
   __syncthreads();
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -504,16 +520,148 @@ attention_tile_kernel(const float* __restrict__ qkv, const int* __restrict__ ids
   }
 }
 
+// Key-block version for S > 256: the same CTA shape and score / P.V loops as attention_tile_kernel<2>, but K and V pass
+// through shared memory 64 keys at a time, so shared memory does not grow with S. Online softmax (Milakov & Gimelshein
+// 2018): each row keeps a running max m and its lanes partial sums l; when a block raises m, l and the P.V accumulators
+// are rescaled by exp(m_old - m_new). A lane owns output dims lane*2 and 64 + lane*2 (d <= 128, d % 4 == 0).
+constexpr int kAttnKeyBlock = 64;
+__global__ void __launch_bounds__(128)
+attention_keyblock_kernel(const float* __restrict__ qkv, const int* __restrict__ ids, float* __restrict__ ctx, int S, int H,
+                          int heads) {
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tensor-core GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
+  extern __shared__ __align__(16) float sm[];
+  constexpr int KB = kAttnKeyBlock;
+  const int d = H / heads, ds = d + 4;
+  const int b = blockIdx.y / heads, hd = blockIdx.y % heads, q0 = blockIdx.x * 32;
+  float* Ks = sm;                        // [KB][ds]
+  float* Vs = Ks + (size_t)KB * ds;      // [KB][d]
+  float* Qs = Vs + (size_t)KB * d;       // [32][d]
+  float* Ps = Qs + 32 * d;               // [32][KB]
+  float* Ms = Ps + 32 * KB;              // [KB] additive mask (-FLT_MAX beyond S)
+  const float* base = qkv + (size_t)b * S * 3 * H;
+  const int d4 = d >> 2;
+  for (int idx = threadIdx.x; idx < 32 * d4; idx += 128) {
+    const int r = idx / d4, c = (idx - r * d4) << 2;
+    float4 qv = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (q0 + r < S) qv = __ldg(reinterpret_cast<const float4*>(base + (size_t)(q0 + r) * 3 * H + hd * d + c));
+    *reinterpret_cast<float4*>(Qs + r * d + c) = qv;
+  }
+  const bool all_pad = attention_all_pad(ids, b, S);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int r0 = warp * 8;
+  const float scale = rsqrtf((float)d);
+  float mrow[8], lsum[8];
+  float2 acc[2][8];
+#pragma unroll
+  for (int r = 0; r < 8; ++r) {
+    mrow[r] = -FLT_MAX;
+    lsum[r] = 0.f;
+    acc[0][r] = acc[1][r] = make_float2(0.f, 0.f);
+  }
+  for (int j0 = 0; j0 < S; j0 += KB) {
+    __syncthreads();  // the previous block's K / V / mask are no longer read
+    for (int idx = threadIdx.x; idx < KB * d4; idx += 128) {
+      const int j = idx / d4, c = (idx - j * d4) << 2;
+      float4 kv = make_float4(0.f, 0.f, 0.f, 0.f), vv = kv;
+      if (j0 + j < S) {
+        kv = __ldg(reinterpret_cast<const float4*>(base + (size_t)(j0 + j) * 3 * H + H + hd * d + c));
+        vv = __ldg(reinterpret_cast<const float4*>(base + (size_t)(j0 + j) * 3 * H + 2 * H + hd * d + c));
+      }
+      *reinterpret_cast<float4*>(Ks + (size_t)j * ds + c) = kv;
+      *reinterpret_cast<float4*>(Vs + (size_t)j * d + c) = vv;
+    }
+    for (int j = threadIdx.x; j < KB; j += 128) Ms[j] = j0 + j >= S ? -FLT_MAX : attention_mask(ids, b, S, j0 + j, all_pad);
+    __syncthreads();
+
+    float sc[8][2];
+#pragma unroll
+    for (int r = 0; r < 8; ++r) sc[r][0] = sc[r][1] = 0.f;
+    for (int c = 0; c < d; c += 4) {
+      float4 kq[2];
+#pragma unroll
+      for (int t = 0; t < 2; ++t) kq[t] = *reinterpret_cast<const float4*>(Ks + (size_t)(lane + 32 * t) * ds + c);
+#pragma unroll
+      for (int r = 0; r < 8; ++r) {
+        const float4 qv = *reinterpret_cast<const float4*>(Qs + (r0 + r) * d + c);
+#pragma unroll
+        for (int t = 0; t < 2; ++t)
+          sc[r][t] = fmaf(qv.x, kq[t].x, fmaf(qv.y, kq[t].y, fmaf(qv.z, kq[t].z, fmaf(qv.w, kq[t].w, sc[r][t]))));
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      float mx = mrow[r];
+#pragma unroll
+      for (int t = 0; t < 2; ++t) {
+        const float m = Ms[lane + 32 * t];
+        sc[r][t] = m == -FLT_MAX ? -FLT_MAX : sc[r][t] * scale + m;
+        mx = fmaxf(mx, sc[r][t]);
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+      // every block holds at least one key < S, so mx is finite from the first block on
+      const float alpha = mrow[r] == -FLT_MAX ? 0.f : expf(mrow[r] - mx);
+      mrow[r] = mx;
+      float part = 0.f;
+#pragma unroll
+      for (int t = 0; t < 2; ++t) {
+        const float e = sc[r][t] == -FLT_MAX ? 0.f : expf(sc[r][t] - mx);
+        Ps[(r0 + r) * KB + lane + 32 * t] = e;
+        part += e;
+      }
+      lsum[r] = fmaf(lsum[r], alpha, part);
+      acc[0][r].x *= alpha;
+      acc[0][r].y *= alpha;
+      acc[1][r].x *= alpha;
+      acc[1][r].y *= alpha;
+    }
+    __syncwarp();  // a warp only reads the 8 rows of P it wrote
+    const int n4 = (min(KB, S - j0) + 3) & ~3;  // V rows and P columns in [S - j0, n4) are zeros
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int dd = lane * 2 + 64 * h;
+      if (dd >= d) break;
+      for (int j = 0; j < n4; j += 4) {
+        float2 v[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) v[u] = *reinterpret_cast<const float2*>(Vs + (size_t)(j + u) * d + dd);
+#pragma unroll
+        for (int r = 0; r < 8; ++r) {
+          const float4 p = *reinterpret_cast<const float4*>(Ps + (r0 + r) * KB + j);
+          acc[h][r].x = fmaf(p.x, v[0].x, fmaf(p.y, v[1].x, fmaf(p.z, v[2].x, fmaf(p.w, v[3].x, acc[h][r].x))));
+          acc[h][r].y = fmaf(p.x, v[0].y, fmaf(p.y, v[1].y, fmaf(p.z, v[2].y, fmaf(p.w, v[3].y, acc[h][r].y))));
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int r = 0; r < 8; ++r) {
+    float l = lsum[r];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
+    const float inv = 1.f / l;
+    if (q0 + r0 + r >= S) continue;
+    float* out = ctx + ((size_t)b * S + q0 + r0 + r) * H + hd * d;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int dd = lane * 2 + 64 * h;
+      if (dd < d) *reinterpret_cast<float2*>(out + dd) = make_float2(acc[h][r].x * inv, acc[h][r].y * inv);
+    }
+  }
+}
+
 static size_t attention_tile_smem(int S, int d, int kpl) {
   const size_t sp = 32 * (size_t)kpl;
   (void)S;
   return (sp * (d + 4) + sp * d + 32 * (size_t)d + 32 * sp + sp) * sizeof(float);
 }
 
-size_t attention_smem_bytes(int S, int H, int heads) {
-  const int d = H / heads;
-  return ((size_t)S * (d + 1) + (size_t)S * d + (size_t)8 * S + 8 * d + S) * sizeof(float);
+static size_t attention_keyblock_smem(int d) {
+  const size_t kb = kAttnKeyBlock;
+  return (kb * (d + 4) + kb * d + 32 * (size_t)d + 32 * kb + kb) * sizeof(float);
 }
+
 
 template <int KPL>
 static cudaError_t launch_attention_tile(const float* qkv, const int* ids, float* ctx, int Bn, int S, int H, int heads, cudaStream_t s) {
@@ -522,7 +670,7 @@ static cudaError_t launch_attention_tile(const float* qkv, const int* ids, float
   int dev = 0;
   cudaGetDevice(&dev);
   if (!attr[dev & 63]) {
-    cudaError_t e = cudaFuncSetAttribute(attention_tile_kernel<KPL>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(attention_tile_kernel<KPL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttnSmemCap);
     if (e != cudaSuccess) return e;
     attr[dev & 63] = true;
   }
@@ -531,24 +679,42 @@ static cudaError_t launch_attention_tile(const float* qkv, const int* ids, float
   return cudaGetLastError();
 }
 
-cudaError_t launch_attention(const float* qkv, const int* ids, float* ctx, int Bn, int S, int H, int heads, cudaStream_t s) {
-  if (Bn <= 0) return cudaSuccess;
-  const int d = H / heads;
-  const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;
-  if (d % 4 == 0 && H % 4 == 0 && al && d <= 128) {
-    const int kpl = (S + 31) / 32;
-    if (kpl <= 1 && attention_tile_smem(S, d, 1) <= 200 * 1024) return launch_attention_tile<1>(qkv, ids, ctx, Bn, S, H, heads, s);
-    if (kpl <= 2 && attention_tile_smem(S, d, 2) <= 200 * 1024) return launch_attention_tile<2>(qkv, ids, ctx, Bn, S, H, heads, s);
-    if (kpl <= 4 && attention_tile_smem(S, d, 4) <= 200 * 1024) return launch_attention_tile<4>(qkv, ids, ctx, Bn, S, H, heads, s);
-    if (kpl <= 8 && attention_tile_smem(S, d, 8) <= 200 * 1024) return launch_attention_tile<8>(qkv, ids, ctx, Bn, S, H, heads, s);
-  }
-  const size_t smem = attention_smem_bytes(S, H, heads);
-  if (smem > 200 * 1024) return cudaErrorInvalidValue;
+static cudaError_t launch_attention_keyblock(const float* qkv, const int* ids, float* ctx, int Bn, int S, int H, int heads,
+                                             cudaStream_t s) {
+  const size_t smem = attention_keyblock_smem(H / heads);
   static bool attr[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   if (!attr[dev & 63]) {
-    cudaError_t e = cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(attention_keyblock_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)attention_keyblock_smem(128));
+    if (e != cudaSuccess) return e;
+    attr[dev & 63] = true;
+  }
+  attention_keyblock_kernel<<<dim3((S + 31) / 32, Bn * heads), 128, smem, s>>>(qkv, ids, ctx, S, H, heads);
+  g_launches_nn++;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_attention(const float* qkv, const int* ids, float* ctx, int Bn, int S, int H, int heads, cudaStream_t s) {
+  if (Bn <= 0) return cudaSuccess;
+  const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;
+  if (!attention_supported(S, H, heads, al)) return cudaErrorInvalidValue;
+  const int d = H / heads;
+  if (d % 4 == 0 && H % 4 == 0 && al && d <= 128) {
+    const int kpl = (S + 31) / 32;
+    if (kpl <= 1 && attention_tile_smem(S, d, 1) <= kAttnSmemCap) return launch_attention_tile<1>(qkv, ids, ctx, Bn, S, H, heads, s);
+    if (kpl <= 2 && attention_tile_smem(S, d, 2) <= kAttnSmemCap) return launch_attention_tile<2>(qkv, ids, ctx, Bn, S, H, heads, s);
+    if (kpl <= 4 && attention_tile_smem(S, d, 4) <= kAttnSmemCap) return launch_attention_tile<4>(qkv, ids, ctx, Bn, S, H, heads, s);
+    if (kpl <= 8 && attention_tile_smem(S, d, 8) <= kAttnSmemCap) return launch_attention_tile<8>(qkv, ids, ctx, Bn, S, H, heads, s);
+    return launch_attention_keyblock(qkv, ids, ctx, Bn, S, H, heads, s);
+  }
+  const size_t smem = attention_smem_bytes(S, H, heads);
+  static bool attr[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (!attr[dev & 63]) {
+    cudaError_t e = cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttnSmemCap);
     if (e != cudaSuccess) return e;
     attr[dev & 63] = true;
   }

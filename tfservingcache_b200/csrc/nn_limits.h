@@ -1,0 +1,29 @@
+// Shapes the transformer kernels of nn_kernels.cu can run. Host-only (no CUDA headers): the manifest loader (model.cc)
+// rejects a bundle with the same rule the launchers apply, so a model that pages in can always be served.
+#pragma once
+#include <cstddef>
+
+namespace tfsc {
+
+constexpr size_t kAttnSmemCap = 200 * 1024;  // dynamic shared memory the attention kernels opt in to
+
+// row-at-a-time attention kernel: K [S][d+1], V [S][d], P [8][S], Q [8][d] and the mask [S] of one head
+inline size_t attention_smem_bytes(int S, int H, int heads) {
+  const int d = H / heads;
+  return ((size_t)S * (d + 1) + (size_t)S * d + (size_t)8 * S + 8 * d + S) * sizeof(float);
+}
+
+// Head width d = H / heads with d % 4 == 0 and d <= 128 runs at every S (tiled kernels up to S = 256, the key-block kernel
+// above) on 16-byte aligned qkv / ctx; every other width runs on the row kernel while its shared memory fits.
+inline bool attention_supported(int S, int H, int heads, bool aligned16) {
+  if (S < 1 || heads < 1 || H < heads || H % heads) return false;
+  const int d = H / heads;
+  if (d % 4 == 0 && H % 4 == 0 && d <= 128 && aligned16) return true;
+  return attention_smem_bytes(S, H, heads) <= kAttnSmemCap;
+}
+
+// LayerNorm stages one row of H floats in dynamic shared memory next to its 64-byte reduction scratch, within the 48 KB a
+// kernel gets without opting in: H <= 12272
+inline bool layernorm_supported(int H) { return H >= 1 && (size_t)H * sizeof(float) + 64 <= 48 * 1024; }
+
+}  // namespace tfsc

@@ -602,7 +602,7 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
   if (d.tmpl == Template::Graph) {
     // conv net: NHWC activations in `n_buffers` scratch buffers, conv = (im2col +) GEMM with fused bias /
     // residual / ReLU epilogue (BN is folded into the kernel + bias when the bundle is written)
-    const size_t buf_bytes = (size_t)rows * d.buf_elems * 4;
+    const size_t buf_bytes = d.graph_buf_bytes(rows);  // 256-byte aligned buffers: the loader's kernel checks rely on it
     char* col = scratch + (size_t)d.n_buffers * buf_bytes;
     auto buf = [&](int i) -> char* { return i == -1 ? const_cast<char*>(x) : i == -2 ? y : scratch + (size_t)i * buf_bytes; };
     const int B = (int)rows;

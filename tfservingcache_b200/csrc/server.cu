@@ -1392,6 +1392,23 @@ int tfsc_k_avgpool(const float* x, float* y, int batch, int hw, int c, void* str
   cudaError_t e = launch_avgpool(x, y, batch, hw, c, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "avgpool: %s", cudaGetErrorString(e));
 }
+int tfsc_k_attention(const float* qkv, const int* ids, float* ctx, int batch, int seq, int hidden, int heads, void* stream) {
+  if (int rc = check_device()) return rc;
+  const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;
+  if (!qkv || !ctx || batch < 1 || (int64_t)batch * heads > 65535 || !attention_supported(seq, hidden, heads, al))
+    return fail(TFSC_E_INVALID, "attention: no kernel for batch %d, seq %d, hidden %d, heads %d", batch, seq, hidden, heads);
+  cudaError_t e = launch_attention(qkv, ids, ctx, batch, seq, hidden, heads, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "attention: %s", cudaGetErrorString(e));
+}
+int tfsc_k_layernorm(const float* x, const float* res, const float* gamma, const float* beta, float* y, int tokens, int hidden,
+                     float eps, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (!x || !gamma || !beta || !y || tokens < 0 || !layernorm_supported(hidden))
+    return fail(TFSC_E_INVALID, "layernorm: no kernel for %d tokens of hidden %d (hidden in 1..12272)", tokens, hidden);
+  cudaError_t e = launch_layernorm(x, res, nullptr, nullptr, nullptr, nullptr, gamma, beta, y, tokens, 1, hidden, 0, eps,
+                                   (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "layernorm: %s", cudaGetErrorString(e));
+}
 int tfsc_debug_gemm_trace(long long*) {
   return fail(TFSC_E_UNIMPLEMENTED, "no GEMM clock trace: the persistent GEMM kernel it timed is not part of the sm_90a build");
 }
