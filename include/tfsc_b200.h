@@ -147,7 +147,8 @@ uint32_t tfsc_crc32c(const void* data, size_t len);   /* CRC-32C (Castagnoli), t
 typedef struct tfsc_server tfsc_server;
 
 typedef struct tfsc_tensor {
-  const char* name;   /* signature key ("x", "y", ...); may be NULL for the only input/output */
+  const char* name;   /* signature key ("x", "y", "input_ids", ...); may be NULL for the only input/output, required when
+                         a request passes several inputs */
   int32_t dtype;      /* TFSC_DT_* */
   int32_t rank;
   int64_t shape[8];
@@ -196,7 +197,12 @@ int tfsc_host_list(tfsc_server* s, int node, char* buf, size_t cap);
 /* proxyServiceServer.Predict (tfservingproxy.go:201-212) with the forward replaced by on-GPU
  * execution: route -> ensure-resident -> batch -> kernels. Host tensors in, host tensors out;
  * out[i].data/nbytes must be a caller buffer large enough for the result (shape is filled).
- * `version` is the verbatim string ("00000123" routes differently from "123": reference quirk). */
+ * `version` is the verbatim string ("00000123" routes differently from "123": reference quirk).
+ * Inputs: n_in >= 1 named tensors. A single-input model takes one tensor (its name may be NULL). A model whose manifest
+ * declares signature.inputs (e.g. BERT: input_ids / input_mask / segment_ids) takes exactly those, each DT_INT32
+ * [batch, seq] (or [seq]) with the same batch; a missing, extra or misnamed input, unequal batch sizes, a wrong per-row
+ * size or a float tensor answer TFSC_E_INVALID naming the expected inputs (after the model is made resident, as every
+ * input error; nothing is launched). The same holds for _deadline, _member and _submit. */
 int tfsc_predict(tfsc_server* s, const char* model_name, const char* version,
                  const tfsc_tensor* in, int n_in, tfsc_tensor* out, int n_out);
 /* tfsc_predict with a deadline (absolute, on the clock of tfsc_now_ns() = CLOCK_MONOTONIC; 0 = none): a request still
@@ -241,7 +247,10 @@ int tfsc_rest_handle(tfsc_server* s, const char* method, const char* url, const 
 /* Device-resident predict on an explicit node/stream: x and y are DEVICE pointers (possibly
  * peer memory of another GPU: the forward hop a6 becomes NVLink loads/stores inside the first /
  * last kernel). rows = batch rows. stream = cudaStream_t or NULL for the node's compute stream.
- * The model must have been made resident (tfsc_model_ensure); it is pinned for the launch. */
+ * The model must have been made resident (tfsc_model_ensure); it is pinned for the launch.
+ * x holds `rows` packed rows of the model's in_dim values. A multi-input model's row is the concatenation of its inputs'
+ * rows (seq int32 values each) in byte-wise sorted NAME order, e.g. input_ids | input_mask | segment_ids: the ids of row r
+ * are x[r*3*seq .. r*3*seq + seq). The kernels read the ids, the attention mask and the segment ids from there. */
 int tfsc_predict_device(tfsc_server* s, int node, const char* model_name, int64_t version,
                         const void* x, int64_t rows, void* y, void* stream);
 int tfsc_node_sync(tfsc_server* s, int node);
@@ -324,6 +333,16 @@ int tfsc_k_avgpool(const float* x, float* y, int batch, int hw, int c, void* str
  * d % 4 == 0 and d <= 128 on 16-byte aligned qkv / ctx; other head widths while the row kernel's K / V fit in shared
  * memory. TFSC_E_INVALID for shapes no kernel can run. */
 int tfsc_k_attention(const float* qkv, const int* ids, float* ctx, int batch, int seq, int hidden, int heads, void* stream);
+/* The same with an explicit attention mask: key j of sequence b is masked iff mask[b*mask_stride + j] == 0 (the same
+ * fully-masked rule). mask may be NULL; (ids, seq) gives tfsc_k_attention. TFSC_E_INVALID for mask_stride < seq. */
+int tfsc_k_attention_mask(const float* qkv, const int* mask, int mask_stride, float* ctx, int batch, int seq, int hidden,
+                          int heads, void* stream);
+/* BERT embeddings: y[b*seq + s] = LayerNorm(word[id] + pos[s] + type[t]) * gamma + beta with id = ids[b*stride + s]
+ * clamped to 0..vocab-1 and t = types[b*stride + s] clamped to 0..1 (types NULL: t = 0). word[vocab, hidden],
+ * pos[>= seq, hidden], type[2, hidden]. TFSC_E_INVALID for stride < seq or hidden outside 1..12272. */
+int tfsc_k_embed(const int* ids, const int* types, int stride, const float* word, const float* pos, const float* type,
+                 const float* gamma, const float* beta, float* y, int batch, int seq, int hidden, int vocab, float eps,
+                 void* stream);
 /* y[t] = LayerNorm(x[t] (+ res[t])) * gamma + beta over rows of hidden floats (two-pass fp32 mean / variance); res may be
  * NULL; hidden in 1..12272. */
 int tfsc_k_layernorm(const float* x, const float* res, const float* gamma, const float* beta, float* y, int tokens, int hidden,

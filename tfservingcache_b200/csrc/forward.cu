@@ -144,6 +144,11 @@ void write_sig(Writer* w, const FwdSignature& s) {
   w->str(s.output_name);
   w->vec(s.input_shape);
   w->vec(s.output_shape);
+  w->u32((uint32_t)s.input_names.size());
+  for (size_t i = 0; i < s.input_names.size(); ++i) {
+    w->str(s.input_names[i]);
+    w->i32(s.input_roles[i]);
+  }
 }
 
 FwdSignature read_sig(Reader* r) {
@@ -156,6 +161,12 @@ FwdSignature read_sig(Reader* r) {
   s.output_name = r->str();
   s.input_shape = r->vec();
   s.output_shape = r->vec();
+  const uint32_t k = r->u32();
+  if (k > 3) r->ok = false;
+  for (uint32_t i = 0; r->ok && i < k; ++i) {
+    s.input_names.push_back(r->str());
+    s.input_roles.push_back(r->i32());
+  }
   return s;
 }
 
@@ -207,6 +218,10 @@ void FwdSignature::to_desc(ModelDesc* d) const {
   d->output_name = output_name;
   d->input_shape = input_shape;
   d->output_shape = output_shape;
+  d->inputs.clear();
+  const int64_t S = input_names.empty() ? 0 : in_dim / (int64_t)input_names.size();
+  for (size_t i = 0; i < input_names.size(); ++i)
+    d->inputs.push_back({input_names[i], (InputRole)input_roles[i], (int64_t)i * S});
 }
 
 FwdSignature FwdSignature::from_desc(const ModelDesc& d) {
@@ -219,6 +234,10 @@ FwdSignature FwdSignature::from_desc(const ModelDesc& d) {
   s.output_name = d.output_name;
   s.input_shape = d.input_shape;
   s.output_shape = d.output_shape;
+  for (auto& mi : d.inputs) {
+    s.input_names.push_back(mi.name);
+    s.input_roles.push_back((int32_t)mi.role);
+  }
   return s;
 }
 
@@ -566,6 +585,19 @@ void Forwarder::handle_fwd(const std::shared_ptr<Conn>& c, const std::string& pa
   const int64_t deadline = r.i64();
   const std::string name = r.str();
   const int64_t version = r.i64();
+  // the packed layout the ingress rank wrote: names and values per row in packed order, its batch size, and what its
+  // manifest-free checks found (reported after residency, like every input error)
+  InputLayout l;
+  l.n_elems = n_elems;
+  l.dtype = dtype;
+  const uint32_t k = r.u32();
+  if (k > 64) r.ok = false;
+  for (uint32_t i = 0; r.ok && i < k; ++i) {
+    l.names.push_back(r.str());
+    l.row_elems.push_back(r.i64());
+  }
+  l.rows = r.i64();
+  l.error = r.str();
   {
     std::lock_guard<std::mutex> lk(inc_mu_);
     incoming_[in] = std::move(owned);
@@ -574,7 +606,7 @@ void Forwarder::handle_fwd(const std::shared_ptr<Conn>& c, const std::string& pa
   if (!r.ok) return send_done(in, TFSC_E_INVALID, "forward: malformed FWD message");
   std::string err;
   // the owner node runs the cache tier exactly as for a local request: fetchModel (hit / reload / miss), then the batcher
-  int rc = node_->prepare({name, version}, n_elems, dtype, &in->req, &in->outcome, &err);
+  int rc = node_->prepare({name, version}, l, &in->req, &in->outcome, &err);
   if (rc < 0) return send_done(in, rc, err);
   const ModelDesc& d = in->req.dm->desc;
   in->sig = FwdSignature::from_desc(d);
@@ -611,8 +643,10 @@ void Forwarder::release_slot(int s) {
   slot_cv_.notify_one();
 }
 
-int Forwarder::forward(int peer, const std::string& name, int64_t version, const void* x, int64_t n_elems, int dtype,
+int Forwarder::forward(int peer, const std::string& name, int64_t version, const std::vector<InTensor>& ts, const InputLayout& l,
                        const OutAllocFn& y_alloc, int* outcome, int64_t deadline_ns, std::string* err) {
+  const int64_t n_elems = l.n_elems;
+  const void* x = ts.empty() ? nullptr : ts[0].data;
   const auto t0 = std::chrono::steady_clock::now();
   stats_.out_requests++;
   auto failed = [&](int rc, const std::string& msg) {
@@ -648,8 +682,10 @@ int Forwarder::forward(int peer, const std::string& name, int64_t version, const
   cudaStream_t stream = streams_[rr_++ % 8];
   char* sx = window_ + (size_t)slot * cfg_.slot_bytes;
   char* sy = sx + half;
-  memcpy(st, x, in_bytes);
-  cudaError_t e = cudaMemcpyAsync(sx, st, in_bytes, cudaMemcpyHostToDevice, stream);
+  // a layout that failed its manifest-free checks is not packed: the owner rejects it once the model is resident
+  const size_t packed = l.error.empty() ? in_bytes : 0;
+  if (packed) pack_rows(ts, l, l.rows, st);  // one tensor: the same bytes as a memcpy of it
+  cudaError_t e = packed ? cudaMemcpyAsync(sx, st, packed, cudaMemcpyHostToDevice, stream) : cudaSuccess;
   if (e == cudaSuccess) e = cudaStreamSynchronize(stream);  // x sits in this rank's HBM before the owner is told about it
   if (e != cudaSuccess) {
     cudaGetLastError();
@@ -668,10 +704,17 @@ int Forwarder::forward(int peer, const std::string& name, int64_t version, const
   m.u64((uint64_t)(sx - window_));
   m.u64((uint64_t)(sy - window_));
   m.i64(n_elems);
-  m.i32(dtype);
+  m.i32(l.dtype);
   m.i64(deadline_ns > 0 ? (int64_t)(budget * 1e9) : 0);
   m.str(name);
   m.i64(version);
+  m.u32((uint32_t)l.names.size());
+  for (size_t i = 0; i < l.names.size(); ++i) {
+    m.str(l.names[i]);
+    m.i64(l.row_elems[i]);
+  }
+  m.i64(l.rows);
+  m.str(l.error);
   bool sent = send_msg(c.get(), MSG_FWD, m.b);
   bool got = false;
   if (sent) {

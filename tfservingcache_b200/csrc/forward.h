@@ -51,6 +51,8 @@ struct FwdSignature {
   int input_dtype = TFSC_DT_FLOAT;
   std::string input_name, output_name;
   std::vector<int64_t> input_shape, output_shape;
+  std::vector<std::string> input_names;  // signature.inputs in packed order (empty: single-input model)
+  std::vector<int32_t> input_roles;
   void to_desc(ModelDesc* d) const;
   static FwdSignature from_desc(const ModelDesc& d);
 };
@@ -61,9 +63,11 @@ class Forwarder {
   ~Forwarder();
   bool init(std::string* err);
 
-  // ingress side: run `name:version` on rank `peer` with host rows x; y_alloc(sig, rows) supplies the host output buffer.
+  // ingress side: run `name:version` on rank `peer` with the host tensors ts (sorted and described by layout_inputs): they
+  // are packed into this rank's window slot and the FWD message carries the layout, which the owner checks against its
+  // manifest. y_alloc(sig, rows) supplies the host output buffer.
   using OutAllocFn = std::function<void*(const ModelDesc&, int64_t rows)>;
-  int forward(int peer, const std::string& name, int64_t version, const void* x, int64_t n_elems, int dtype,
+  int forward(int peer, const std::string& name, int64_t version, const std::vector<InTensor>& ts, const InputLayout& l,
               const OutAllocFn& y_alloc, int* outcome, int64_t deadline_ns, std::string* err);
 
   // device-resident use (bench `value`, tfsc_predict_device with peer pointers)

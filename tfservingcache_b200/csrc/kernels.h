@@ -46,13 +46,16 @@ cudaError_t launch_im2col(const float* x, float* col, int Bn, int H, int W, int 
 cudaError_t launch_maxpool(const float* x, float* y, int Bn, int H, int W, int C, int KH, int KW, int stride, int pad, int OH,
                            int OW, cudaStream_t s);
 cudaError_t launch_avgpool(const float* x, float* y, int Bn, int HW, int C, cudaStream_t s);
-// y = LayerNorm(x (+res)) or, with ids != nullptr, LayerNorm(word[id] + pos[s] + type[0]) (BERT embeddings)
-cudaError_t launch_layernorm(const float* x, const float* res, const int* ids, const float* word, const float* pos,
-                             const float* type, const float* gamma, const float* beta, float* y, int tokens, int S, int H,
-                             int vocab, float eps, cudaStream_t s);
-// multi-head self-attention: qkv[B, S, 3H] (q | k | v), ctx[B, S, H], ids[B, S] ([PAD] = 0 masks a key) or nullptr.
+// y = LayerNorm(x (+res)) or, with ids != nullptr, LayerNorm(word[id] + pos[s] + type[t]) (BERT embeddings): token
+// b*S + s reads ids[b*stride + s] and, unless types is nullptr (segment 0), t = clamp(types[b*stride + s], 0, 1)
+cudaError_t launch_layernorm(const float* x, const float* res, const int* ids, const int* types, int stride, const float* word,
+                             const float* pos, const float* type, const float* gamma, const float* beta, float* y, int tokens,
+                             int S, int H, int vocab, float eps, cudaStream_t s);
+// multi-head self-attention: qkv[B, S, 3H] (q | k | v), ctx[B, S, H]; key j of sequence b is masked when
+// mask[b*mask_stride + j] == 0 (an attention-mask input, or the token ids with stride S: [PAD] = 0); mask may be nullptr.
 // Both launchers return cudaErrorInvalidValue for shapes outside attention_supported / layernorm_supported (nn_limits.h).
-cudaError_t launch_attention(const float* qkv, const int* ids, float* ctx, int Bn, int S, int H, int heads, cudaStream_t s);
+cudaError_t launch_attention(const float* qkv, const int* mask, int mask_stride, float* ctx, int Bn, int S, int H, int heads,
+                             cudaStream_t s);
 
 // wgmma 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
 bool gemm_tc_supported(const float* A, const float* B, const float* bias, const float* R, const float* C, int M, int N, int K,

@@ -20,6 +20,7 @@ static void finish(ModelDesc* d) {
   if (d->tmpl == Template::Graph) {
     d->in_dim = 1;
     for (auto v : d->input_shape) d->in_dim *= v;
+    if (!d->inputs.empty()) d->in_dim *= (int64_t)d->inputs.size();  // the packed row: S values per declared input
     d->out_dim = 1;
     for (auto v : d->output_shape) d->out_dim *= v;
     return;
@@ -84,6 +85,45 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
   if (const Json* sig = j.get("signature")) {
     d->input_name = sig->get_str("input", "x");
     d->output_name = sig->get_str("output", "y");
+    if (const Json* ins = sig->get("inputs")) {
+      if (sig->get("input")) {
+        *err = "signature: 'inputs' and 'input' are mutually exclusive";
+        return false;
+      }
+      if (ins->type != Json::Arr || ins->arr.empty() || ins->arr.size() > 3) {
+        *err = "signature.inputs must list 1 to 3 inputs";
+        return false;
+      }
+      for (auto& ij : ins->arr) {
+        ModelInput mi;
+        mi.name = ij.get_str("name", "");
+        const std::string role = ij.get_str("role", "");
+        if (role == "ids") mi.role = InputRole::Ids;
+        else if (role == "mask") mi.role = InputRole::Mask;
+        else if (role == "type_ids") mi.role = InputRole::TypeIds;
+        else {
+          *err = "signature.inputs: unknown role '" + role + "' (ids, mask, type_ids)";
+          return false;
+        }
+        if (mi.name.empty()) {
+          *err = "signature.inputs: every input needs a name";
+          return false;
+        }
+        for (auto& o : d->inputs)
+          if (o.name == mi.name || o.role == mi.role) {
+            *err = "signature.inputs: duplicate " + std::string(o.name == mi.name ? "name '" + mi.name + "'" : "role '" + role + "'");
+            return false;
+          }
+        d->inputs.push_back(mi);
+      }
+      if (!d->input(InputRole::Ids)) {
+        *err = "signature.inputs: no input has the role 'ids'";
+        return false;
+      }
+      // the packed row holds the inputs in byte-wise name order, so a rank can pack a request without the manifest
+      std::sort(d->inputs.begin(), d->inputs.end(), [](const ModelInput& a, const ModelInput& b) { return a.name < b.name; });
+      d->input_name = d->input(InputRole::Ids)->name;
+    }
   }
   if (const Json* ex = j.get("extra_signatures")) {
     for (auto& e : ex->arr) {
@@ -290,6 +330,21 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
   } else {
     *err = "unknown template '" + t + "'";
     return false;
+  }
+  if (!d->inputs.empty()) {
+    // several inputs feed the embedding (ids, segment ids) and attention (mask) only: every other op reads scratch buffers
+    bool ok = d->tmpl == Template::Graph && d->ops.front().kind == OpKind::Embed;
+    for (size_t i = 1; ok && i < d->ops.size(); ++i) ok = d->ops[i].src != -1 && d->ops[i].res != -1;
+    if (!ok) {
+      *err = "signature.inputs needs a graph bundle whose first op is 'embed' and the only op that reads the request";
+      return false;
+    }
+    if (d->input_dtype != TFSC_DT_INT32) {
+      *err = "signature.inputs needs input_dtype int32";
+      return false;
+    }
+    const int64_t S = d->ops.front().h;
+    for (size_t i = 0; i < d->inputs.size(); ++i) d->inputs[i].offset = (int64_t)i * S;
   }
   finish(d);
   return true;

@@ -46,6 +46,14 @@ struct ExtraSignature {
   std::string feature;
 };
 
+// One declared input of a multi-input graph bundle (signature.inputs): BERT's input_ids / input_mask / segment_ids.
+enum class InputRole { Ids, Mask, TypeIds };
+struct ModelInput {
+  std::string name;
+  InputRole role = InputRole::Ids;
+  int64_t offset = 0;  // elements into the packed request row (inputs in byte-wise sorted name order, S values each)
+};
+
 struct ModelDesc {
   Template tmpl = Template::Mlp;
   std::vector<ExtraSignature> extra_sigs;
@@ -64,6 +72,13 @@ struct ModelDesc {
   std::vector<int64_t> input_shape;   // per image, e.g. [224,224,3]
   std::vector<int64_t> output_shape;  // per image, e.g. [1000]
   int input_dtype = TFSC_DT_FLOAT;    // TFSC_DT_INT32 for token-id inputs (BERT)
+  // signature.inputs, sorted by name (= packed row order); empty for single-input bundles (input_name, in_dim elements)
+  std::vector<ModelInput> inputs;
+  const ModelInput* input(InputRole r) const {
+    for (auto& i : inputs)
+      if (i.role == r) return &i;
+    return nullptr;
+  }
   // bytes of executor scratch (activation buffers + im2col) for `rows` images / batch rows
   size_t scratch_bytes(int64_t rows) const;
   // stride of the graph activation buffers in that scratch: rounded up to 256 bytes, so every buffer (and the im2col

@@ -291,29 +291,34 @@ __device__ __forceinline__ float2 block_sum2(float a, float b, float2* sh) {
 }
 
 // one CTA per token: y = LayerNorm(v) * gamma + beta, where v = x[token] (+ res[token]) or, for the embedding
-// op, word[id] + pos[s] + type[0]. Two-pass mean / variance in fp32 (H <= 4096).
+// op, word[id] + pos[s] + type[t]. Token b*S + s reads its id at ids[b*stride + s] and its segment t at
+// types[b*stride + s] (clamped to 0 / 1, as ids are clamped to the vocabulary); types == nullptr means segment 0.
+// Two-pass mean / variance in fp32 (H <= 4096).
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const float* __restrict__ x, const float* __restrict__ res, const int* __restrict__ ids,
-                 const float* __restrict__ word, const float* __restrict__ pos, const float* __restrict__ type,
-                 const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ y, int S, int H,
-                 int vocab, float eps) {
+                 const int* __restrict__ types, int stride, const float* __restrict__ word, const float* __restrict__ pos,
+                 const float* __restrict__ type, const float* __restrict__ gamma, const float* __restrict__ beta,
+                 float* __restrict__ y, int S, int H, int vocab, float eps) {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tensor-core GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
   __shared__ float2 sh[8];
   extern __shared__ float row[];
   const int token = blockIdx.x;
   const float* xr = nullptr;
   const float* wr = nullptr;
+  const float* tr = type;
   if (ids) {
-    int id = __ldg(ids + token);
+    const size_t at = (size_t)(token / S) * stride + token % S;
+    int id = __ldg(ids + at);
     id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
     wr = word + (size_t)id * H;
+    if (types && __ldg(types + at) > 0) tr = type + H;
   } else {
     xr = x + (size_t)token * H;
   }
   float s = 0.f;
   for (int h = threadIdx.x; h < H; h += blockDim.x) {
     float v;
-    if (ids) v = __ldg(wr + h) + __ldg(pos + (size_t)(token % S) * H + h) + __ldg(type + h);
+    if (ids) v = __ldg(wr + h) + __ldg(pos + (size_t)(token % S) * H + h) + __ldg(tr + h);
     else v = __ldg(xr + h) + (res ? __ldg(res + (size_t)token * H + h) : 0.f);
     row[h] = v;
     s += v;
@@ -330,27 +335,30 @@ layernorm_kernel(const float* __restrict__ x, const float* __restrict__ res, con
     y[(size_t)token * H + h] = (row[h] - mean) * inv * __ldg(gamma + h) + __ldg(beta + h);
 }
 
-cudaError_t launch_layernorm(const float* x, const float* res, const int* ids, const float* word, const float* pos,
-                             const float* type, const float* gamma, const float* beta, float* y, int tokens, int S, int H,
-                             int vocab, float eps, cudaStream_t s) {
+cudaError_t launch_layernorm(const float* x, const float* res, const int* ids, const int* types, int stride, const float* word,
+                             const float* pos, const float* type, const float* gamma, const float* beta, float* y, int tokens,
+                             int S, int H, int vocab, float eps, cudaStream_t s) {
   if (tokens <= 0) return cudaSuccess;
   if (!layernorm_supported(H)) return cudaErrorInvalidValue;
-  layernorm_kernel<<<tokens, 256, (size_t)H * sizeof(float), s>>>(x, res, ids, word, pos, type, gamma, beta, y, S, H, vocab, eps);
+  layernorm_kernel<<<tokens, 256, (size_t)H * sizeof(float), s>>>(x, res, ids, types, stride, word, pos, type, gamma, beta, y, S,
+                                                                   H, vocab, eps);
   g_launches_nn++;
   return cudaGetLastError();
 }
 
-// Additive BERT mask of sequence b: keys whose token id is 0 ([PAD]) get -10000. When every key of the sequence is [PAD]
-// the same constant is added to every score and softmax is invariant to it, so no key is masked: adding -10000 in fp32
-// would round each score to a multiple of 2^-10 and shift the weights by up to 5e-4. Call from every thread of the CTA.
-__device__ __forceinline__ bool attention_all_pad(const int* __restrict__ ids, int b, int S) {
+// Additive BERT mask of sequence b: key j gets -10000 when mask[b*mask_stride + j] == 0. The mask is the request's
+// attention-mask input, or its token ids with mask_stride = S ([PAD] = 0) for bundles that declare no mask. When every
+// key of the sequence is masked the same constant is added to every score and softmax is invariant to it, so no key is
+// masked: adding -10000 in fp32 would round each score to a multiple of 2^-10 and shift the weights by up to 5e-4. Call
+// from every thread of the CTA.
+__device__ __forceinline__ bool attention_all_pad(const int* __restrict__ mask, int mask_stride, int b, int S) {
   int real = 0;
-  if (ids)
-    for (int j = threadIdx.x; j < S && !real; j += blockDim.x) real = __ldg(ids + (size_t)b * S + j) != 0;
-  return ids && !__syncthreads_or(real);
+  if (mask)
+    for (int j = threadIdx.x; j < S && !real; j += blockDim.x) real = __ldg(mask + (size_t)b * mask_stride + j) != 0;
+  return mask && !__syncthreads_or(real);
 }
-__device__ __forceinline__ float attention_mask(const int* __restrict__ ids, int b, int S, int j, bool all_pad) {
-  return (ids && !all_pad && __ldg(ids + (size_t)b * S + j) == 0) ? -10000.f : 0.f;
+__device__ __forceinline__ float attention_mask(const int* __restrict__ mask, int mask_stride, int b, int j, bool all_pad) {
+  return (mask && !all_pad && __ldg(mask + (size_t)b * mask_stride + j) == 0) ? -10000.f : 0.f;
 }
 
 // Multi-head self-attention on a packed qkv buffer [B, S, 3H] (q | k | v), one CTA per (batch, head): K and V of
@@ -358,7 +366,8 @@ __device__ __forceinline__ float attention_mask(const int* __restrict__ ids, int
 // id is 0 ([PAD]) get the BERT additive mask -10000. ctx[B, S, H]. Serves head widths the tiled kernels do not take
 // (d % 4 != 0, d > 128) while S·(2d+10)+8d floats fit in shared memory.
 __global__ void __launch_bounds__(256)
-attention_kernel(const float* __restrict__ qkv, const int* __restrict__ ids, float* __restrict__ ctx, int S, int H, int heads) {
+attention_kernel(const float* __restrict__ qkv, const int* __restrict__ mask, int mask_stride, float* __restrict__ ctx, int S, int H,
+                 int heads) {
   extern __shared__ float sm[];
   const int d = H / heads;            // 64 for BERT-base
   const int b = blockIdx.x / heads, hd = blockIdx.x % heads;
@@ -373,8 +382,8 @@ attention_kernel(const float* __restrict__ qkv, const int* __restrict__ ids, flo
     Ks[j * (d + 1) + c] = __ldg(base + (size_t)j * 3 * H + H + hd * d + c);
     Vs[j * d + c] = __ldg(base + (size_t)j * 3 * H + 2 * H + hd * d + c);
   }
-  const bool all_pad = attention_all_pad(ids, b, S);
-  for (int j = threadIdx.x; j < S; j += blockDim.x) Ms[j] = attention_mask(ids, b, S, j, all_pad);
+  const bool all_pad = attention_all_pad(mask, mask_stride, b, S);
+  for (int j = threadIdx.x; j < S; j += blockDim.x) Ms[j] = attention_mask(mask, mask_stride, b, j, all_pad);
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float scale = rsqrtf((float)d);
@@ -420,7 +429,8 @@ attention_kernel(const float* __restrict__ qkv, const int* __restrict__ ids, flo
 // instructions per FMA than the row-at-a-time kernel above, and 4x the CTAs (BERT-base, 8 x 128: 384 CTAs, 2 per SM).
 template <int KPL>
 __global__ void __launch_bounds__(128)
-attention_tile_kernel(const float* __restrict__ qkv, const int* __restrict__ ids, float* __restrict__ ctx, int S, int H, int heads) {
+attention_tile_kernel(const float* __restrict__ qkv, const int* __restrict__ mask, int mask_stride, float* __restrict__ ctx, int S,
+                      int H, int heads) {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tensor-core GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
   extern __shared__ __align__(16) float sm[];
   constexpr int SP = 32 * KPL;           // padded key count
@@ -449,8 +459,8 @@ attention_tile_kernel(const float* __restrict__ qkv, const int* __restrict__ ids
     if (q0 + r < S) qv = __ldg(reinterpret_cast<const float4*>(base + (size_t)(q0 + r) * 3 * H + hd * d + c));
     *reinterpret_cast<float4*>(Qs + r * d + c) = qv;
   }
-  const bool all_pad = attention_all_pad(ids, b, S);
-  for (int j = threadIdx.x; j < SP; j += 128) Ms[j] = j >= S ? -FLT_MAX : attention_mask(ids, b, S, j, all_pad);
+  const bool all_pad = attention_all_pad(mask, mask_stride, b, S);
+  for (int j = threadIdx.x; j < SP; j += 128) Ms[j] = j >= S ? -FLT_MAX : attention_mask(mask, mask_stride, b, j, all_pad);
   __syncthreads();
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -526,8 +536,8 @@ attention_tile_kernel(const float* __restrict__ qkv, const int* __restrict__ ids
 // are rescaled by exp(m_old - m_new). A lane owns output dims lane*2 and 64 + lane*2 (d <= 128, d % 4 == 0).
 constexpr int kAttnKeyBlock = 64;
 __global__ void __launch_bounds__(128)
-attention_keyblock_kernel(const float* __restrict__ qkv, const int* __restrict__ ids, float* __restrict__ ctx, int S, int H,
-                          int heads) {
+attention_keyblock_kernel(const float* __restrict__ qkv, const int* __restrict__ mask, int mask_stride, float* __restrict__ ctx,
+                          int S, int H, int heads) {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");  // a tensor-core GEMM that follows may start its setup + weight prefetch now (it waits for this grid before touching activations)
   extern __shared__ __align__(16) float sm[];
   constexpr int KB = kAttnKeyBlock;
@@ -546,7 +556,7 @@ attention_keyblock_kernel(const float* __restrict__ qkv, const int* __restrict__
     if (q0 + r < S) qv = __ldg(reinterpret_cast<const float4*>(base + (size_t)(q0 + r) * 3 * H + hd * d + c));
     *reinterpret_cast<float4*>(Qs + r * d + c) = qv;
   }
-  const bool all_pad = attention_all_pad(ids, b, S);
+  const bool all_pad = attention_all_pad(mask, mask_stride, b, S);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r0 = warp * 8;
@@ -571,7 +581,7 @@ attention_keyblock_kernel(const float* __restrict__ qkv, const int* __restrict__
       *reinterpret_cast<float4*>(Ks + (size_t)j * ds + c) = kv;
       *reinterpret_cast<float4*>(Vs + (size_t)j * d + c) = vv;
     }
-    for (int j = threadIdx.x; j < KB; j += 128) Ms[j] = j0 + j >= S ? -FLT_MAX : attention_mask(ids, b, S, j0 + j, all_pad);
+    for (int j = threadIdx.x; j < KB; j += 128) Ms[j] = j0 + j >= S ? -FLT_MAX : attention_mask(mask, mask_stride, b, j0 + j, all_pad);
     __syncthreads();
 
     float sc[8][2];
@@ -664,7 +674,8 @@ static size_t attention_keyblock_smem(int d) {
 
 
 template <int KPL>
-static cudaError_t launch_attention_tile(const float* qkv, const int* ids, float* ctx, int Bn, int S, int H, int heads, cudaStream_t s) {
+static cudaError_t launch_attention_tile(const float* qkv, const int* mask, int mask_stride, float* ctx, int Bn, int S, int H, int heads,
+                                         cudaStream_t s) {
   const size_t smem = attention_tile_smem(S, H / heads, KPL);
   static bool attr[64] = {};
   int dev = 0;
@@ -674,13 +685,13 @@ static cudaError_t launch_attention_tile(const float* qkv, const int* ids, float
     if (e != cudaSuccess) return e;
     attr[dev & 63] = true;
   }
-  attention_tile_kernel<KPL><<<dim3((S + 31) / 32, Bn * heads), 128, smem, s>>>(qkv, ids, ctx, S, H, heads);
+  attention_tile_kernel<KPL><<<dim3((S + 31) / 32, Bn * heads), 128, smem, s>>>(qkv, mask, mask_stride, ctx, S, H, heads);
   g_launches_nn++;
   return cudaGetLastError();
 }
 
-static cudaError_t launch_attention_keyblock(const float* qkv, const int* ids, float* ctx, int Bn, int S, int H, int heads,
-                                             cudaStream_t s) {
+static cudaError_t launch_attention_keyblock(const float* qkv, const int* mask, int mask_stride, float* ctx, int Bn, int S, int H,
+                                             int heads, cudaStream_t s) {
   const size_t smem = attention_keyblock_smem(H / heads);
   static bool attr[64] = {};
   int dev = 0;
@@ -691,23 +702,24 @@ static cudaError_t launch_attention_keyblock(const float* qkv, const int* ids, f
     if (e != cudaSuccess) return e;
     attr[dev & 63] = true;
   }
-  attention_keyblock_kernel<<<dim3((S + 31) / 32, Bn * heads), 128, smem, s>>>(qkv, ids, ctx, S, H, heads);
+  attention_keyblock_kernel<<<dim3((S + 31) / 32, Bn * heads), 128, smem, s>>>(qkv, mask, mask_stride, ctx, S, H, heads);
   g_launches_nn++;
   return cudaGetLastError();
 }
 
-cudaError_t launch_attention(const float* qkv, const int* ids, float* ctx, int Bn, int S, int H, int heads, cudaStream_t s) {
+cudaError_t launch_attention(const float* qkv, const int* mask, int mask_stride, float* ctx, int Bn, int S, int H, int heads,
+                             cudaStream_t s) {
   if (Bn <= 0) return cudaSuccess;
   const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;
   if (!attention_supported(S, H, heads, al)) return cudaErrorInvalidValue;
   const int d = H / heads;
   if (d % 4 == 0 && H % 4 == 0 && al && d <= 128) {
     const int kpl = (S + 31) / 32;
-    if (kpl <= 1 && attention_tile_smem(S, d, 1) <= kAttnSmemCap) return launch_attention_tile<1>(qkv, ids, ctx, Bn, S, H, heads, s);
-    if (kpl <= 2 && attention_tile_smem(S, d, 2) <= kAttnSmemCap) return launch_attention_tile<2>(qkv, ids, ctx, Bn, S, H, heads, s);
-    if (kpl <= 4 && attention_tile_smem(S, d, 4) <= kAttnSmemCap) return launch_attention_tile<4>(qkv, ids, ctx, Bn, S, H, heads, s);
-    if (kpl <= 8 && attention_tile_smem(S, d, 8) <= kAttnSmemCap) return launch_attention_tile<8>(qkv, ids, ctx, Bn, S, H, heads, s);
-    return launch_attention_keyblock(qkv, ids, ctx, Bn, S, H, heads, s);
+    if (kpl <= 1 && attention_tile_smem(S, d, 1) <= kAttnSmemCap) return launch_attention_tile<1>(qkv, mask, mask_stride, ctx, Bn, S, H, heads, s);
+    if (kpl <= 2 && attention_tile_smem(S, d, 2) <= kAttnSmemCap) return launch_attention_tile<2>(qkv, mask, mask_stride, ctx, Bn, S, H, heads, s);
+    if (kpl <= 4 && attention_tile_smem(S, d, 4) <= kAttnSmemCap) return launch_attention_tile<4>(qkv, mask, mask_stride, ctx, Bn, S, H, heads, s);
+    if (kpl <= 8 && attention_tile_smem(S, d, 8) <= kAttnSmemCap) return launch_attention_tile<8>(qkv, mask, mask_stride, ctx, Bn, S, H, heads, s);
+    return launch_attention_keyblock(qkv, mask, mask_stride, ctx, Bn, S, H, heads, s);
   }
   const size_t smem = attention_smem_bytes(S, H, heads);
   static bool attr[64] = {};
@@ -718,7 +730,7 @@ cudaError_t launch_attention(const float* qkv, const int* ids, float* ctx, int B
     if (e != cudaSuccess) return e;
     attr[dev & 63] = true;
   }
-  attention_kernel<<<Bn * heads, 256, smem, s>>>(qkv, ids, ctx, S, H, heads);
+  attention_kernel<<<Bn * heads, 256, smem, s>>>(qkv, mask, mask_stride, ctx, S, H, heads);
   g_launches_nn++;
   return cudaGetLastError();
 }

@@ -606,6 +606,20 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
     char* col = scratch + (size_t)d.n_buffers * buf_bytes;
     auto buf = [&](int i) -> char* { return i == -1 ? const_cast<char*>(x) : i == -2 ? y : scratch + (size_t)i * buf_bytes; };
     const int B = (int)rows;
+    // token-id inputs: single-input bundles read ids [B, S] and derive the attention mask from them ([PAD] = 0, stride S);
+    // multi-input bundles read each declared input at its offset in the packed row, stride in_dim (inputs.h)
+    const int* ids = (const int*)x;
+    const int* mask = d.input_dtype == TFSC_DT_INT32 ? ids : nullptr;
+    const int* types = nullptr;
+    int stride = 0;  // single-input: each op's own S
+    if (!d.inputs.empty()) {
+      const ModelInput* mi = d.input(InputRole::Mask);
+      const ModelInput* ti = d.input(InputRole::TypeIds);
+      ids = (const int*)x + d.input(InputRole::Ids)->offset;
+      mask = mi ? (const int*)x + mi->offset : ids;  // no mask input: [PAD] = 0 of the ids, as single-input bundles
+      types = ti ? (const int*)x + ti->offset : nullptr;
+      stride = (int)d.in_dim;
+    }
     for (const GraphOp& o : d.ops) {
       const float* src = (const float*)buf(o.src);
       float* dst = (float*)buf(o.dst);
@@ -641,14 +655,15 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
       } else if (o.kind == OpKind::MaxPool) {
         e = launch_maxpool(src, dst, B, o.h, o.w, o.c, o.kh, o.kw, o.stride, o.pad, o.oh, o.ow, st);
       } else if (o.kind == OpKind::Embed) {
-        e = launch_layernorm(nullptr, nullptr, (const int*)x, (const float*)(dm.dptr + o.word_off), (const float*)(dm.dptr + o.pos_off),
-                             (const float*)(dm.dptr + o.type_off), (const float*)(dm.dptr + o.w_off), (const float*)(dm.dptr + o.b_off),
-                             dst, B * o.h, o.h, o.c, o.vocab, o.eps, st);
+        e = launch_layernorm(nullptr, nullptr, ids, types, stride ? stride : o.h, (const float*)(dm.dptr + o.word_off),
+                             (const float*)(dm.dptr + o.pos_off), (const float*)(dm.dptr + o.type_off),
+                             (const float*)(dm.dptr + o.w_off), (const float*)(dm.dptr + o.b_off), dst, B * o.h, o.h, o.c, o.vocab,
+                             o.eps, st);
       } else if (o.kind == OpKind::LayerNorm) {
-        e = launch_layernorm(src, o.res == -100 ? nullptr : (const float*)buf(o.res), nullptr, nullptr, nullptr, nullptr,
+        e = launch_layernorm(src, o.res == -100 ? nullptr : (const float*)buf(o.res), nullptr, nullptr, 0, nullptr, nullptr, nullptr,
                              (const float*)(dm.dptr + o.w_off), (const float*)(dm.dptr + o.b_off), dst, B * o.h, o.h, o.c, 0, o.eps, st);
       } else if (o.kind == OpKind::Attention) {
-        e = launch_attention(src, d.input_dtype == TFSC_DT_INT32 ? (const int*)x : nullptr, dst, B, o.h, o.cout, o.heads, st);
+        e = launch_attention(src, mask, stride ? stride : o.h, dst, B, o.h, o.cout, o.heads, st);
       } else {
         e = launch_avgpool(src, dst, B, o.h * o.w, o.c, st);
       }
@@ -762,7 +777,7 @@ int Node::describe(const ModelId& id, ModelDesc* desc, int* outcome, std::string
   return 0;
 }
 
-int Node::prepare(const ModelId& id, int64_t n_elems, int in_dtype, PredictRequest* req, int* outcome, std::string* err) {
+int Node::prepare(const ModelId& id, const InputLayout& l, PredictRequest* req, int* outcome, std::string* err) {
   int rc = fetch(id, &req->dm, err);  // handleModelRequest -> fetchModel, before any input validation (as the reference)
   if (rc < 0) return rc;
   if (outcome) *outcome = rc;
@@ -774,6 +789,16 @@ int Node::prepare(const ModelId& id, int64_t n_elems, int in_dtype, PredictReque
     *err = msg;
     return TFSC_E_INVALID;
   };
+  std::string why;
+  if (!check_layout(d, l, &why)) return reject(why);
+  const int64_t n_elems = l.n_elems;
+  const int in_dtype = l.dtype;
+  if (l.multi()) {
+    if (l.rows > cfg_.max_request_rows)
+      return reject("request has " + std::to_string(l.rows) + " rows; gpu.maxRequestRows is " + std::to_string(cfg_.max_request_rows));
+    req->rows = l.rows;
+    return 0;
+  }
   if (in_dtype != d.input_dtype)
     return reject("input dtype " + std::to_string(in_dtype) + " does not match the model signature (expects dtype " +
                   std::to_string(d.input_dtype) + ")");
@@ -827,8 +852,18 @@ void Node::complete(PredictRequest* r, int rc, const std::string& err) {
 
 int Node::predict_host(const ModelId& id, const void* x, int64_t n_elems, int in_dtype, const OutAllocFn& y_alloc,
                        int* outcome, ModelDesc* desc_out, std::string* err, int64_t deadline_ns) {
+  std::vector<InTensor> ts(1);
+  ts[0].dtype = in_dtype;
+  ts[0].data = x;
+  ts[0].n = x ? n_elems : 0;
+  const InputLayout l = layout_inputs(&ts);
+  return predict_host(id, ts, l, y_alloc, outcome, desc_out, err, deadline_ns);
+}
+
+int Node::predict_host(const ModelId& id, const std::vector<InTensor>& ts, const InputLayout& l, const OutAllocFn& y_alloc,
+                       int* outcome, ModelDesc* desc_out, std::string* err, int64_t deadline_ns) {
   PredictRequest req;
-  int rc = prepare(id, x ? n_elems : 0, in_dtype, &req, outcome, err);
+  int rc = prepare(id, l, &req, outcome, err);
   if (rc < 0) return rc;
   const ModelDesc& d = req.dm->desc;
   if (desc_out) *desc_out = d;
@@ -848,7 +883,7 @@ int Node::predict_host(const ModelId& id, const void* x, int64_t n_elems, int in
     *err = "cannot pin " + std::to_string(in_al + out_b) + " bytes of request staging";
     return TFSC_E_EXHAUSTED;
   }
-  memcpy(st, x, in_b);
+  pack_rows(ts, l, req.rows, st);  // one tensor: the same bytes as a memcpy of it
   req.x = st;
   req.y = st + in_al;
   req.host_staged = true;

@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "arena.h"
+#include "inputs.h"
 #include "lru.h"
 #include "model.h"
 #include "provider.h"
@@ -87,15 +88,19 @@ class Node {
   std::string resident_lines();
   std::string host_lines();
 
-  // host-buffer predict through the batcher (blocks the caller). n_elems = fp32 elements in x;
-  // rows are derived from the model (n_elems / in_dim). y_alloc(desc, rows) supplies the output
-  // buffer once the model is known (return nullptr to reject, e.g. caller buffer too small).
+  // host-buffer predict through the batcher (blocks the caller). `ts` are the request tensors sorted and described by
+  // layout_inputs (inputs.h); one tensor of n_elems values is split into rows by the model (n_elems / in_dim), several
+  // are packed row by row. y_alloc(desc, rows) supplies the output buffer once the model is known (return nullptr to
+  // reject, e.g. caller buffer too small).
   using OutAllocFn = std::function<void*(const ModelDesc&, int64_t rows)>;
-  int predict_host(const ModelId& id, const void* x, int64_t n_elems, int in_dtype, const OutAllocFn& y_alloc, int* outcome,
+  int predict_host(const ModelId& id, const std::vector<InTensor>& ts, const InputLayout& l, const OutAllocFn& y_alloc, int* outcome,
                    ModelDesc* desc_out, std::string* err, int64_t deadline_ns = 0);
+  int predict_host(const ModelId& id, const void* x, int64_t n_elems, int in_dtype, const OutAllocFn& y_alloc, int* outcome,
+                   ModelDesc* desc_out, std::string* err, int64_t deadline_ns = 0);  // one unnamed tensor
   // The two halves of predict_host for asynchronous callers (tickets, forwarded requests):
-  // prepare = fetchModel + signature checks, fills req->dm (pinned) and req->rows; on error nothing stays pinned.
-  int prepare(const ModelId& id, int64_t n_elems, int in_dtype, PredictRequest* req, int* outcome, std::string* err);
+  // prepare = fetchModel + input checks (the layout against the model), fills req->dm (pinned) and req->rows; on error
+  // nothing stays pinned.
+  int prepare(const ModelId& id, const InputLayout& l, PredictRequest* req, int* outcome, std::string* err);
   // enqueue = hand the request to the batcher; req->x / req->y must be set and the request must stay alive until it
   // completes (rc != 1 / on_done called). The pin taken by prepare() is released on completion.
   void enqueue(PredictRequest* req);

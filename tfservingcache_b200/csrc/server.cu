@@ -13,6 +13,7 @@
 #include <stdexcept>
 
 #include "forward.h"
+#include "inputs.h"
 #include "json.h"
 #include "kernels.h"
 #include "node.h"
@@ -332,10 +333,45 @@ static int resolve(tfsc_server* s, const std::string& name, const std::string& v
 
 // ensure-resident -> predict on the owner: a node of this process, or another rank through the forward hop
 // (taskhandler.go:95-147: the request goes to whichever node the ring names, tensors stay in device memory here)
-static int run_predict(tfsc_server* s, Node* node, int remote, const ModelId& id, const void* x, int64_t n, int dtype,
-                       const Node::OutAllocFn& alloc, std::string* err, int64_t deadline_ns = 0) {
-  if (node) return node->predict_host(id, x, n, dtype, alloc, nullptr, nullptr, err, deadline_ns);
-  return s->fwd->forward(remote, id.name, id.version, x, n, dtype, alloc, nullptr, deadline_ns, err);
+static int run_predict(tfsc_server* s, Node* node, int remote, const ModelId& id, const std::vector<InTensor>& ts,
+                       const InputLayout& l, const Node::OutAllocFn& alloc, std::string* err, int64_t deadline_ns = 0) {
+  if (node) return node->predict_host(id, ts, l, alloc, nullptr, nullptr, err, deadline_ns);
+  return s->fwd->forward(remote, id.name, id.version, ts, l, alloc, nullptr, deadline_ns, err);
+}
+static int run_predict_one(tfsc_server* s, Node* node, int remote, const ModelId& id, const void* x, int64_t n, int dtype,
+                           const Node::OutAllocFn& alloc, std::string* err, int64_t deadline_ns = 0) {
+  std::vector<InTensor> ts(1);
+  ts[0].dtype = dtype;
+  ts[0].data = x;
+  ts[0].n = n;
+  const InputLayout l = layout_inputs(&ts);
+  return run_predict(s, node, remote, id, ts, l, alloc, err, deadline_ns);
+}
+
+// The C ABI's input tensors: per-tensor argument checks (before residency, as always), then sorted by name into `ts`.
+// Whether they fit the model is checked once it is resident (Node::prepare, check_layout).
+static int abi_inputs(const tfsc_tensor* in, int n_in, bool need_data, std::vector<InTensor>* ts, InputLayout* l) {
+  for (int i = 0; i < n_in; ++i) {
+    const tfsc_tensor& x = in[i];
+    if ((x.dtype != TFSC_DT_FLOAT && x.dtype != TFSC_DT_INT32) || x.rank < 0 || x.rank > 8)
+      return fail(TFSC_E_INVALID, "predict: input must be DT_FLOAT or DT_INT32, rank <= 8");
+    if (n_in > 1 && !x.name) return fail(TFSC_E_INVALID, "predict: every input needs a name when n_in > 1 (got %d inputs)", n_in);
+    InTensor t;
+    t.name = x.name ? x.name : "";
+    t.dtype = x.dtype;
+    t.data = x.data;
+    t.shape.assign(x.shape, x.shape + x.rank);
+    int64_t n = 1;
+    for (auto d : t.shape) {
+      if (d < 0 || (d != 0 && n > ((int64_t)1 << 40) / d)) return fail(TFSC_E_INVALID, "predict: bad input shape");
+      n *= d;
+    }
+    if ((size_t)n * 4 != x.nbytes || (need_data && !x.data)) return fail(TFSC_E_INVALID, "predict: input nbytes does not match shape");
+    t.n = x.data ? n : 0;
+    ts->push_back(std::move(t));
+  }
+  *l = layout_inputs(ts);
+  return 0;
 }
 
 // Output shape of a request with input shape `in_shape` that the executor will run as `rows` rows. Returns false (with
@@ -412,21 +448,15 @@ static int predict_impl(tfsc_server* s, const char* model_name, const char* vers
   int rc = member >= 0 ? resolve_member(s, member, model_name, version, &node, &id, &remote)
                        : resolve(s, model_name, version, &node, &id, &remote);
   if (rc < 0) return rc;
+  std::vector<InTensor> ts;
+  InputLayout layout;
+  if ((rc = abi_inputs(in, n_in, false, &ts, &layout)) < 0) return rc;
   const tfsc_tensor& x = in[0];
-  if (n_in != 1) return fail(TFSC_E_INVALID, "predict: the model templates take exactly one input tensor (got %d)", n_in);
-  if ((x.dtype != TFSC_DT_FLOAT && x.dtype != TFSC_DT_INT32) || x.rank < 0 || x.rank > 8)
-    return fail(TFSC_E_INVALID, "predict: input must be DT_FLOAT or DT_INT32, rank <= 8");
-  int64_t n = 1;
-  std::vector<int64_t> ishape(x.shape, x.shape + x.rank);
-  for (auto d : ishape) {
-    if (d < 0 || (d != 0 && n > ((int64_t)1 << 40) / d)) return fail(TFSC_E_INVALID, "predict: bad input shape");
-    n *= d;
-  }
-  if ((size_t)n * 4 != x.nbytes) return fail(TFSC_E_INVALID, "predict: input nbytes does not match shape");
+  const std::vector<int64_t>& ishape = ts[0].shape;
   std::string err, bad;
   tfsc_tensor* o = &out[0];
   auto alloc = [&](const ModelDesc& d, int64_t rows) -> void* {
-    if (x.name && d.input_name != x.name) {  // signature check: the template has exactly one input
+    if (d.inputs.empty() && x.name && d.input_name != x.name) {  // signature check of a single-input model
       bad = "input '" + std::string(x.name) + "' does not match the model signature (expects '" + d.input_name + "')";
       return nullptr;
     }
@@ -441,7 +471,7 @@ static int predict_impl(tfsc_server* s, const char* model_name, const char* vers
     o->nbytes = (size_t)on * 4;
     return o->data;
   };
-  rc = run_predict(s, node, remote, id, x.data, n, x.dtype, alloc, &err, deadline_ns);
+  rc = run_predict(s, node, remote, id, ts, layout, alloc, &err, deadline_ns);
   if (rc < 0 && !bad.empty()) return fail(TFSC_E_INVALID, "%s", bad.c_str());
   if (rc < 0) return fail(rc, "%s", err.c_str());
   return 0;
@@ -473,31 +503,40 @@ static int grpc_predict_impl(tfsc_server* s, const void* req, size_t req_len, vo
     if (rc < 0) return fail(rc, "%s", err.c_str());
     return fail(TFSC_E_INVALID, "PredictRequest has no inputs");
   }
-  const TensorView& tv = view.inputs[0];
-  const void* xdata = nullptr;
-  int64_t n = 0;
-  std::vector<float> scratch;
-  std::vector<int32_t> iscratch;
-  bool input_ok;
-  if (tv.dtype == TFSC_DT_INT32) {  // token-id inputs (BERT bundles)
-    const int32_t* ip = nullptr;
-    input_ok = tensor_i32(tv, &ip, &n, &iscratch, &err);
-    xdata = ip;
-  } else {
-    const float* fp = nullptr;
-    input_ok = tensor_f32(tv, &fp, &n, &scratch, &err);
-    xdata = fp;
+  // every named input; tensor_content stays a zero-copy view into the request, packing is the only copy
+  const size_t n_in = view.inputs.size();
+  std::vector<InTensor> ts(n_in);
+  std::vector<std::vector<float>> scratch(n_in);
+  std::vector<std::vector<int32_t>> iscratch(n_in);
+  bool input_ok = true;
+  for (size_t i = 0; i < n_in && input_ok; ++i) {
+    const TensorView& v = view.inputs[i];
+    ts[i].name = v.name;
+    ts[i].shape = v.shape;
+    if (v.dtype == TFSC_DT_INT32) {  // token-id inputs (BERT bundles)
+      const int32_t* ip = nullptr;
+      input_ok = tensor_i32(v, &ip, &ts[i].n, &iscratch[i], &err);
+      ts[i].data = ip;
+      ts[i].dtype = TFSC_DT_INT32;
+    } else {
+      const float* fp = nullptr;
+      input_ok = tensor_f32(v, &fp, &ts[i].n, &scratch[i], &err);
+      ts[i].data = fp;
+      ts[i].dtype = TFSC_DT_FLOAT;
+    }
   }
+  const InputLayout layout = layout_inputs(&ts);
+  const TensorView& tv = view.inputs[0];
   char* buf = nullptr;
   size_t total = 0;
   std::string bad_sig;
   auto alloc = [&](const ModelDesc& d, int64_t rows) -> void* {
-    if (view.inputs.size() != 1 || tv.name != d.input_name) {
+    if (d.inputs.empty() && (n_in != 1 || tv.name != d.input_name)) {
       bad_sig = "input keys do not match the model signature (expects '" + d.input_name + "')";
       return nullptr;
     }
     std::vector<int64_t> sh;
-    if (!out_shape(d, rows, tv.shape, &sh, &bad_sig)) return nullptr;
+    if (!out_shape(d, rows, ts[0].shape, &sh, &bad_sig)) return nullptr;
     std::string prefix, suffix;
     predict_response_frame(view.model_name, id.version, view.signature_name.empty() ? "serving_default" : view.signature_name,
                            d.output_name, sh, &prefix, &suffix);
@@ -517,7 +556,7 @@ static int grpc_predict_impl(tfsc_server* s, const void* req, size_t req_len, vo
     if (rc < 0) return fail(rc, "%s", e2.c_str());
     return fail(TFSC_E_INVALID, "%s", err.c_str());
   }
-  rc = run_predict(s, node, remote, id, xdata, n, tv.dtype == TFSC_DT_INT32 ? TFSC_DT_INT32 : TFSC_DT_FLOAT, alloc, &err);
+  rc = run_predict(s, node, remote, id, ts, layout, alloc, &err);
   if (rc < 0) {
     free(buf);
     s->fail_grpc++;
@@ -557,6 +596,11 @@ static int run_examples(tfsc_server* s, const ExampleRequestView& view, int meth
   ModelDesc d;
   rc = node->describe(id, &d, nullptr, err);  // fetchModel first, like every request of the reference
   if (rc < 0) return rc;
+  if (!d.inputs.empty()) {
+    *err = std::string(method == 1 ? "Classify" : "Regress") + " serves single-input models; " + view.model_name + " has inputs " +
+           expected_inputs(d) + " (use Predict)";
+    return TFSC_E_INVALID;
+  }
   const std::string want = view.signature_name.empty() ? "serving_default" : view.signature_name;
   const ExtraSignature* sg = nullptr;
   for (auto& e : d.extra_sigs)
@@ -658,8 +702,12 @@ static int grpc_session_run_impl(tfsc_server* s, const void* req, size_t req_len
   }
   auto strip = [](const std::string& t) { return t.size() > 2 && t.compare(t.size() - 2, 2, ":0") == 0 ? t.substr(0, t.size() - 2) : t; };
   if (view.feeds.size() != 1 || view.fetch.size() != 1 || !view.target.empty()) {
-    if (node) node->fetch(id, nullptr, &err);
+    ModelDesc d;
+    const bool known = node && node->describe(id, &d, nullptr, &err) >= 0;
     s->fail_grpc++;
+    if (known && !d.inputs.empty())
+      return fail(TFSC_E_INVALID, "SessionRun serves single-input models; %s has inputs %s (use Predict)", view.model_name.c_str(),
+                  expected_inputs(d).c_str());
     return fail(TFSC_E_INVALID, "SessionRun on a model template takes exactly one feed (the signature input) and one fetch (its output)");
   }
   const TensorView& tv = view.feeds[0];
@@ -702,7 +750,7 @@ static int grpc_session_run_impl(tfsc_server* s, const void* req, size_t req_len
     memcpy(buf + prefix.size() + (size_t)on * 4, suffix.data(), suffix.size());
     return buf + prefix.size();
   };
-  rc = run_predict(s, node, remote, id, xdata, n, tv.dtype == TFSC_DT_INT32 ? TFSC_DT_INT32 : TFSC_DT_FLOAT, alloc, &err);
+  rc = run_predict_one(s, node, remote, id, xdata, n, tv.dtype == TFSC_DT_INT32 ? TFSC_DT_INT32 : TFSC_DT_FLOAT, alloc, &err);
   if (rc < 0) {
     free(buf);
     s->fail_grpc++;
@@ -843,9 +891,38 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
     std::vector<int64_t> shape;
     std::vector<float> flat;
     std::string input_key;
+    // several named inputs (multi-input models, e.g. BERT's input_ids / input_mask / segment_ids): one column per key
+    std::vector<std::pair<std::string, Json>> columns;
     bool ok = parsed && ((instances != nullptr) != (inputs != nullptr));
     if (parsed && !ok) err = "JSON body must contain exactly one of 'instances' (row format) or 'inputs' (columnar)";
-    if (ok && instances) {
+    if (ok && instances && instances->type == Json::Arr && !instances->arr.empty() && instances->arr[0].type == Json::Obj &&
+        instances->arr[0].obj.size() > 1) {
+      // row format, {"instances": [{"input_ids": [...], "input_mask": [...]}, ...]}: every instance names the same keys
+      for (auto& kv : instances->arr[0].obj) {
+        columns.emplace_back(kv.first, Json());
+        columns.back().second.type = Json::Arr;
+      }
+      for (auto& inst : instances->arr) {
+        if (inst.type != Json::Obj || inst.obj.size() != columns.size()) {
+          ok = false;
+          err = "every instance object must name the same inputs";
+          break;
+        }
+        for (auto& col : columns) {
+          const Json* v = inst.get(col.first);
+          if (!v) {
+            ok = false;
+            err = "every instance object must name the same inputs (one lacks '" + col.first + "')";
+            break;
+          }
+          col.second.arr.push_back(*v);
+        }
+        if (!ok) break;
+      }
+    } else if (ok && inputs && inputs->type == Json::Obj && inputs->obj.size() > 1) {
+      // columnar format, {"inputs": {"input_ids": [[...]], "input_mask": [[...]], ...}}
+      for (auto& kv : inputs->obj) columns.emplace_back(kv.first, kv.second);
+    } else if (ok && instances) {
       const Json* src = instances;
       Json unwrapped;
       // row format: a list of instances; an instance may be {"<input>": value}
@@ -876,7 +953,20 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
       }
       if (ok) ok = flatten(*src, 0, &shape, &flat, &err);
     }
-    if (!ok || flat.empty()) {
+    std::vector<std::vector<int64_t>> col_shape(columns.size());
+    std::vector<std::vector<int32_t>> col_ints(columns.size());
+    for (size_t i = 0; ok && i < columns.size(); ++i) {
+      std::vector<float> vals;
+      ok = flatten(columns[i].second, 0, &col_shape[i], &vals, &err);
+      if (ok && vals.empty()) {
+        ok = false;
+        err = "input '" + columns[i].first + "' is empty";
+      }
+      // JSON numbers carry no dtype: the inputs of a multi-input model are int32 (token ids, mask, segment ids)
+      col_ints[i].resize(vals.size());
+      for (size_t k = 0; k < vals.size(); ++k) col_ints[i][k] = (int32_t)llround((double)vals[k]);
+    }
+    if (!ok || (flat.empty() && columns.empty())) {
       std::string e2;
       rc = node ? node->fetch(id, nullptr, &e2) : 0;  // residency is ensured before the body is looked at
       if (rc < 0) return fail_http(http_for(rc), e2);
@@ -885,8 +975,18 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
     std::vector<float> y;
     std::vector<int64_t> oshape;
     std::string bad_sig;
+    std::vector<InTensor> ts(columns.size());
+    for (size_t i = 0; i < columns.size(); ++i) {
+      ts[i].name = columns[i].first;
+      ts[i].dtype = TFSC_DT_INT32;
+      ts[i].data = col_ints[i].data();
+      ts[i].shape = col_shape[i];
+      ts[i].n = (int64_t)col_ints[i].size();
+    }
+    const InputLayout layout = layout_inputs(&ts);
+    if (!ts.empty()) shape = ts[0].shape;  // the batch dimension of the response
     auto alloc = [&](const ModelDesc& d, int64_t rows) -> void* {
-      if (!input_key.empty() && input_key != d.input_name) {
+      if (d.inputs.empty() && !input_key.empty() && input_key != d.input_name) {
         bad_sig = "input '" + input_key + "' does not match the model signature (expects '" + d.input_name + "')";
         return nullptr;
       }
@@ -896,13 +996,14 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
       y.resize((size_t)on);
       return y.data();
     };
-    rc = run_predict(s, node, remote, id, flat.data(), (int64_t)flat.size(), TFSC_DT_FLOAT, alloc, &err);
-    if (rc == TFSC_E_INVALID && err.find("input dtype") == 0) {
+    if (!ts.empty()) rc = run_predict(s, node, remote, id, ts, layout, alloc, &err);
+    else rc = run_predict_one(s, node, remote, id, flat.data(), (int64_t)flat.size(), TFSC_DT_FLOAT, alloc, &err);
+    if (ts.empty() && rc == TFSC_E_INVALID && err.find("input dtype") == 0) {
       // JSON numbers carry no dtype: the signature wants int32 (token ids) -> resend the same values as integers
       std::vector<int32_t> ints(flat.size());
       for (size_t i = 0; i < flat.size(); ++i) ints[i] = (int32_t)llround((double)flat[i]);
       err.clear();
-      rc = run_predict(s, node, remote, id, ints.data(), (int64_t)ints.size(), TFSC_DT_INT32, alloc, &err);
+      rc = run_predict_one(s, node, remote, id, ints.data(), (int64_t)ints.size(), TFSC_DT_INT32, alloc, &err);
     }
     if (rc < 0) return fail_http(bad_sig.empty() ? http_for(rc) : 400, bad_sig.empty() ? err : bad_sig);
     // TF-Serving's writer: 4-space indent, arrays on one line, closing bracket on its own line
@@ -933,10 +1034,15 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
       t += "], \"unknown_rank\": false}, \"name\": \"" + key + ":0\"}";
       return t;
     };
+    // every declared input of a multi-input model is DT_INT32 [-1, S]
+    std::string ins;
+    for (auto& mi : d.inputs)
+      ins += (ins.empty() ? "" : ", ") + tensor_info(mi.name, std::to_string(d.in_dim / (int64_t)d.inputs.size()), "DT_INT32");
+    if (d.inputs.empty()) ins = tensor_info(d.input_name, dim, d.input_dtype == TFSC_DT_INT32 ? "DT_INT32" : "DT_FLOAT");
     std::string b = "{\n\"model_spec\": {\"name\": ";
     json_escape(name, &b);
     b += ", \"signature_name\": \"\", \"version\": \"" + std::to_string(id.version) + "\"},\n\"metadata\": {\"signature_def\": {\"signature_def\": {\"serving_default\": {\"inputs\": {" +
-         tensor_info(d.input_name, dim, d.input_dtype == TFSC_DT_INT32 ? "DT_INT32" : "DT_FLOAT") + "}, \"outputs\": {" +
+         ins + "}, \"outputs\": {" +
          tensor_info(d.output_name, odim, "DT_FLOAT") +
          "}, \"method_name\": \"tensorflow/serving/predict\"}}}}\n}\n";
     *http_status = 200;
@@ -1067,7 +1173,9 @@ struct tfsc_ticket {
   std::condition_variable cv;
   int remote_rc = 1;
   std::string remote_err;
-  std::vector<char> remote_x;
+  std::vector<std::vector<char>> remote_x;  // copies of the inputs, so the caller's buffers are free when submit returns
+  std::vector<InTensor> remote_ts;
+  InputLayout remote_l;
   bool delivered = false;
 };
 
@@ -1081,17 +1189,11 @@ static int submit_impl(tfsc_server* s, const char* model_name, const char* versi
   int remote = -1;
   int rc = resolve(s, model_name, version, &node, &id, &remote);
   if (rc < 0) return rc;
+  std::vector<InTensor> ts;
+  InputLayout layout;
+  if ((rc = abi_inputs(in, n_in, true, &ts, &layout)) < 0) return rc;
   const tfsc_tensor& x = in[0];
-  if (n_in != 1) return fail(TFSC_E_INVALID, "predict: the model templates take exactly one input tensor (got %d)", n_in);
-  if ((x.dtype != TFSC_DT_FLOAT && x.dtype != TFSC_DT_INT32) || x.rank < 0 || x.rank > 8)
-    return fail(TFSC_E_INVALID, "predict: input must be DT_FLOAT or DT_INT32, rank <= 8");
-  int64_t n = 1;
-  std::vector<int64_t> ishape(x.shape, x.shape + x.rank);
-  for (auto d : ishape) {
-    if (d < 0 || (d != 0 && n > ((int64_t)1 << 40) / d)) return fail(TFSC_E_INVALID, "predict: bad input shape");
-    n *= d;
-  }
-  if ((size_t)n * 4 != x.nbytes || !x.data) return fail(TFSC_E_INVALID, "predict: input nbytes does not match shape");
+  const std::vector<int64_t> ishape = ts[0].shape;
   auto t = std::make_unique<tfsc_ticket>();
   t->srv = s;
   t->node = node;
@@ -1099,15 +1201,20 @@ static int submit_impl(tfsc_server* s, const char* model_name, const char* versi
   std::string err;
   if (!node) {
     // another rank owns the model: the forward hop is synchronous, run it beside the caller
-    t->remote_x.assign((const char*)x.data, (const char*)x.data + x.nbytes);
+    for (auto& c : ts) {
+      const char* p = static_cast<const char*>(c.data);
+      t->remote_x.emplace_back(p, p + (size_t)c.n * 4);
+      c.data = t->remote_x.back().data();
+    }
+    t->remote_ts = ts;
+    t->remote_l = layout;
     tfsc_ticket* tp = t.get();
-    const int dtype = x.dtype;
     const std::string xname = x.name ? x.name : "";
     const bool has_name = x.name != nullptr;
-    t->remote_thread = std::thread([tp, s, remote, id, n, dtype, ishape, xname, has_name, deadline_ns] {
+    t->remote_thread = std::thread([tp, s, remote, id, ishape, xname, has_name, deadline_ns] {
       std::string e2, bad;
       auto alloc = [&](const ModelDesc& d, int64_t rows) -> void* {
-        if (has_name && d.input_name != xname) {
+        if (d.inputs.empty() && has_name && d.input_name != xname) {
           bad = "input '" + xname + "' does not match the model signature (expects '" + d.input_name + "')";
           return nullptr;
         }
@@ -1118,7 +1225,7 @@ static int submit_impl(tfsc_server* s, const char* model_name, const char* versi
         tp->out_bytes = (size_t)on * 4;
         return tp->out->data;
       };
-      int r = s->fwd->forward(remote, id.name, id.version, tp->remote_x.data(), n, dtype, alloc, nullptr, deadline_ns, &e2);
+      int r = s->fwd->forward(remote, id.name, id.version, tp->remote_ts, tp->remote_l, alloc, nullptr, deadline_ns, &e2);
       std::lock_guard<std::mutex> lk(tp->mu);
       tp->remote_rc = r < 0 && !bad.empty() ? TFSC_E_INVALID : r;
       tp->remote_err = !bad.empty() ? bad : e2;
@@ -1127,11 +1234,11 @@ static int submit_impl(tfsc_server* s, const char* model_name, const char* versi
     *ticket = t.release();
     return 0;
   }
-  rc = node->prepare(id, n, x.dtype, &t->req, nullptr, &err);
+  rc = node->prepare(id, layout, &t->req, nullptr, &err);
   if (rc < 0) return fail(rc, "%s", err.c_str());
   const ModelDesc& d = t->req.dm->desc;
   std::string bad;
-  if (x.name && d.input_name != x.name)
+  if (d.inputs.empty() && x.name && d.input_name != x.name)
     bad = "input '" + std::string(x.name) + "' does not match the model signature (expects '" + d.input_name + "')";
   if (bad.empty()) out_shape(d, t->req.rows, ishape, &t->oshape, &bad);
   if (!bad.empty()) {
@@ -1145,14 +1252,14 @@ static int submit_impl(tfsc_server* s, const char* model_name, const char* versi
     node->abandon(&t->req);
     return fail(TFSC_E_BUFFER, "output buffer too small");
   }
-  t->in_al = (x.nbytes + 255) & ~(size_t)255;
+  t->in_al = ((size_t)layout.n_elems * 4 + 255) & ~(size_t)255;
   t->staging_bytes = t->in_al + t->out_bytes;
   t->staging = static_cast<char*>(node->staging_alloc(t->staging_bytes));
   if (!t->staging) {
     node->abandon(&t->req);
     return fail(TFSC_E_EXHAUSTED, "cannot pin %zu bytes of request staging", t->staging_bytes);
   }
-  memcpy(t->staging, x.data, x.nbytes);
+  pack_rows(ts, layout, t->req.rows, t->staging);  // one tensor: the same bytes as a memcpy of it
   t->req.x = t->staging;
   t->req.y = t->staging + t->in_al;
   t->req.host_staged = true;
@@ -1397,15 +1504,37 @@ int tfsc_k_attention(const float* qkv, const int* ids, float* ctx, int batch, in
   const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;
   if (!qkv || !ctx || batch < 1 || (int64_t)batch * heads > 65535 || !attention_supported(seq, hidden, heads, al))
     return fail(TFSC_E_INVALID, "attention: no kernel for batch %d, seq %d, hidden %d, heads %d", batch, seq, hidden, heads);
-  cudaError_t e = launch_attention(qkv, ids, ctx, batch, seq, hidden, heads, (cudaStream_t)stream);
+  cudaError_t e = launch_attention(qkv, ids, seq, ctx, batch, seq, hidden, heads, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "attention: %s", cudaGetErrorString(e));
+}
+int tfsc_k_attention_mask(const float* qkv, const int* mask, int mask_stride, float* ctx, int batch, int seq, int hidden, int heads,
+                          void* stream) {
+  if (int rc = check_device()) return rc;
+  const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;
+  if (!qkv || !ctx || batch < 1 || (int64_t)batch * heads > 65535 || !attention_supported(seq, hidden, heads, al))
+    return fail(TFSC_E_INVALID, "attention_mask: no kernel for batch %d, seq %d, hidden %d, heads %d", batch, seq, hidden, heads);
+  if (mask && mask_stride < seq) return fail(TFSC_E_INVALID, "attention_mask: mask_stride %d is below seq %d", mask_stride, seq);
+  cudaError_t e = launch_attention(qkv, mask, mask_stride, ctx, batch, seq, hidden, heads, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "attention_mask: %s", cudaGetErrorString(e));
+}
+int tfsc_k_embed(const int* ids, const int* types, int stride, const float* word, const float* pos, const float* type,
+                 const float* gamma, const float* beta, float* y, int batch, int seq, int hidden, int vocab, float eps, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (!ids || !word || !pos || !type || !gamma || !beta || !y || batch < 0 || seq < 1 || vocab < 1 ||
+      (int64_t)batch * seq > 0x7fffffff || !layernorm_supported(hidden))
+    return fail(TFSC_E_INVALID, "embed: no kernel for batch %d, seq %d, hidden %d, vocab %d (hidden in 1..12272)", batch, seq, hidden,
+                vocab);
+  if (stride < seq) return fail(TFSC_E_INVALID, "embed: stride %d is below seq %d", stride, seq);
+  cudaError_t e = launch_layernorm(nullptr, nullptr, ids, types, stride, word, pos, type, gamma, beta, y, batch * seq, seq, hidden,
+                                   vocab, eps, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "embed: %s", cudaGetErrorString(e));
 }
 int tfsc_k_layernorm(const float* x, const float* res, const float* gamma, const float* beta, float* y, int tokens, int hidden,
                      float eps, void* stream) {
   if (int rc = check_device()) return rc;
   if (!x || !gamma || !beta || !y || tokens < 0 || !layernorm_supported(hidden))
     return fail(TFSC_E_INVALID, "layernorm: no kernel for %d tokens of hidden %d (hidden in 1..12272)", tokens, hidden);
-  cudaError_t e = launch_layernorm(x, res, nullptr, nullptr, nullptr, nullptr, gamma, beta, y, tokens, 1, hidden, 0, eps,
+  cudaError_t e = launch_layernorm(x, res, nullptr, nullptr, 0, nullptr, nullptr, nullptr, gamma, beta, y, tokens, 1, hidden, 0, eps,
                                    (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "layernorm: %s", cudaGetErrorString(e));
 }

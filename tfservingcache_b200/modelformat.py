@@ -57,7 +57,7 @@ def _write(version_dir: str, man: dict, blob: np.ndarray):
     blob.astype("<f4").tofile(os.path.join(version_dir, "weights.bin"))
 
 
-def _graph_manifest(input_shape, ops, n_buffers, input_name="x", output_name="y", input_dtype="float32"):
+def _graph_manifest(input_shape, ops, n_buffers, input_name="x", output_name="y", input_dtype="float32", inputs=None):
     off = 0
 
     def take(nbytes):
@@ -78,8 +78,11 @@ def _graph_manifest(input_shape, ops, n_buffers, input_name="x", output_name="y"
                 op["word_offset"] = take(op["vocab"] * op["c"] * 4)
                 op["pos_offset"] = take(op["max_pos"] * op["c"] * 4)
                 op["type_offset"] = take(2 * op["c"] * 4)
+    sig = {"input": input_name, "output": output_name}
+    if inputs is not None:   # several named inputs with roles: "inputs" replaces "input"
+        sig = {"inputs": [{"name": i["name"], "role": i["role"]} for i in inputs], "output": output_name}
     return {"format": "tfsc-b200-v1", "template": "graph", "dtype": "float32", "input_dtype": input_dtype,
-            "signature": {"input": input_name, "output": output_name}, "input_shape": list(input_shape),
+            "signature": sig, "input_shape": list(input_shape),
             "n_buffers": n_buffers, "ops": ops, "weights_bytes": off}
 
 
@@ -122,10 +125,21 @@ def write_graph_bundle(version_dir: str, manifest: dict, blob: np.ndarray):
     _write(version_dir, manifest, np.asarray(blob, np.float32))
 
 
-def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30522, max_pos=512, labels=2):
+BERT_INPUTS = [{"name": "input_ids", "role": "ids"}, {"name": "input_mask", "role": "mask"},
+               {"name": "segment_ids", "role": "type_ids"}]
+
+
+def packed_input_order(inputs):
+    """Names of `inputs` in the order their rows are concatenated in a request row: byte-wise sorted."""
+    return sorted((i["name"] for i in inputs), key=lambda n: n.encode())
+
+
+def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30522, max_pos=512, labels=2, inputs=None):
     """BERT-base fine-tune variant (Devlin et al. 2018) as a graph bundle: token ids int32 [B, seq] -> logits
-    [B, labels]. A sequence is an "image" with h = seq tokens, w = 1, c = width; dense layers are 1x1 convs; the
-    attention mask is derived from the ids ([PAD] = 0), token_type is 0.
+    [B, labels]. A sequence is an "image" with h = seq tokens, w = 1, c = width; dense layers are 1x1 convs.
+    With inputs=None the bundle takes the ids only: the attention mask is derived from them ([PAD] = 0), token_type is 0.
+    With inputs = a list of {"name", "role"} (roles "ids", "mask", "type_ids"; e.g. BERT_INPUTS) it declares those int32
+    [B, seq] inputs, and the kernels read the attention mask and the segment ids from the request.
     Buffers: 0 hidden, 1 qkv / ffn-intermediate, 2 context / post-attention, 3 dense output."""
     ops = [{"op": "embed", "src": -1, "dst": 0, "h": seq, "w": 1, "c": hidden, "vocab": vocab, "max_pos": max_pos, "eps": 1e-12}]
 
@@ -146,4 +160,4 @@ def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30
         ops.append({"op": "layernorm", "src": 3, "res": 2, "dst": 0, "h": seq, "w": 1, "c": hidden, "eps": 1e-12})
     ops.append({"op": "dense", "src": 0, "dst": 1, "h": 1, "w": 1, "c": hidden, "cout": hidden, "act": "tanh"})   # pooler on [CLS]
     ops.append({"op": "dense", "src": 1, "dst": -2, "h": 1, "w": 1, "c": hidden, "cout": labels, "act": "none"})
-    return _graph_manifest([seq], ops, 4, input_name="input_ids", output_name="logits", input_dtype="int32")
+    return _graph_manifest([seq], ops, 4, input_name="input_ids", output_name="logits", input_dtype="int32", inputs=inputs)

@@ -69,46 +69,39 @@ class Server:
     def host_models(self, node: int):
         return [(n, int(v), int(b)) for n, v, b, _p in self._lines(lib.tfsc_host_list, node)]
 
-    def predict(self, model_name: str, version: str, x: np.ndarray, out_capacity_elems: int | None = None,
+    def predict(self, model_name: str, version: str, x, out_capacity_elems: int | None = None,
                 input_name: str | None = None) -> np.ndarray:
-        is_int = np.issubdtype(np.asarray(x).dtype, np.integer)   # token-id inputs (BERT bundles) travel as DT_INT32
-        x = np.ascontiguousarray(x, dtype=np.int32 if is_int else np.float32)
-        tin = TfscTensor()
-        tin.name = input_name.encode() if input_name else None
-        tin.dtype = _lib.DT_INT32 if is_int else _lib.DT_FLOAT
-        tin.rank = x.ndim
-        for i, d in enumerate(x.shape):
-            tin.shape[i] = d
-        tin.data = x.ctypes.data
-        tin.nbytes = x.nbytes
-        cap = out_capacity_elems if out_capacity_elems is not None else max(x.size, 1) * 4 + 65536
-        y = np.empty(cap, dtype=np.float32)
-        tout = TfscTensor()
-        tout.data = y.ctypes.data
-        tout.nbytes = y.nbytes
-        check(lib.tfsc_predict(self._h, model_name.encode(), version.encode(), C.byref(tin), 1, C.byref(tout), 1),
+        """x: one array, or {name: array} for a model with several inputs (e.g. BERT's input_ids / input_mask /
+        segment_ids, int32 [batch, seq] each)."""
+        _x, tin, y, tout = self._tensors(x, out_capacity_elems, input_name)
+        check(lib.tfsc_predict(self._h, model_name.encode(), version.encode(), tin, len(tin), C.byref(tout), 1),
               "predict")
-        shape = tuple(tout.shape[i] for i in range(tout.rank))
-        n = int(np.prod(shape)) if shape else 1
-        return y[:n].reshape(shape).copy()
+        return self._result(y, tout)
 
-    def _tensors(self, x, out_capacity_elems, input_name):
-        is_int = np.issubdtype(np.asarray(x).dtype, np.integer)
-        x = np.ascontiguousarray(x, dtype=np.int32 if is_int else np.float32)
-        tin = TfscTensor()
-        tin.name = input_name.encode() if input_name else None
-        tin.dtype = _lib.DT_INT32 if is_int else _lib.DT_FLOAT
-        tin.rank = x.ndim
-        for i, d in enumerate(x.shape):
-            tin.shape[i] = d
-        tin.data = x.ctypes.data
-        tin.nbytes = x.nbytes
-        cap = out_capacity_elems if out_capacity_elems is not None else max(x.size, 1) * 4 + 65536
+    @staticmethod
+    def _tensors(x, out_capacity_elems, input_name):
+        """(the arrays kept alive, an array of input tensors, the output buffer, the output tensor). x is one array
+        (named input_name, or unnamed) or a {name: array} dict."""
+        items = list(x.items()) if isinstance(x, dict) else [(input_name, x)]
+        arrays, tin = [], (TfscTensor * len(items))()
+        for t, (name, a) in zip(tin, items):
+            is_int = np.issubdtype(np.asarray(a).dtype, np.integer)   # token-id inputs (BERT bundles) travel as DT_INT32
+            a = np.ascontiguousarray(a, dtype=np.int32 if is_int else np.float32)
+            arrays.append(a)
+            t.name = name.encode() if name else None
+            t.dtype = _lib.DT_INT32 if is_int else _lib.DT_FLOAT
+            t.rank = a.ndim
+            for i, d in enumerate(a.shape):
+                t.shape[i] = d
+            t.data = a.ctypes.data
+            t.nbytes = a.nbytes
+        size = sum(a.size for a in arrays)
+        cap = out_capacity_elems if out_capacity_elems is not None else max(size, 1) * 4 + 65536
         y = np.empty(cap, dtype=np.float32)
         tout = TfscTensor()
         tout.data = y.ctypes.data
         tout.nbytes = y.nbytes
-        return x, tin, y, tout
+        return arrays, tin, y, tout
 
     @staticmethod
     def _result(y, tout):
@@ -119,14 +112,14 @@ class Server:
     def predict_deadline(self, model_name: str, version: str, x: np.ndarray, deadline_ns: int, **kw) -> np.ndarray:
         """tfsc_predict_deadline: deadline is absolute on the clock of now_ns() (0 = none)."""
         _x, tin, y, tout = self._tensors(x, kw.get("out_capacity_elems"), kw.get("input_name"))
-        check(lib.tfsc_predict_deadline(self._h, model_name.encode(), version.encode(), C.byref(tin), 1, C.byref(tout), 1,
+        check(lib.tfsc_predict_deadline(self._h, model_name.encode(), version.encode(), tin, len(tin), C.byref(tout), 1,
                                         int(deadline_ns)), "predict")
         return self._result(y, tout)
 
     def predict_member(self, member: int, model_name: str, version: str, x: np.ndarray, deadline_ns: int = 0, **kw) -> np.ndarray:
         """tfsc_predict_member: the cache tier of member `member` (index into gpu.members), no ring lookup."""
         _x, tin, y, tout = self._tensors(x, kw.get("out_capacity_elems"), kw.get("input_name"))
-        check(lib.tfsc_predict_member(self._h, member, model_name.encode(), version.encode(), C.byref(tin), 1, C.byref(tout), 1,
+        check(lib.tfsc_predict_member(self._h, member, model_name.encode(), version.encode(), tin, len(tin), C.byref(tout), 1,
                                       int(deadline_ns)), "predict_member")
         return self._result(y, tout)
 
@@ -138,7 +131,7 @@ class Server:
         """Asynchronous Predict (tfsc_predict_submit): returns a Ticket; .wait() yields the result."""
         xk, tin, y, tout = self._tensors(x, kw.get("out_capacity_elems"), kw.get("input_name"))
         t = C.c_void_p()
-        check(lib.tfsc_predict_submit(self._h, model_name.encode(), version.encode(), C.byref(tin), 1, C.byref(tout), 1,
+        check(lib.tfsc_predict_submit(self._h, model_name.encode(), version.encode(), tin, len(tin), C.byref(tout), 1,
                                       int(deadline_ns), C.byref(t)), "predict_submit")
         return Ticket(t, y, tout)
 
