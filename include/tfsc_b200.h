@@ -134,6 +134,10 @@ int64_t tfsc_disk_model_size(const char* base_dir, const char* model_name, int64
  * TFSC_E_INVALID with the offending node in tfsc_last_error(). Needs no GPU. */
 int tfsc_savedmodel_convert(const char* version_dir, const char* out_dir);
 uint32_t tfsc_crc32c(const void* data, size_t len);   /* CRC-32C (Castagnoli), the tensor-bundle / table checksum */
+/* Checks a tfsc_model.json text with the rules the loader applies; needs no GPU. TFSC_E_INVALID with the loader's reason in
+ * tfsc_last_error(), or writes {"in_dim", "out_dim", "head_n", "head_k", "outputs": [{"name", "kind", "offset", "width",
+ * "dtype"}]} (the packed response row of signature.outputs, offsets and widths in 32-bit words) and returns its strlen. */
+int tfsc_manifest_check(const char* manifest_json, char* buf, size_t cap);
 
 /* ---------------------------------------------------------------- server (a6,a8,a10,X) ------
  * One server = the cache tier + proxy tier of cmd/taskhandler/main.go:45-113 for the GPUs of
@@ -202,7 +206,12 @@ int tfsc_host_list(tfsc_server* s, int node, char* buf, size_t cap);
  * declares signature.inputs (e.g. BERT: input_ids / input_mask / segment_ids) takes exactly those, each DT_INT32
  * [batch, seq] (or [seq]) with the same batch; a missing, extra or misnamed input, unequal batch sizes, a wrong per-row
  * size or a float tensor answer TFSC_E_INVALID naming the expected inputs (after the model is made resident, as every
- * input error; nothing is launched). The same holds for _deadline, _member and _submit. */
+ * input error; nothing is launched). The same holds for _deadline, _member and _submit.
+ * Outputs: a single-output model fills out[0] (DT_FLOAT; out[0].name is not looked at) and ignores out[1..n_out). A model
+ * whose manifest declares signature.outputs (logits, probabilities, classes, top_k_classes, top_k_probabilities) fills
+ * out[i] with the output named out[i].name, in the caller's order: dtype (DT_INT64 for classes, DT_INT32 for
+ * top_k_classes, DT_FLOAT otherwise), shape (batch dims, then [N], nothing or [k]) and nbytes. A NULL, unknown or repeated
+ * name is TFSC_E_INVALID and the message lists the outputs; a buffer too small for its output is TFSC_E_BUFFER. */
 int tfsc_predict(tfsc_server* s, const char* model_name, const char* version,
                  const tfsc_tensor* in, int n_in, tfsc_tensor* out, int n_out);
 /* tfsc_predict with a deadline (absolute, on the clock of tfsc_now_ns() = CLOCK_MONOTONIC; 0 = none): a request still
@@ -250,7 +259,11 @@ int tfsc_rest_handle(tfsc_server* s, const char* method, const char* url, const 
  * The model must have been made resident (tfsc_model_ensure); it is pinned for the launch.
  * x holds `rows` packed rows of the model's in_dim values. A multi-input model's row is the concatenation of its inputs'
  * rows (seq int32 values each) in byte-wise sorted NAME order, e.g. input_ids | input_mask | segment_ids: the ids of row r
- * are x[r*3*seq .. r*3*seq + seq). The kernels read the ids, the attention mask and the segment ids from there. */
+ * are x[r*3*seq .. r*3*seq + seq). The kernels read the ids, the attention mask and the segment ids from there.
+ * y receives `rows` packed rows the same way. A multi-output model's row is the concatenation of its outputs' rows in
+ * byte-wise sorted NAME order, in 32-bit words: logits / probabilities N floats, classes 2 words (the int64 index,
+ * little-endian), top_k_classes k int32, top_k_probabilities k floats; e.g. classes | logits | probabilities is 2 + 2N words
+ * per row, logits of row r at y + r*(2+2N) + 2. A single-output model's row is its out_dim floats. */
 int tfsc_predict_device(tfsc_server* s, int node, const char* model_name, int64_t version,
                         const void* x, int64_t rows, void* y, void* stream);
 int tfsc_node_sync(tfsc_server* s, int node);
@@ -347,6 +360,13 @@ int tfsc_k_embed(const int* ids, const int* types, int stride, const float* word
  * NULL; hidden in 1..12272. */
 int tfsc_k_layernorm(const float* x, const float* res, const float* gamma, const float* beta, float* y, int tokens, int hidden,
                      float eps, void* stream);
+/* Classification head of multi-output bundles, one launch for logits[rows, n] (fp32, device): probs[rows, n] = softmax
+ * (max-subtracted, fp32), classes[rows] = argmax (ties: lowest index), topk_idx[rows, k] = the k largest logits' indices in
+ * descending order (ties: lower index first, as tf.math.top_k), topk_prob[rows, k] = probs at those indices (the same bits).
+ * Selection compares the fp32 logits exactly. Every output pointer may be NULL (not written). Logits must be finite.
+ * TFSC_E_INVALID unless 1 <= n <= 32768 and 1 <= k <= min(n, 32). */
+int tfsc_k_classify_head(const float* logits, int rows, int n, int k, float* probs, int64_t* classes, int32_t* topk_idx,
+                         float* topk_prob, void* stream);
 
 #ifdef __cplusplus
 }

@@ -86,6 +86,7 @@ _sig("tfsc_disk_find_version_dir", C.c_int, cp, cp, i64, C.c_char_p, sz)
 _sig("tfsc_disk_model_size", i64, cp, cp, i64)
 _sig("tfsc_savedmodel_convert", C.c_int, cp, cp)
 _sig("tfsc_crc32c", C.c_uint32, vp, sz)
+_sig("tfsc_manifest_check", C.c_int, cp, C.c_char_p, sz)
 _sig("tfsc_server_create", vp, cp)
 _sig("tfsc_server_destroy", None, vp)
 _sig("tfsc_server_num_nodes", C.c_int, vp)
@@ -138,6 +139,7 @@ _sig("tfsc_k_attention", C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int
 _sig("tfsc_k_attention_mask", C.c_int, vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp)
 _sig("tfsc_k_embed", C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp)
 _sig("tfsc_k_layernorm", C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_float, vp)
+_sig("tfsc_k_classify_head", C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp)
 
 
 class TfscError(RuntimeError):

@@ -149,6 +149,13 @@ void write_sig(Writer* w, const FwdSignature& s) {
     w->str(s.input_names[i]);
     w->i32(s.input_roles[i]);
   }
+  w->u32((uint32_t)s.output_names.size());
+  for (size_t i = 0; i < s.output_names.size(); ++i) {
+    w->str(s.output_names[i]);
+    w->i32(s.output_kinds[i]);
+  }
+  w->i32(s.head_n);
+  w->i32(s.head_k);
 }
 
 FwdSignature read_sig(Reader* r) {
@@ -167,6 +174,16 @@ FwdSignature read_sig(Reader* r) {
     s.input_names.push_back(r->str());
     s.input_roles.push_back(r->i32());
   }
+  const uint32_t m = r->u32();
+  if (m > (uint32_t)kMaxOutputs) r->ok = false;
+  for (uint32_t i = 0; r->ok && i < m; ++i) {
+    s.output_names.push_back(r->str());
+    const int32_t kind = r->i32();
+    if (kind < 0 || kind > (int32_t)OutputKind::TopKProbabilities) r->ok = false;
+    s.output_kinds.push_back(kind);
+  }
+  s.head_n = r->i32();
+  s.head_k = r->i32();
   return s;
 }
 
@@ -222,6 +239,21 @@ void FwdSignature::to_desc(ModelDesc* d) const {
   const int64_t S = input_names.empty() ? 0 : in_dim / (int64_t)input_names.size();
   for (size_t i = 0; i < input_names.size(); ++i)
     d->inputs.push_back({input_names[i], (InputRole)input_roles[i], (int64_t)i * S});
+  // the ingress rank splits the packed response rows with the owner's layout rule (layout_outputs), never with its own manifest
+  d->outputs.clear();
+  d->head_n = head_n;
+  d->head_k = head_k;
+  for (size_t i = 0; i < output_names.size(); ++i) {
+    ModelOutput o;
+    o.name = output_names[i];
+    o.kind = (OutputKind)output_kinds[i];
+    d->outputs.push_back(o);
+  }
+  std::string err;
+  if (!d->outputs.empty() && !layout_outputs(d, &err)) {  // unusable: no front-end can size a response for 0 words per row
+    d->outputs.clear();
+    d->out_dim = 0;
+  }
 }
 
 FwdSignature FwdSignature::from_desc(const ModelDesc& d) {
@@ -238,6 +270,12 @@ FwdSignature FwdSignature::from_desc(const ModelDesc& d) {
     s.input_names.push_back(mi.name);
     s.input_roles.push_back((int32_t)mi.role);
   }
+  for (auto& mo : d.outputs) {
+    s.output_names.push_back(mo.name);
+    s.output_kinds.push_back((int32_t)mo.kind);
+  }
+  s.head_n = d.head_n;
+  s.head_k = d.head_k;
   return s;
 }
 

@@ -53,6 +53,9 @@ struct FwdSignature {
   std::vector<int64_t> input_shape, output_shape;
   std::vector<std::string> input_names;  // signature.inputs in packed order (empty: single-input model)
   std::vector<int32_t> input_roles;
+  std::vector<std::string> output_names;  // signature.outputs in packed order (empty: single-output model)
+  std::vector<int32_t> output_kinds;
+  int32_t head_n = 0, head_k = 0;
   void to_desc(ModelDesc* d) const;
   static FwdSignature from_desc(const ModelDesc& d);
 };

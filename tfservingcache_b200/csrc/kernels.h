@@ -57,6 +57,25 @@ cudaError_t launch_layernorm(const float* x, const float* res, const int* ids, c
 cudaError_t launch_attention(const float* qkv, const int* mask, int mask_stride, float* ctx, int Bn, int S, int H, int heads,
                              cudaStream_t s);
 
+// Classification head (head.cu): from logits[rows, n] writes, for each non-null pointer, row r of that output at
+// ptr + r * ld (ld in 32-bit words): a copy of the logits [n], softmax probabilities [n], the argmax class as a
+// little-endian int64 (two words: index, 0), the top k indices [k] (descending logit, ties to the lower index) and their
+// probabilities [k] (the same bits as probabilities[index]). k counts only when a top-k pointer is set.
+// cudaErrorInvalidValue outside head_supported (nn_limits.h).
+struct HeadOutputs {
+  float* logits = nullptr;
+  int64_t logits_ld = 0;
+  float* probs = nullptr;
+  int64_t probs_ld = 0;
+  int* classes = nullptr;
+  int64_t classes_ld = 0;
+  int* topk_idx = nullptr;
+  int64_t topk_idx_ld = 0;
+  float* topk_prob = nullptr;
+  int64_t topk_prob_ld = 0;
+};
+cudaError_t launch_classify_head(const float* logits, int rows, int n, int k, const HeadOutputs& o, cudaStream_t s);
+
 // wgmma 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
 bool gemm_tc_supported(const float* A, const float* B, const float* bias, const float* R, const float* C, int M, int N, int K,
                        int lda);

@@ -9,12 +9,64 @@ namespace tfsc {
 static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 size_t ModelDesc::scratch_bytes(int64_t rows) const {
+  // an mlp's head reads the last layer's logits from the activation buffer that layer would have used, so only graph
+  // bundles with outputs need more: rows * head_n floats after the buffers and the im2col matrix
   if (tmpl == Template::Mlp) return 2 * (((size_t)rows * (size_t)(max_width > 0 ? max_width : 1) * 4 + 255) & ~(size_t)255);
-  if (tmpl == Template::Graph) return (size_t)n_buffers * graph_buf_bytes(rows) + align256((size_t)rows * (size_t)col_elems * 4);
+  if (tmpl == Template::Graph)
+    return head_scratch_offset(rows) + (outputs.empty() ? 0 : align256((size_t)rows * (size_t)head_n * 4));
   return 256;
 }
 
 size_t ModelDesc::graph_buf_bytes(int64_t rows) const { return align256((size_t)rows * (size_t)buf_elems * 4); }
+
+size_t ModelDesc::head_scratch_offset(int64_t rows) const {
+  return (size_t)n_buffers * graph_buf_bytes(rows) + align256((size_t)rows * (size_t)col_elems * 4);
+}
+
+const char* output_kind_name(OutputKind k) {
+  switch (k) {
+    case OutputKind::Logits: return "logits";
+    case OutputKind::Probabilities: return "probabilities";
+    case OutputKind::Classes: return "classes";
+    case OutputKind::TopKClasses: return "top_k_classes";
+    default: return "top_k_probabilities";
+  }
+}
+
+int output_dtype(OutputKind k) {
+  return k == OutputKind::Classes ? TFSC_DT_INT64 : k == OutputKind::TopKClasses ? TFSC_DT_INT32 : TFSC_DT_FLOAT;
+}
+
+bool layout_outputs(ModelDesc* d, std::string* err) {
+  const bool topk = d->output(OutputKind::TopKClasses) || d->output(OutputKind::TopKProbabilities);
+  if (!head_supported(d->head_n, topk ? d->head_k : 1) || (!topk && d->head_k != 0)) {
+    *err = "signature.outputs: no head kernel for " + std::to_string(d->head_n) + " logits and k = " + std::to_string(d->head_k) +
+           " (1 <= N <= " + std::to_string(kHeadMaxN) + ", 1 <= k <= min(N, " + std::to_string(kHeadMaxK) + "))";
+    return false;
+  }
+  // the packed row holds the outputs in byte-wise name order, so a rank can split a response without the manifest
+  std::sort(d->outputs.begin(), d->outputs.end(), [](const ModelOutput& a, const ModelOutput& b) { return a.name < b.name; });
+  int64_t off = 0;
+  for (auto& o : d->outputs) {
+    o.offset = off;
+    o.width = o.kind == OutputKind::Classes ? 2 : (o.kind == OutputKind::TopKClasses || o.kind == OutputKind::TopKProbabilities)
+                                                      ? d->head_k
+                                                      : d->head_n;
+    off += o.width;
+  }
+  d->out_dim = off;
+  return true;
+}
+
+std::string expected_outputs(const ModelDesc& d) {
+  std::string s;
+  for (auto& o : d.outputs) {
+    if (!s.empty()) s += ", ";
+    const int dt = output_dtype(o.kind);
+    s += "'" + o.name + "' (" + (dt == TFSC_DT_INT64 ? "int64" : dt == TFSC_DT_INT32 ? "int32" : "float") + ")";
+  }
+  return s;
+}
 
 static void finish(ModelDesc* d) {
   if (d->tmpl == Template::Graph) {
@@ -123,6 +175,54 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       // the packed row holds the inputs in byte-wise name order, so a rank can pack a request without the manifest
       std::sort(d->inputs.begin(), d->inputs.end(), [](const ModelInput& a, const ModelInput& b) { return a.name < b.name; });
       d->input_name = d->input(InputRole::Ids)->name;
+    }
+    if (const Json* outs = sig->get("outputs")) {
+      if (sig->get("output")) {
+        *err = "signature: 'outputs' and 'output' are mutually exclusive";
+        return false;
+      }
+      if (outs->type != Json::Arr || outs->arr.empty() || outs->arr.size() > (size_t)kMaxOutputs) {
+        *err = "signature.outputs must list 1 to " + std::to_string(kMaxOutputs) + " outputs";
+        return false;
+      }
+      int k = -1;
+      for (auto& oj : outs->arr) {
+        ModelOutput mo;
+        mo.name = oj.type == Json::Obj ? oj.get_str("name", "") : "";
+        const std::string kind = oj.type == Json::Obj ? oj.get_str("kind", "") : "";
+        if (kind == "logits") mo.kind = OutputKind::Logits;
+        else if (kind == "probabilities") mo.kind = OutputKind::Probabilities;
+        else if (kind == "classes") mo.kind = OutputKind::Classes;
+        else if (kind == "top_k_classes") mo.kind = OutputKind::TopKClasses;
+        else if (kind == "top_k_probabilities") mo.kind = OutputKind::TopKProbabilities;
+        else {
+          *err = "signature.outputs: unknown kind '" + kind + "' (logits, probabilities, classes, top_k_classes, top_k_probabilities)";
+          return false;
+        }
+        if (mo.name.empty()) {
+          *err = "signature.outputs: every output needs a name";
+          return false;
+        }
+        for (auto& o : d->outputs)
+          if (o.name == mo.name || o.kind == mo.kind) {
+            *err = "signature.outputs: duplicate " + std::string(o.name == mo.name ? "name '" + mo.name + "'" : "kind '" + kind + "'");
+            return false;
+          }
+        const bool topk = mo.kind == OutputKind::TopKClasses || mo.kind == OutputKind::TopKProbabilities;
+        if (topk) {
+          const Json* kj = oj.get("k");
+          if (!kj || kj->type != Json::Num || kj->num != (double)(int)kj->num || (k >= 0 && (int)kj->num != k)) {
+            *err = "signature.outputs: '" + mo.name + "' needs an integer 'k', the same for both top-k outputs";
+            return false;
+          }
+          k = (int)kj->num;
+        } else if (oj.get("k")) {
+          *err = "signature.outputs: 'k' belongs to the top-k outputs only ('" + mo.name + "' is " + kind + ")";
+          return false;
+        }
+        d->outputs.push_back(mo);
+      }
+      d->head_k = k < 0 ? 0 : k;
     }
   }
   if (const Json* ex = j.get("extra_signatures")) {
@@ -347,8 +447,56 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
     for (size_t i = 0; i < d->inputs.size(); ++i) d->inputs[i].offset = (int64_t)i * S;
   }
   finish(d);
+  if (!d->outputs.empty()) {
+    if (d->tmpl == Template::Affine) {
+      *err = "signature.outputs needs an mlp or graph bundle (an affine bundle has no logits row)";
+      return false;
+    }
+    if (d->tmpl == Template::Graph && d->output_shape.size() != 1) {
+      *err = "signature.outputs needs a graph whose output is one vector of logits per row (output_shape has rank " +
+             std::to_string(d->output_shape.size()) + ")";
+      return false;
+    }
+    for (auto& o : d->outputs) {
+      bool clash = d->inputs.empty() && o.name == d->input_name;
+      for (auto& i : d->inputs) clash = clash || o.name == i.name;
+      if (clash) {
+        *err = "signature.outputs: '" + o.name + "' is also an input name";
+        return false;
+      }
+    }
+    d->head_n = d->out_dim > 0x7fffffff ? 0 : (int)d->out_dim;  // the last op's per-row width
+    if (!layout_outputs(d, err)) return false;
+  }
   return true;
 }
+
+}  // namespace tfsc
+
+// Offline manifest check (no device): the loader's verdict on a tfsc_model.json and the packed row layout it derives.
+extern "C" int tfsc_manifest_check(const char* manifest_json, char* buf, size_t cap) {
+  using namespace tfsc;
+  Json j;
+  ModelDesc d;
+  std::string err;
+  if (!manifest_json || !json_parse(manifest_json, &j, &err) || !parse_manifest(j, &d, &err))
+    return fail(TFSC_E_INVALID, "%s", err.empty() ? "manifest_check: no manifest" : err.c_str());
+  std::string s = "{\"in_dim\": " + std::to_string(d.in_dim) + ", \"out_dim\": " + std::to_string(d.out_dim) +
+                  ", \"head_n\": " + std::to_string(d.head_n) + ", \"head_k\": " + std::to_string(d.head_k) + ", \"outputs\": [";
+  for (size_t i = 0; i < d.outputs.size(); ++i) {
+    const ModelOutput& o = d.outputs[i];
+    const int dt = output_dtype(o.kind);
+    s += i ? ", {\"name\": " : "{\"name\": ";
+    json_escape(o.name, &s);
+    s += ", \"kind\": \"" + std::string(output_kind_name(o.kind)) + "\", \"offset\": " + std::to_string(o.offset) +
+         ", \"width\": " + std::to_string(o.width) + ", \"dtype\": \"" +
+         (dt == TFSC_DT_INT64 ? "int64" : dt == TFSC_DT_INT32 ? "int32" : "float32") + "\"}";
+  }
+  s += "]}";
+  return copy_out(s, buf, cap);
+}
+
+namespace tfsc {
 
 std::string manifest_json(const ModelDesc& d) {
   std::string s = "{\"format\":\"tfsc-b200-v1\",\"dtype\":\"float32\",\"signature\":{\"input\":";

@@ -54,6 +54,20 @@ struct ModelInput {
   int64_t offset = 0;  // elements into the packed request row (inputs in byte-wise sorted name order, S values each)
 };
 
+// One declared output of a multi-output bundle (signature.outputs), computed from the last op's N logits by the head kernel
+// (head.cu). Per row: logits / probabilities [N] float, classes a scalar int64 (two 32-bit words, little-endian),
+// top_k_classes [k] int32, top_k_probabilities [k] float.
+enum class OutputKind { Logits, Probabilities, Classes, TopKClasses, TopKProbabilities };
+struct ModelOutput {
+  std::string name;
+  OutputKind kind = OutputKind::Logits;
+  int64_t offset = 0;  // elements (32-bit words) into the packed response row (outputs in byte-wise sorted name order)
+  int64_t width = 0;   // words per row: N, N, 2, k, k
+};
+const char* output_kind_name(OutputKind k);
+int output_dtype(OutputKind k);  // TFSC_DT_FLOAT / TFSC_DT_INT64 / TFSC_DT_INT32
+constexpr int kMaxOutputs = 5;
+
 struct ModelDesc {
   Template tmpl = Template::Mlp;
   std::vector<ExtraSignature> extra_sigs;
@@ -79,12 +93,34 @@ struct ModelDesc {
       if (i.role == r) return &i;
     return nullptr;
   }
+  // signature.outputs, sorted by name (= packed response row order); empty for single-output bundles (output_name, out_dim
+  // elements). With outputs, out_dim is the packed row width and head_n / head_k the logits width and top-k (0: none).
+  std::vector<ModelOutput> outputs;
+  int head_n = 0, head_k = 0;
+  const ModelOutput* output(OutputKind k) const {
+    for (auto& o : outputs)
+      if (o.kind == k) return &o;
+    return nullptr;
+  }
+  const ModelOutput* output(const std::string& name) const {
+    for (auto& o : outputs)
+      if (o.name == name) return &o;
+    return nullptr;
+  }
   // bytes of executor scratch (activation buffers + im2col) for `rows` images / batch rows
   size_t scratch_bytes(int64_t rows) const;
   // stride of the graph activation buffers in that scratch: rounded up to 256 bytes, so every buffer (and the im2col
   // matrix after them) starts 256-byte aligned whatever rows * buf_elems is
   size_t graph_buf_bytes(int64_t rows) const;
+  // offset of the head's logits in that scratch (graph bundles with outputs: after the buffers and the im2col matrix)
+  size_t head_scratch_offset(int64_t rows) const;
 };
+
+// Sort d->outputs by name, set their offsets and widths from d->head_n / d->head_k and d->out_dim to the packed row width.
+// Fails on a shape the head kernel cannot run (head_supported).
+bool layout_outputs(ModelDesc* d, std::string* err);
+// "'classes' (int64), 'logits' (float), ..." for error messages
+std::string expected_outputs(const ModelDesc& d);
 
 bool parse_manifest(const Json& j, ModelDesc* d, std::string* err);
 ModelDesc make_mlp_desc(const std::vector<int>& dims, const std::vector<std::string>& activations);

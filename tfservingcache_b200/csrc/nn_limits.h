@@ -26,4 +26,9 @@ inline bool attention_supported(int S, int H, int heads, bool aligned16) {
 // kernel gets without opting in: H <= 12272
 inline bool layernorm_supported(int H) { return H >= 1 && (size_t)H * sizeof(float) + 64 <= 48 * 1024; }
 
+// Classification head (head.cu): one CTA stages a row of N logits in shared memory (128 KB at N = 32768, a BERT-vocab head
+// of 30522 fits) and selects the top k of them by k block-wide argmax rounds. A head without top-k outputs runs as k = 1.
+constexpr int kHeadMaxN = 32768, kHeadMaxK = 32;
+inline bool head_supported(int N, int k) { return N >= 1 && N <= kHeadMaxN && k >= 1 && k <= kHeadMaxK && k <= N; }
+
 }  // namespace tfsc

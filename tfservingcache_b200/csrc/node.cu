@@ -592,6 +592,24 @@ static bool conv_tc_enabled() {  // TFSC_CONV_TC=0: explicit im2col + GEMM (the 
   return v;
 }
 
+// multi-output bundles: one head launch writes every declared output of a row at its offset in the packed row (out_dim words)
+static cudaError_t run_head(const ModelDesc& d, const float* logits, int64_t rows, char* y, cudaStream_t st) {
+  HeadOutputs o;
+  float* yf = reinterpret_cast<float*>(y);
+  const int64_t ld = d.out_dim;
+  for (const ModelOutput& m : d.outputs) {
+    float* p = yf + m.offset;
+    switch (m.kind) {
+      case OutputKind::Logits: o.logits = p, o.logits_ld = ld; break;
+      case OutputKind::Probabilities: o.probs = p, o.probs_ld = ld; break;
+      case OutputKind::Classes: o.classes = reinterpret_cast<int*>(p), o.classes_ld = ld; break;
+      case OutputKind::TopKClasses: o.topk_idx = reinterpret_cast<int*>(p), o.topk_idx_ld = ld; break;
+      case OutputKind::TopKProbabilities: o.topk_prob = p, o.topk_prob_ld = ld; break;
+    }
+  }
+  return launch_classify_head(logits, (int)rows, d.head_n, d.head_k, o, st);
+}
+
 cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, char* y, char* scratch, void* ws,
                             size_t ws_cap, cudaStream_t st) {
   const ModelDesc& d = dm.desc;
@@ -604,7 +622,9 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
     // residual / ReLU epilogue (BN is folded into the kernel + bias when the bundle is written)
     const size_t buf_bytes = d.graph_buf_bytes(rows);  // 256-byte aligned buffers: the loader's kernel checks rely on it
     char* col = scratch + (size_t)d.n_buffers * buf_bytes;
-    auto buf = [&](int i) -> char* { return i == -1 ? const_cast<char*>(x) : i == -2 ? y : scratch + (size_t)i * buf_bytes; };
+    // with signature.outputs the op that writes the response (-2) writes the logits to scratch, and the head writes y
+    char* out = d.outputs.empty() ? y : scratch + d.head_scratch_offset(rows);
+    auto buf = [&](int i) -> char* { return i == -1 ? const_cast<char*>(x) : i == -2 ? out : scratch + (size_t)i * buf_bytes; };
     const int B = (int)rows;
     // token-id inputs: single-input bundles read ids [B, S] and derive the attention mask from them ([PAD] = 0, stride S);
     // multi-input bundles read each declared input at its offset in the packed row, stride in_dim (inputs.h)
@@ -669,20 +689,21 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
       }
       if (e != cudaSuccess) return e;
     }
-    return cudaSuccess;
+    return d.outputs.empty() ? cudaSuccess : run_head(d, (const float*)out, rows, y, st);
   }
   char* act0 = scratch;
   char* act1 = scratch + d.scratch_bytes(rows) / 2;
   const char* in = x;
   for (size_t l = 0; l < d.layers.size(); ++l) {
     const DenseLayer& L = d.layers[l];
-    char* out = (l + 1 == d.layers.size()) ? y : ((l & 1) ? act1 : act0);
+    // with signature.outputs the last layer writes its logits to the next activation buffer, and the head writes y
+    char* out = (l + 1 == d.layers.size() && d.outputs.empty()) ? y : ((l & 1) ? act1 : act0);
     cudaError_t e = launch_dense((const float*)in, (const float*)(dm.dptr + L.w_off), (const float*)(dm.dptr + L.b_off),
                                  (float*)out, (int)rows, L.in, L.out, L.relu, ws, ws_cap, st);
     if (e != cudaSuccess) return e;
     in = out;
   }
-  return cudaSuccess;
+  return d.outputs.empty() ? cudaSuccess : run_head(d, (const float*)in, rows, y, st);
 }
 
 size_t Node::row_in_bytes(const ModelDesc& d) { return d.tmpl == Template::Affine ? 4 : (size_t)d.in_dim * 4; }

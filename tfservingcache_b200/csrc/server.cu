@@ -417,6 +417,122 @@ static bool out_shape(const ModelDesc& d, int64_t rows, const std::vector<int64_
   return true;
 }
 
+// ---- multi-output models (signature.outputs): the executor writes packed rows (model.h); every front-end cuts the
+// outputs it serves out of them with the same rule, for local and forwarded requests alike.
+
+// The selected outputs of one response, in the order they are answered, with their full shapes (batch dims + per row).
+struct OutputPlan {
+  std::vector<ModelOutput> sel;
+  std::vector<std::vector<int64_t>> shapes;
+  int64_t out_dim = 0, rows = 0;
+};
+
+static int64_t product(const std::vector<int64_t>& v) {
+  int64_t n = 1;
+  for (auto x : v) n *= x;
+  return n;
+}
+
+// The batch dims of a request with input shape `in_shape` that runs as `rows` rows, by the rule out_shape applies to a
+// single output: a graph keeps what precedes the per-image input shape, an mlp the leading dims of the input.
+static bool batch_dims(const ModelDesc& d, int64_t rows, const std::vector<int64_t>& in_shape, std::vector<int64_t>* dims,
+                       std::string* why) {
+  dims->clear();
+  if (d.tmpl == Template::Graph) {
+    if (in_shape.size() > d.input_shape.size())
+      for (size_t i = 0; i + d.input_shape.size() < in_shape.size(); ++i) dims->push_back(in_shape[i]);
+  } else if (in_shape.size() <= 1) {
+    if (rows != 1 || in_shape.empty()) dims->push_back(rows);
+  } else {
+    for (size_t i = 0; i + 1 < in_shape.size(); ++i) dims->push_back(in_shape[i]);
+  }
+  int64_t on = 1;
+  for (auto v : *dims) {
+    if (v < 0 || (v != 0 && on > ((int64_t)1 << 40) / v)) return false;
+    on *= v;
+  }
+  if (on != rows) {
+    std::string sh = "[";
+    for (size_t i = 0; i < in_shape.size(); ++i) sh += (i ? "," : "") + std::to_string(in_shape[i]);
+    *why = "input shape " + sh + "] does not match the model signature: the trailing dimensions must hold exactly " +
+           std::to_string(d.in_dim) + " elements per row";
+    return false;
+  }
+  return true;
+}
+
+// `names` (empty = every output, in packed order) must name declared outputs, each once
+static bool plan_outputs(const ModelDesc& d, int64_t rows, const std::vector<int64_t>& in_shape, const std::vector<std::string>& names,
+                         OutputPlan* p, std::string* why) {
+  std::vector<int64_t> dims;
+  if (!batch_dims(d, rows, in_shape, &dims, why)) return false;
+  p->sel.clear();
+  p->shapes.clear();
+  p->out_dim = d.out_dim;
+  p->rows = rows;
+  std::vector<std::string> want = names;
+  if (want.empty())
+    for (auto& o : d.outputs) want.push_back(o.name);
+  for (size_t i = 0; i < want.size(); ++i) {
+    const ModelOutput* o = d.output(want[i]);
+    for (size_t j = 0; o && j < i; ++j)
+      if (want[j] == want[i]) {
+        *why = "output '" + want[i] + "' is requested twice; model outputs: " + expected_outputs(d);
+        return false;
+      }
+    if (!o) {
+      *why = "unknown output '" + want[i] + "'; model outputs: " + expected_outputs(d);
+      return false;
+    }
+    p->sel.push_back(*o);
+    std::vector<int64_t> sh = dims;
+    if (o->kind != OutputKind::Classes) sh.push_back(o->kind == OutputKind::Logits || o->kind == OutputKind::Probabilities ? d.head_n : d.head_k);
+    p->shapes.push_back(sh);
+  }
+  return true;
+}
+
+// the values of output i of the plan, cut out of `rows` packed rows (fp32 and int32: one word each, int64: two)
+static void split_output(const OutputPlan& p, size_t i, const void* packed, void* dst) {
+  const ModelOutput& o = p.sel[i];
+  const char* src = static_cast<const char*>(packed);
+  char* out = static_cast<char*>(dst);
+  for (int64_t r = 0; r < p.rows; ++r)
+    memcpy(out + (size_t)(r * o.width) * 4, src + (size_t)(r * p.out_dim + o.offset) * 4, (size_t)o.width * 4);
+}
+
+static std::string dtype_name(int dt) { return dt == TFSC_DT_INT64 ? "DT_INT64" : dt == TFSC_DT_INT32 ? "DT_INT32" : "DT_FLOAT"; }
+
+// C ABI, multi-output model: out[i].name selects the outputs (any order, no repeats); checks that every caller buffer
+// holds its output and returns the packed staging rows for the executor (nullptr + *bad, or nullptr alone: buffer too small)
+static void* abi_outputs_alloc(const ModelDesc& d, int64_t rows, const std::vector<int64_t>& in_shape, const tfsc_tensor* out,
+                               int n_out, OutputPlan* plan, std::vector<float>* packed, std::string* bad) {
+  std::vector<std::string> names;
+  for (int i = 0; i < n_out; ++i) {
+    if (!out[i].name) {
+      *bad = "predict: the model has several outputs, every out[i].name must name one of " + expected_outputs(d);
+      return nullptr;
+    }
+    names.push_back(out[i].name);
+  }
+  if (!plan_outputs(d, rows, in_shape, names, plan, bad)) return nullptr;
+  for (size_t i = 0; i < plan->sel.size(); ++i)
+    if (!out[i].data || out[i].nbytes < (size_t)(rows * plan->sel[i].width) * 4 || plan->shapes[i].size() > 8) return nullptr;
+  packed->assign((size_t)(rows * d.out_dim), 0.f);
+  return packed->data();
+}
+
+// fills out[i] (data, dtype, shape, nbytes) for every output of the plan; nothing for a single-output model (empty plan)
+static void abi_outputs_deliver(const OutputPlan& plan, const void* packed, tfsc_tensor* out) {
+  for (size_t i = 0; i < plan.sel.size(); ++i) {
+    split_output(plan, i, packed, out[i].data);
+    out[i].dtype = output_dtype(plan.sel[i].kind);
+    out[i].rank = (int32_t)plan.shapes[i].size();
+    for (size_t j = 0; j < plan.shapes[i].size(); ++j) out[i].shape[j] = plan.shapes[i][j];
+    out[i].nbytes = (size_t)(plan.rows * plan.sel[i].width) * 4;
+  }
+}
+
 // owner = member `member` of the current member list (the cache tier of that member, cachemanager.ServeRest/ServeGrpc: no
 // ring lookup -- the caller already routed, e.g. with tfsc_route), local node or another rank
 static int resolve_member(tfsc_server* s, int member, const std::string& name, const std::string& version, Node** node,
@@ -455,11 +571,14 @@ static int predict_impl(tfsc_server* s, const char* model_name, const char* vers
   const std::vector<int64_t>& ishape = ts[0].shape;
   std::string err, bad;
   tfsc_tensor* o = &out[0];
+  OutputPlan plan;
+  std::vector<float> packed;
   auto alloc = [&](const ModelDesc& d, int64_t rows) -> void* {
     if (d.inputs.empty() && x.name && d.input_name != x.name) {  // signature check of a single-input model
       bad = "input '" + std::string(x.name) + "' does not match the model signature (expects '" + d.input_name + "')";
       return nullptr;
     }
+    if (!d.outputs.empty()) return abi_outputs_alloc(d, rows, ishape, out, n_out, &plan, &packed, &bad);
     std::vector<int64_t> sh;
     if (!out_shape(d, rows, ishape, &sh, &bad)) return nullptr;
     int64_t on = 1;
@@ -474,8 +593,11 @@ static int predict_impl(tfsc_server* s, const char* model_name, const char* vers
   rc = run_predict(s, node, remote, id, ts, layout, alloc, &err, deadline_ns);
   if (rc < 0 && !bad.empty()) return fail(TFSC_E_INVALID, "%s", bad.c_str());
   if (rc < 0) return fail(rc, "%s", err.c_str());
+  abi_outputs_deliver(plan, packed.data(), out);
   return 0;
 }
+
+static void set_resp_bytes(const std::string& body, void** resp, size_t* resp_len);
 
 static int grpc_predict_impl(tfsc_server* s, const void* req, size_t req_len, void** resp, size_t* resp_len) {
   if (!s || !req || !resp || !resp_len) return fail(TFSC_E_INVALID, "grpc_predict: bad arguments");
@@ -530,10 +652,32 @@ static int grpc_predict_impl(tfsc_server* s, const void* req, size_t req_len, vo
   char* buf = nullptr;
   size_t total = 0;
   std::string bad_sig;
+  OutputPlan plan;
+  std::vector<float> packed;
   auto alloc = [&](const ModelDesc& d, int64_t rows) -> void* {
     if (d.inputs.empty() && (n_in != 1 || tv.name != d.input_name)) {
       bad_sig = "input keys do not match the model signature (expects '" + d.input_name + "')";
       return nullptr;
+    }
+    if (!d.outputs.empty()) {
+      // output_filter selects outputs (empty: all); the response map lists them in sorted name order. The two messages follow
+      // TF-Serving's predict_util.cc as far as they are known (wording unverified against its source).
+      std::set<std::string> sel;
+      for (auto& a : view.output_filter) {
+        if (!d.output(a)) {
+          std::string set;
+          for (auto& o : d.outputs) set += (set.empty() ? "" : ",") + o.name;
+          bad_sig = "output tensor alias not found in signature: " + a + " Outputs expected to be in the set {" + set + "}.";
+          return nullptr;
+        }
+        if (!sel.insert(a).second) {
+          bad_sig = "duplicate output tensor alias: " + a;
+          return nullptr;
+        }
+      }
+      if (!plan_outputs(d, rows, ts[0].shape, std::vector<std::string>(sel.begin(), sel.end()), &plan, &bad_sig)) return nullptr;
+      packed.assign((size_t)(rows * d.out_dim), 0.f);
+      return packed.data();
     }
     std::vector<int64_t> sh;
     if (!out_shape(d, rows, ts[0].shape, &sh, &bad_sig)) return nullptr;
@@ -562,6 +706,23 @@ static int grpc_predict_impl(tfsc_server* s, const void* req, size_t req_len, vo
     s->fail_grpc++;
     if (!bad_sig.empty()) return fail(TFSC_E_INVALID, "%s", bad_sig.c_str());
     return fail(rc, "%s", err.c_str());
+  }
+  if (!plan.sel.empty()) {
+    std::vector<std::vector<char>> vals(plan.sel.size());
+    std::vector<OutTensor> outs(plan.sel.size());
+    for (size_t i = 0; i < plan.sel.size(); ++i) {
+      vals[i].resize((size_t)(plan.rows * plan.sel[i].width) * 4);
+      split_output(plan, i, packed.data(), vals[i].data());
+      outs[i].name = plan.sel[i].name;
+      outs[i].dtype = output_dtype(plan.sel[i].kind);
+      outs[i].shape = plan.shapes[i];
+      outs[i].data = vals[i].data();
+      outs[i].n = product(plan.shapes[i]);
+    }
+    set_resp_bytes(encode_predict_response(view.model_name, id.version,
+                                           view.signature_name.empty() ? "serving_default" : view.signature_name, outs),
+                   resp, resp_len);
+    return 0;
   }
   *resp = buf;
   *resp_len = total;
@@ -599,6 +760,11 @@ static int run_examples(tfsc_server* s, const ExampleRequestView& view, int meth
   if (!d.inputs.empty()) {
     *err = std::string(method == 1 ? "Classify" : "Regress") + " serves single-input models; " + view.model_name + " has inputs " +
            expected_inputs(d) + " (use Predict)";
+    return TFSC_E_INVALID;
+  }
+  if (!d.outputs.empty()) {
+    *err = std::string(method == 1 ? "Classify" : "Regress") + " serves single-output models; " + view.model_name + " has outputs " +
+           expected_outputs(d) + " (use Predict)";
     return TFSC_E_INVALID;
   }
   const std::string want = view.signature_name.empty() ? "serving_default" : view.signature_name;
@@ -732,7 +898,18 @@ static int grpc_session_run_impl(tfsc_server* s, const void* req, size_t req_len
   char* buf = nullptr;
   size_t total = 0;
   std::string bad;
+  OutputPlan plan;
+  std::vector<float> packed;
   auto alloc = [&](const ModelDesc& d, int64_t rows) -> void* {
+    if (!d.outputs.empty()) {  // a multi-output model: the fetch names any one of its outputs
+      if (strip(tv.name) != d.input_name || !d.output(strip(view.fetch[0]))) {
+        bad = "feed / fetch do not name the model's tensors (feed '" + d.input_name + ":0', fetch one of " + expected_outputs(d) + ")";
+        return nullptr;
+      }
+      if (!plan_outputs(d, rows, tv.shape, {strip(view.fetch[0])}, &plan, &bad)) return nullptr;
+      packed.assign((size_t)(rows * d.out_dim), 0.f);
+      return packed.data();
+    }
     if (strip(tv.name) != d.input_name || strip(view.fetch[0]) != d.output_name) {
       bad = "feed / fetch do not name the model's tensors (feed '" + d.input_name + ":0', fetch '" + d.output_name + ":0')";
       return nullptr;
@@ -756,6 +933,18 @@ static int grpc_session_run_impl(tfsc_server* s, const void* req, size_t req_len
     s->fail_grpc++;
     if (!bad.empty()) return fail(TFSC_E_INVALID, "%s", bad.c_str());
     return fail(rc, "%s", err.c_str());
+  }
+  if (!plan.sel.empty()) {
+    std::vector<char> vals((size_t)(plan.rows * plan.sel[0].width) * 4);
+    split_output(plan, 0, packed.data(), vals.data());
+    OutTensor t;
+    t.name = view.fetch[0];
+    t.dtype = output_dtype(plan.sel[0].kind);
+    t.shape = plan.shapes[0];
+    t.data = vals.data();
+    t.n = product(plan.shapes[0]);
+    set_resp_bytes(encode_session_run_response(view.model_name, id.version, view.signature_name, t), resp, resp_len);
+    return 0;
   }
   *resp = buf;
   *resp_len = total;
@@ -835,6 +1024,75 @@ static void write_tensor_json(const float* v, const std::vector<int64_t>& shape,
     write_tensor_json(v, shape, dim + 1, idx, s);
   }
   *s += "]";
+}
+
+// one value of a packed row as JSON: fp32 as json_float, int32 / int64 as integers
+static void json_word_value(OutputKind k, const uint32_t* w, std::string* s) {
+  if (k == OutputKind::Classes) {
+    *s += std::to_string((int64_t)((uint64_t)w[0] | ((uint64_t)w[1] << 32)));
+  } else if (k == OutputKind::TopKClasses) {
+    *s += std::to_string((int32_t)w[0]);
+  } else {
+    float f;
+    memcpy(&f, w, 4);
+    json_float(f, s);
+  }
+}
+
+// values [dims...] of one output, row-major, `step` words per value
+static void json_nested(OutputKind k, const uint32_t* w, const std::vector<int64_t>& dims, size_t dim, int64_t* idx, int step,
+                        std::string* s) {
+  if (dim == dims.size()) {
+    json_word_value(k, w + *idx * step, s);
+    ++*idx;
+    return;
+  }
+  *s += "[";
+  for (int64_t i = 0; i < dims[dim]; ++i) {
+    if (i) *s += ", ";
+    json_nested(k, w, dims, dim + 1, idx, step, s);
+  }
+  *s += "]";
+}
+
+// TF-Serving's multi-output REST shapes: row format {"predictions": [{"<output>": value, ...} per row]}, columnar format
+// {"outputs": {"<output>": tensor, ...}}; keys in packed (sorted name) order
+static std::string rest_multi_output_json(const OutputPlan& p, const float* packed, bool row_format) {
+  const uint32_t* words = reinterpret_cast<const uint32_t*>(packed);
+  std::string b = std::string("{\n    \"") + (row_format ? "predictions" : "outputs") + "\": " + (row_format ? "[" : "{");
+  if (row_format) {
+    for (int64_t r = 0; r < p.rows; ++r) {
+      b += r ? ", {" : "{";
+      for (size_t i = 0; i < p.sel.size(); ++i) {
+        const ModelOutput& o = p.sel[i];
+        if (i) b += ", ";
+        json_escape(o.name, &b);
+        b += ": ";
+        const uint32_t* w = words + r * p.out_dim + o.offset;
+        if (o.kind == OutputKind::Classes) {
+          json_word_value(o.kind, w, &b);
+        } else {
+          int64_t idx = 0;
+          json_nested(o.kind, w, {o.width}, 0, &idx, 1, &b);
+        }
+      }
+      b += "}";
+    }
+    b += "]\n}";
+    return b;
+  }
+  for (size_t i = 0; i < p.sel.size(); ++i) {
+    const ModelOutput& o = p.sel[i];
+    std::vector<uint32_t> vals((size_t)(p.rows * o.width));
+    split_output(p, i, packed, vals.data());
+    if (i) b += ", ";
+    json_escape(o.name, &b);
+    b += ": ";
+    int64_t idx = 0;
+    json_nested(o.kind, vals.data(), p.shapes[i], 0, &idx, o.kind == OutputKind::Classes ? 2 : 1, &b);
+  }
+  b += "}\n}";
+  return b;
 }
 
 static int rest_handle_impl(tfsc_server* s, const char* method, const char* url, const void* body, size_t body_len,
@@ -975,6 +1233,7 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
     std::vector<float> y;
     std::vector<int64_t> oshape;
     std::string bad_sig;
+    OutputPlan plan;
     std::vector<InTensor> ts(columns.size());
     for (size_t i = 0; i < columns.size(); ++i) {
       ts[i].name = columns[i].first;
@@ -989,6 +1248,11 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
       if (d.inputs.empty() && !input_key.empty() && input_key != d.input_name) {
         bad_sig = "input '" + input_key + "' does not match the model signature (expects '" + d.input_name + "')";
         return nullptr;
+      }
+      if (!d.outputs.empty()) {  // every output (REST has no output filter), answered in packed order below
+        if (!plan_outputs(d, rows, shape, {}, &plan, &bad_sig)) return nullptr;
+        y.assign((size_t)(rows * d.out_dim), 0.f);
+        return y.data();
       }
       if (!out_shape(d, rows, shape, &oshape, &bad_sig)) return nullptr;
       int64_t on = 1;
@@ -1006,6 +1270,11 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
       rc = run_predict_one(s, node, remote, id, ints.data(), (int64_t)ints.size(), TFSC_DT_INT32, alloc, &err);
     }
     if (rc < 0) return fail_http(bad_sig.empty() ? http_for(rc) : 400, bad_sig.empty() ? err : bad_sig);
+    if (!plan.sel.empty()) {
+      *http_status = 200;
+      set_resp(rest_multi_output_json(plan, y.data(), instances != nullptr), resp, resp_len);
+      return 0;
+    }
     // TF-Serving's writer: 4-space indent, arrays on one line, closing bracket on its own line
     std::string b = std::string("{\n    \"") + (instances ? "predictions" : "outputs") + "\": ";
     size_t idx = 0;
@@ -1039,12 +1308,19 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
     for (auto& mi : d.inputs)
       ins += (ins.empty() ? "" : ", ") + tensor_info(mi.name, std::to_string(d.in_dim / (int64_t)d.inputs.size()), "DT_INT32");
     if (d.inputs.empty()) ins = tensor_info(d.input_name, dim, d.input_dtype == TFSC_DT_INT32 ? "DT_INT32" : "DT_FLOAT");
+    // a multi-output model lists every output: logits / probabilities [-1, N], classes [-1] (int64), top-k [-1, k]
+    std::string outs;
+    for (auto& mo : d.outputs) {
+      const std::string last = mo.kind == OutputKind::Classes ? ""
+                               : mo.kind == OutputKind::Logits || mo.kind == OutputKind::Probabilities ? std::to_string(d.head_n)
+                                                                                                        : std::to_string(d.head_k);
+      outs += (outs.empty() ? "" : ", ") + tensor_info(mo.name, last, dtype_name(output_dtype(mo.kind)).c_str());
+    }
+    if (d.outputs.empty()) outs = tensor_info(d.output_name, odim, "DT_FLOAT");
     std::string b = "{\n\"model_spec\": {\"name\": ";
     json_escape(name, &b);
     b += ", \"signature_name\": \"\", \"version\": \"" + std::to_string(id.version) + "\"},\n\"metadata\": {\"signature_def\": {\"signature_def\": {\"serving_default\": {\"inputs\": {" +
-         ins + "}, \"outputs\": {" +
-         tensor_info(d.output_name, odim, "DT_FLOAT") +
-         "}, \"method_name\": \"tensorflow/serving/predict\"}}}}\n}\n";
+         ins + "}, \"outputs\": {" + outs + "}, \"method_name\": \"tensorflow/serving/predict\"}}}}\n}\n";
     *http_status = 200;
     set_resp(b, resp, resp_len);
     return 0;
@@ -1166,7 +1442,10 @@ struct tfsc_ticket {
   char* staging = nullptr;
   size_t staging_bytes = 0, in_al = 0, out_bytes = 0;
   tfsc_tensor* out = nullptr;
+  int n_out = 0;
   std::vector<int64_t> oshape;
+  OutputPlan plan;            // multi-output model: the outputs out[i] asked for, split from `packed` by wait()
+  std::vector<float> packed;
   // requests owned by another rank take the (synchronous) forward hop on a helper thread
   std::thread remote_thread;
   std::mutex mu;
@@ -1198,6 +1477,7 @@ static int submit_impl(tfsc_server* s, const char* model_name, const char* versi
   t->srv = s;
   t->node = node;
   t->out = &out[0];
+  t->n_out = n_out;
   std::string err;
   if (!node) {
     // another rank owns the model: the forward hop is synchronous, run it beside the caller
@@ -1217,6 +1497,11 @@ static int submit_impl(tfsc_server* s, const char* model_name, const char* versi
         if (d.inputs.empty() && has_name && d.input_name != xname) {
           bad = "input '" + xname + "' does not match the model signature (expects '" + d.input_name + "')";
           return nullptr;
+        }
+        if (!d.outputs.empty()) {
+          void* y = abi_outputs_alloc(d, rows, ishape, tp->out, tp->n_out, &tp->plan, &tp->packed, &bad);
+          tp->out_bytes = tp->packed.size() * 4;
+          return y;
         }
         if (!out_shape(d, rows, ishape, &tp->oshape, &bad)) return nullptr;
         int64_t on = 1;
@@ -1240,15 +1525,20 @@ static int submit_impl(tfsc_server* s, const char* model_name, const char* versi
   std::string bad;
   if (d.inputs.empty() && x.name && d.input_name != x.name)
     bad = "input '" + std::string(x.name) + "' does not match the model signature (expects '" + d.input_name + "')";
-  if (bad.empty()) out_shape(d, t->req.rows, ishape, &t->oshape, &bad);
+  bool buffers_ok = true;
+  if (bad.empty() && !d.outputs.empty()) {
+    buffers_ok = abi_outputs_alloc(d, t->req.rows, ishape, out, n_out, &t->plan, &t->packed, &bad) != nullptr;
+  } else if (bad.empty()) {
+    out_shape(d, t->req.rows, ishape, &t->oshape, &bad);
+  }
   if (!bad.empty()) {
     node->abandon(&t->req);
     return fail(TFSC_E_INVALID, "%s", bad.c_str());
   }
   int64_t on = 1;
   for (auto v : t->oshape) on *= v;
-  t->out_bytes = (size_t)on * 4;
-  if (!out[0].data || out[0].nbytes < t->out_bytes || t->oshape.size() > 8) {
+  t->out_bytes = d.outputs.empty() ? (size_t)on * 4 : t->packed.size() * 4;
+  if (d.outputs.empty() ? (!out[0].data || out[0].nbytes < t->out_bytes || t->oshape.size() > 8) : !buffers_ok) {
     node->abandon(&t->req);
     return fail(TFSC_E_BUFFER, "output buffer too small");
   }
@@ -1289,9 +1579,14 @@ static int wait_impl(tfsc_ticket* t, int64_t timeout_ns) {
       return fail(TFSC_E_TIMEOUT, "predict_wait: request still in flight");
     rc = t->req.rc;
     err = t->req.err;
-    if (rc == 0 && !t->delivered) memcpy(t->out->data, t->staging + t->in_al, t->out_bytes);
+    if (rc == 0 && !t->delivered)
+      memcpy(t->plan.sel.empty() ? t->out->data : (void*)t->packed.data(), t->staging + t->in_al, t->out_bytes);
   }
   if (rc < 0) return fail(rc, "%s", err.c_str());
+  if (!t->delivered && !t->plan.sel.empty()) {
+    abi_outputs_deliver(t->plan, t->packed.data(), t->out);
+    t->delivered = true;
+  }
   if (!t->delivered) {
     t->out->dtype = TFSC_DT_FLOAT;
     t->out->rank = (int32_t)t->oshape.size();
@@ -1537,6 +1832,24 @@ int tfsc_k_layernorm(const float* x, const float* res, const float* gamma, const
   cudaError_t e = launch_layernorm(x, res, nullptr, nullptr, 0, nullptr, nullptr, nullptr, gamma, beta, y, tokens, 1, hidden, 0, eps,
                                    (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "layernorm: %s", cudaGetErrorString(e));
+}
+int tfsc_k_classify_head(const float* logits, int rows, int n, int k, float* probs, int64_t* classes, int32_t* topk_idx,
+                         float* topk_prob, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (!logits || rows < 0 || !head_supported(n, k))
+    return fail(TFSC_E_INVALID, "classify_head: no kernel for %d rows of %d logits, k = %d (1 <= n <= %d, 1 <= k <= min(n, %d))", rows,
+                n, k, kHeadMaxN, kHeadMaxK);
+  HeadOutputs o;
+  o.probs = probs;
+  o.probs_ld = n;
+  o.classes = reinterpret_cast<int*>(classes);
+  o.classes_ld = 2;
+  o.topk_idx = topk_idx;
+  o.topk_idx_ld = k;
+  o.topk_prob = topk_prob;
+  o.topk_prob_ld = k;
+  cudaError_t e = launch_classify_head(logits, rows, n, k, o, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "classify_head: %s", cudaGetErrorString(e));
 }
 int tfsc_debug_gemm_trace(long long*) {
   return fail(TFSC_E_UNIMPLEMENTED, "no GEMM clock trace: the persistent GEMM kernel it timed is not part of the sm_90a build");

@@ -607,4 +607,60 @@ void session_run_response_frame(const std::string& model_name, int64_t version, 
   put_ld(suffix, 3, spec_bytes(model_name, version, signature_name));
 }
 
+// ------------------------------------------------------------------ multi-output responses ----
+static std::string tensor_proto(const OutTensor& t) {
+  std::string s;
+  put_tag(&s, 1, 0);
+  put_varint(&s, (uint64_t)t.dtype);
+  std::string sh;
+  for (auto d : t.shape) {
+    std::string dim;
+    if (d != 0) {
+      put_tag(&dim, 1, 0);
+      put_varint(&dim, (uint64_t)d);
+    }
+    put_ld(&sh, 2, dim);
+  }
+  put_ld(&s, 2, sh);
+  if (t.n > 0) {
+    std::string vals;
+    if (t.dtype == TFSC_DT_FLOAT) {
+      vals.assign(static_cast<const char*>(t.data), (size_t)t.n * 4);  // packed float_val = little-endian fp32
+      put_ld(&s, 5, vals);
+    } else if (t.dtype == TFSC_DT_INT64) {
+      const int64_t* v = static_cast<const int64_t*>(t.data);
+      for (int64_t i = 0; i < t.n; ++i) put_varint(&vals, (uint64_t)v[i]);
+      put_ld(&s, 10, vals);  // packed int64_val
+    } else {
+      const int32_t* v = static_cast<const int32_t*>(t.data);
+      for (int64_t i = 0; i < t.n; ++i) put_varint(&vals, (uint64_t)(int64_t)v[i]);  // int32 varints sign-extend
+      put_ld(&s, 7, vals);  // packed int_val
+    }
+  }
+  return s;
+}
+
+std::string encode_predict_response(const std::string& model_name, int64_t version, const std::string& signature_name,
+                                    const std::vector<OutTensor>& outs) {
+  std::string s;
+  for (auto& t : outs) {
+    std::string entry;
+    put_ld(&entry, 1, t.name);
+    put_ld(&entry, 2, tensor_proto(t));
+    put_ld(&s, 1, entry);
+  }
+  put_ld(&s, 2, spec_bytes(model_name, version, signature_name));
+  return s;
+}
+
+std::string encode_session_run_response(const std::string& model_name, int64_t version, const std::string& signature_name,
+                                        const OutTensor& t) {
+  std::string named, s;
+  if (!t.name.empty()) put_ld(&named, 1, t.name);
+  put_ld(&named, 2, tensor_proto(t));
+  put_ld(&s, 1, named);
+  put_ld(&s, 3, spec_bytes(model_name, version, signature_name));
+  return s;
+}
+
 }  // namespace tfsc

@@ -57,6 +57,22 @@ void predict_response_frame(const std::string& model_name, int64_t version, cons
                             const std::string& output_name, const std::vector<int64_t>& shape, std::string* prefix,
                             std::string* suffix);
 
+// One output of a multi-output response: fp32 values go in packed float_val (field 5), int64 in packed int64_val
+// (field 10), int32 in packed int_val (field 7), as TF-Serving's AsProtoField writes them.
+struct OutTensor {
+  std::string name;
+  int dtype = TFSC_DT_FLOAT;
+  std::vector<int64_t> shape;
+  const void* data = nullptr;
+  int64_t n = 0;
+};
+// PredictResponse{outputs (in the given order), model_spec}
+std::string encode_predict_response(const std::string& model_name, int64_t version, const std::string& signature_name,
+                                    const std::vector<OutTensor>& outs);
+// SessionRunResponse{tensor = [NamedTensorProto{name, t}], model_spec}
+std::string encode_session_run_response(const std::string& model_name, int64_t version, const std::string& signature_name,
+                                        const OutTensor& t);
+
 // ---- Classify / Regress (tfservingproxy.go:173-198): ClassificationRequest / RegressionRequest{model_spec=1, input=2
 // Input{example_list=1{examples=1}, example_list_with_context=2{examples=1, context=2}}}, tf.Example{features=1{feature=1
 // map<string, Feature{bytes_list=1, float_list=2{value=1 packed}, int64_list=3}>}} (proto/tensorflow/serving/

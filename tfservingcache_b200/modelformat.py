@@ -14,7 +14,47 @@ def _align256(x: int) -> int:
     return (x + 255) & ~255
 
 
-def write_mlp_bundle(version_dir: str, weights, biases, activations=None, input_name="x", output_name="y", extra_signatures=None):
+OUTPUT_KINDS = ("logits", "probabilities", "classes", "top_k_classes", "top_k_probabilities")
+
+
+def _signature(sig: dict, outputs):
+    """signature.outputs replaces signature.output: a list of {"name", "kind"} (+ "k" for the top-k kinds)."""
+    if outputs is None:
+        return sig
+    sig = {k: v for k, v in sig.items() if k != "output"}
+    sig["outputs"] = [dict(o) for o in outputs]
+    return sig
+
+
+def packed_output_layout(outputs, n):
+    """(name, element offset, width, dtype) of every output in a packed response row, in packed order (byte-wise sorted
+    names). Offsets and widths count 32-bit words: logits / probabilities n floats, classes 2 words (one little-endian
+    int64), top-k k values (int32 classes, float probabilities). n = the last op's per-row width."""
+    out, off = [], 0
+    for o in sorted(outputs, key=lambda o: o["name"].encode()):
+        kind = o["kind"]
+        width = {"logits": n, "probabilities": n, "classes": 2}.get(kind, o.get("k"))
+        dtype = {"classes": "int64", "top_k_classes": "int32"}.get(kind, "float32")
+        out.append((o["name"], off, int(width), dtype))
+        off += int(width)
+    return out
+
+
+def split_packed_rows(rows_words: np.ndarray, outputs, n) -> dict:
+    """{name: array} from packed rows ([rows, out_dim] of any 4-byte dtype, e.g. the float32 view of tfsc_predict_device's y)."""
+    w = np.ascontiguousarray(rows_words).view(np.uint32).reshape(len(rows_words), -1)
+    res = {}
+    for name, off, width, dtype in packed_output_layout(outputs, n):
+        part = np.ascontiguousarray(w[:, off:off + width])
+        if dtype == "int64":
+            res[name] = part.view("<i8").reshape(-1)
+        else:
+            res[name] = part.view("<i4" if dtype == "int32" else "<f4")
+    return res
+
+
+def write_mlp_bundle(version_dir: str, weights, biases, activations=None, input_name="x", output_name="y", extra_signatures=None,
+                     outputs=None):
     n = len(weights)
     if activations is None:
         activations = ["relu"] * (n - 1) + ["linear"]
@@ -31,7 +71,7 @@ def write_mlp_bundle(version_dir: str, weights, biases, activations=None, input_
         blob[L["w_offset"] // 4: L["w_offset"] // 4 + w.size] = np.asarray(w, np.float32).ravel()
         blob[L["b_offset"] // 4: L["b_offset"] // 4 + b.size] = np.asarray(b, np.float32).ravel()
     man = {"format": "tfsc-b200-v1", "template": "mlp", "dtype": "float32",
-           "signature": {"input": input_name, "output": output_name}, "layers": layers, "weights_bytes": off}
+           "signature": _signature({"input": input_name, "output": output_name}, outputs), "layers": layers, "weights_bytes": off}
     if extra_signatures:   # classify / regress signatures: [{"name", "method": "classify"|"regress", "feature"}]
         man["extra_signatures"] = list(extra_signatures)
     _write(version_dir, man, blob)
@@ -57,7 +97,7 @@ def _write(version_dir: str, man: dict, blob: np.ndarray):
     blob.astype("<f4").tofile(os.path.join(version_dir, "weights.bin"))
 
 
-def _graph_manifest(input_shape, ops, n_buffers, input_name="x", output_name="y", input_dtype="float32", inputs=None):
+def _graph_manifest(input_shape, ops, n_buffers, input_name="x", output_name="y", input_dtype="float32", inputs=None, outputs=None):
     off = 0
 
     def take(nbytes):
@@ -82,13 +122,14 @@ def _graph_manifest(input_shape, ops, n_buffers, input_name="x", output_name="y"
     if inputs is not None:   # several named inputs with roles: "inputs" replaces "input"
         sig = {"inputs": [{"name": i["name"], "role": i["role"]} for i in inputs], "output": output_name}
     return {"format": "tfsc-b200-v1", "template": "graph", "dtype": "float32", "input_dtype": input_dtype,
-            "signature": sig, "input_shape": list(input_shape),
+            "signature": _signature(sig, outputs), "input_shape": list(input_shape),
             "n_buffers": n_buffers, "ops": ops, "weights_bytes": off}
 
 
-def resnet50_manifest(image=224, classes=1000, width=64, blocks=(3, 4, 6, 3)):
+def resnet50_manifest(image=224, classes=1000, width=64, blocks=(3, 4, 6, 3), outputs=None):
     """ResNet-50 v1.5 (torchvision topology: stride on the 3x3 conv) as a graph bundle, NHWC, BatchNorm folded into
-    kernel + bias. Buffers: 0 = block input / identity, 1 = 1x1 out, 2 = 3x3 out, 3 = block out, 4 = downsample."""
+    kernel + bias. Buffers: 0 = block input / identity, 1 = 1x1 out, 2 = 3x3 out, 3 = block out, 4 = downsample.
+    outputs: signature.outputs (a list of {"name", "kind"[, "k"]}) in place of the single logits output."""
     ops, h = [], image
     ops.append({"op": "conv", "src": -1, "dst": 0, "h": h, "w": h, "c": 3, "kh": 7, "kw": 7, "stride": 2, "pad": 3,
                 "cout": width, "act": "relu"})
@@ -118,7 +159,7 @@ def resnet50_manifest(image=224, classes=1000, width=64, blocks=(3, 4, 6, 3)):
     a = [x for x in range(5) if x != cur][0]
     ops.append({"op": "avgpool", "src": cur, "dst": a, "h": h, "w": h, "c": cin})
     ops.append({"op": "dense", "src": a, "dst": -2, "h": 1, "w": 1, "c": cin, "cout": classes, "act": "none"})
-    return _graph_manifest([image, image, 3], ops, 5)
+    return _graph_manifest([image, image, 3], ops, 5, outputs=outputs)
 
 
 def write_graph_bundle(version_dir: str, manifest: dict, blob: np.ndarray):
@@ -134,12 +175,15 @@ def packed_input_order(inputs):
     return sorted((i["name"] for i in inputs), key=lambda n: n.encode())
 
 
-def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30522, max_pos=512, labels=2, inputs=None):
+def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30522, max_pos=512, labels=2, inputs=None,
+                  outputs=None):
     """BERT-base fine-tune variant (Devlin et al. 2018) as a graph bundle: token ids int32 [B, seq] -> logits
     [B, labels]. A sequence is an "image" with h = seq tokens, w = 1, c = width; dense layers are 1x1 convs.
     With inputs=None the bundle takes the ids only: the attention mask is derived from them ([PAD] = 0), token_type is 0.
     With inputs = a list of {"name", "role"} (roles "ids", "mask", "type_ids"; e.g. BERT_INPUTS) it declares those int32
     [B, seq] inputs, and the kernels read the attention mask and the segment ids from the request.
+    With outputs = a list of {"name", "kind"[, "k"]} (kinds in OUTPUT_KINDS) the bundle answers those outputs, computed
+    from the logits on the GPU, in place of the single "logits" output.
     Buffers: 0 hidden, 1 qkv / ffn-intermediate, 2 context / post-attention, 3 dense output."""
     ops = [{"op": "embed", "src": -1, "dst": 0, "h": seq, "w": 1, "c": hidden, "vocab": vocab, "max_pos": max_pos, "eps": 1e-12}]
 
@@ -160,4 +204,5 @@ def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30
         ops.append({"op": "layernorm", "src": 3, "res": 2, "dst": 0, "h": seq, "w": 1, "c": hidden, "eps": 1e-12})
     ops.append({"op": "dense", "src": 0, "dst": 1, "h": 1, "w": 1, "c": hidden, "cout": hidden, "act": "tanh"})   # pooler on [CLS]
     ops.append({"op": "dense", "src": 1, "dst": -2, "h": 1, "w": 1, "c": hidden, "cout": labels, "act": "none"})
-    return _graph_manifest([seq], ops, 4, input_name="input_ids", output_name="logits", input_dtype="int32", inputs=inputs)
+    return _graph_manifest([seq], ops, 4, input_name="input_ids", output_name="logits", input_dtype="int32", inputs=inputs,
+                           outputs=outputs)

@@ -70,13 +70,45 @@ class Server:
         return [(n, int(v), int(b)) for n, v, b, _p in self._lines(lib.tfsc_host_list, node)]
 
     def predict(self, model_name: str, version: str, x, out_capacity_elems: int | None = None,
-                input_name: str | None = None) -> np.ndarray:
+                input_name: str | None = None, outputs=None):
         """x: one array, or {name: array} for a model with several inputs (e.g. BERT's input_ids / input_mask /
-        segment_ids, int32 [batch, seq] each)."""
+        segment_ids, int32 [batch, seq] each). outputs: names of outputs of a multi-output model (signature.outputs,
+        e.g. ("classes", "probabilities")): the result is then {name: ndarray} (classes int64, top-k classes int32);
+        without it the result is the one ndarray of a single-output model."""
+        if outputs is not None:
+            _x, tin, ys, touts = self._tensors_multi(x, out_capacity_elems, input_name, outputs)
+            check(lib.tfsc_predict(self._h, model_name.encode(), version.encode(), tin, len(tin), touts, len(outputs)),
+                  "predict")
+            return self._results(ys, touts, outputs)
         _x, tin, y, tout = self._tensors(x, out_capacity_elems, input_name)
         check(lib.tfsc_predict(self._h, model_name.encode(), version.encode(), tin, len(tin), C.byref(tout), 1),
               "predict")
         return self._result(y, tout)
+
+    @staticmethod
+    def _tensors_multi(x, out_capacity_elems, input_name, outputs):
+        """_tensors with one named output tensor per entry of `outputs`, each with its own buffer"""
+        arrays, tin, _y, _t = Server._tensors(x, 1, input_name)
+        if out_capacity_elems is None:
+            lead = arrays[0].shape[0] if arrays[0].ndim > 1 else 1
+            out_capacity_elems = max(sum(a.size for a in arrays) * 4 + 65536, lead * 32768 * 2)
+        ys, touts = [], (TfscTensor * len(outputs))()
+        for t, name in zip(touts, outputs):
+            y = np.empty(out_capacity_elems * 4, dtype=np.uint8)
+            ys.append(y)
+            t.name = name.encode()
+            t.data = y.ctypes.data
+            t.nbytes = y.nbytes
+        return arrays, tin, ys, touts
+
+    @staticmethod
+    def _results(ys, touts, outputs) -> dict:
+        np_dt = {_lib.DT_FLOAT: np.float32, _lib.DT_INT32: np.int32, _lib.DT_INT64: np.int64}
+        res = {}
+        for y, t, name in zip(ys, touts, outputs):
+            shape = tuple(t.shape[i] for i in range(t.rank))
+            res[name] = y[:t.nbytes].view(np_dt[t.dtype]).reshape(shape).copy()
+        return res
 
     @staticmethod
     def _tensors(x, out_capacity_elems, input_name):
@@ -110,14 +142,27 @@ class Server:
         return y[:n].reshape(shape).copy()
 
     def predict_deadline(self, model_name: str, version: str, x: np.ndarray, deadline_ns: int, **kw) -> np.ndarray:
-        """tfsc_predict_deadline: deadline is absolute on the clock of now_ns() (0 = none)."""
+        """tfsc_predict_deadline: deadline is absolute on the clock of now_ns() (0 = none). outputs= as for predict()."""
+        if kw.get("outputs") is not None:
+            outs = kw["outputs"]
+            _x, tin, ys, touts = self._tensors_multi(x, kw.get("out_capacity_elems"), kw.get("input_name"), outs)
+            check(lib.tfsc_predict_deadline(self._h, model_name.encode(), version.encode(), tin, len(tin), touts, len(outs),
+                                            int(deadline_ns)), "predict")
+            return self._results(ys, touts, outs)
         _x, tin, y, tout = self._tensors(x, kw.get("out_capacity_elems"), kw.get("input_name"))
         check(lib.tfsc_predict_deadline(self._h, model_name.encode(), version.encode(), tin, len(tin), C.byref(tout), 1,
                                         int(deadline_ns)), "predict")
         return self._result(y, tout)
 
     def predict_member(self, member: int, model_name: str, version: str, x: np.ndarray, deadline_ns: int = 0, **kw) -> np.ndarray:
-        """tfsc_predict_member: the cache tier of member `member` (index into gpu.members), no ring lookup."""
+        """tfsc_predict_member: the cache tier of member `member` (index into gpu.members), no ring lookup. outputs= as for
+        predict()."""
+        if kw.get("outputs") is not None:
+            outs = kw["outputs"]
+            _x, tin, ys, touts = self._tensors_multi(x, kw.get("out_capacity_elems"), kw.get("input_name"), outs)
+            check(lib.tfsc_predict_member(self._h, member, model_name.encode(), version.encode(), tin, len(tin), touts,
+                                          len(outs), int(deadline_ns)), "predict_member")
+            return self._results(ys, touts, outs)
         _x, tin, y, tout = self._tensors(x, kw.get("out_capacity_elems"), kw.get("input_name"))
         check(lib.tfsc_predict_member(self._h, member, model_name.encode(), version.encode(), tin, len(tin), C.byref(tout), 1,
                                       int(deadline_ns)), "predict_member")
@@ -128,9 +173,16 @@ class Server:
         return lib.tfsc_now_ns()
 
     def predict_submit(self, model_name: str, version: str, x: np.ndarray, deadline_ns: int = 0, **kw) -> "Ticket":
-        """Asynchronous Predict (tfsc_predict_submit): returns a Ticket; .wait() yields the result."""
-        xk, tin, y, tout = self._tensors(x, kw.get("out_capacity_elems"), kw.get("input_name"))
+        """Asynchronous Predict (tfsc_predict_submit): returns a Ticket; .wait() yields the result. outputs= as for
+        predict()."""
         t = C.c_void_p()
+        if kw.get("outputs") is not None:
+            outs = list(kw["outputs"])
+            xk, tin, ys, touts = self._tensors_multi(x, kw.get("out_capacity_elems"), kw.get("input_name"), outs)
+            check(lib.tfsc_predict_submit(self._h, model_name.encode(), version.encode(), tin, len(tin), touts, len(outs),
+                                          int(deadline_ns), C.byref(t)), "predict_submit")
+            return Ticket(t, ys, touts, outs, keep=xk)
+        xk, tin, y, tout = self._tensors(x, kw.get("out_capacity_elems"), kw.get("input_name"))
         check(lib.tfsc_predict_submit(self._h, model_name.encode(), version.encode(), tin, len(tin), C.byref(tout), 1,
                                       int(deadline_ns), C.byref(t)), "predict_submit")
         return Ticket(t, y, tout)
@@ -204,11 +256,13 @@ class Server:
 class Ticket:
     """An in-flight asynchronous Predict (tfsc_ticket). Keeps the output buffer alive until released."""
 
-    def __init__(self, handle, y, tout):
-        self._t, self._y, self._tout = handle, y, tout
+    def __init__(self, handle, y, tout, outputs=None, keep=None):
+        self._t, self._y, self._tout, self._outputs, self._keep = handle, y, tout, outputs, keep
 
-    def wait(self, timeout_s: float | None = None) -> np.ndarray:
+    def wait(self, timeout_s: float | None = None):
         check(lib.tfsc_predict_wait(self._t, -1 if timeout_s is None else int(timeout_s * 1e9)), "predict_wait")
+        if self._outputs is not None:
+            return Server._results(self._y, self._tout, self._outputs)
         return Server._result(self._y, self._tout)
 
     def release(self):
