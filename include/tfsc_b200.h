@@ -208,9 +208,10 @@ int tfsc_host_list(tfsc_server* s, int node, char* buf, size_t cap);
  * size or a float tensor answer TFSC_E_INVALID naming the expected inputs (after the model is made resident, as every
  * input error; nothing is launched). The same holds for _deadline, _member and _submit.
  * Outputs: a single-output model fills out[0] (DT_FLOAT; out[0].name is not looked at) and ignores out[1..n_out). A model
- * whose manifest declares signature.outputs (logits, probabilities, classes, top_k_classes, top_k_probabilities) fills
- * out[i] with the output named out[i].name, in the caller's order: dtype (DT_INT64 for classes, DT_INT32 for
- * top_k_classes, DT_FLOAT otherwise), shape (batch dims, then [N], nothing or [k]) and nbytes. A NULL, unknown or repeated
+ * whose manifest declares signature.outputs (logits, probabilities, classes, top_k_classes, top_k_probabilities, or the
+ * question-answering start_logits, end_logits, span_starts, span_ends, span_scores) fills out[i] with the output named
+ * out[i].name, in the caller's order: dtype (DT_INT64 for classes, DT_INT32 for top_k_classes, span_starts and span_ends,
+ * DT_FLOAT otherwise), shape (batch dims, then [N] or [S], nothing or [k]) and nbytes. A NULL, unknown or repeated
  * name is TFSC_E_INVALID and the message lists the outputs; a buffer too small for its output is TFSC_E_BUFFER. */
 int tfsc_predict(tfsc_server* s, const char* model_name, const char* version,
                  const tfsc_tensor* in, int n_in, tfsc_tensor* out, int n_out);
@@ -262,8 +263,9 @@ int tfsc_rest_handle(tfsc_server* s, const char* method, const char* url, const 
  * are x[r*3*seq .. r*3*seq + seq). The kernels read the ids, the attention mask and the segment ids from there.
  * y receives `rows` packed rows the same way. A multi-output model's row is the concatenation of its outputs' rows in
  * byte-wise sorted NAME order, in 32-bit words: logits / probabilities N floats, classes 2 words (the int64 index,
- * little-endian), top_k_classes k int32, top_k_probabilities k floats; e.g. classes | logits | probabilities is 2 + 2N words
- * per row, logits of row r at y + r*(2+2N) + 2. A single-output model's row is its out_dim floats. */
+ * little-endian), top_k_classes k int32, top_k_probabilities k floats, start_logits / end_logits S floats, span_starts /
+ * span_ends k int32, span_scores k floats; e.g. classes | logits | probabilities is 2 + 2N words per row, logits of row r at
+ * y + r*(2+2N) + 2. A single-output model's row is its out_dim floats. */
 int tfsc_predict_device(tfsc_server* s, int node, const char* model_name, int64_t version,
                         const void* x, int64_t rows, void* y, void* stream);
 int tfsc_node_sync(tfsc_server* s, int node);
@@ -367,6 +369,18 @@ int tfsc_k_layernorm(const float* x, const float* res, const float* gamma, const
  * TFSC_E_INVALID unless 1 <= n <= 32768 and 1 <= k <= min(n, 32). */
 int tfsc_k_classify_head(const float* logits, int rows, int n, int k, float* probs, int64_t* classes, int32_t* topk_idx,
                          float* topk_prob, void* stream);
+/* Span head of question-answering bundles, one launch for per-token logits[rows, S, 2] (start, end interleaved; fp32,
+ * device): start_logits[rows, S], end_logits[rows, S], and the k best answer spans span_starts[rows, k] / span_ends[rows,
+ * k] (int32) with span_scores[rows, k] = start[i] + end[j] (fp32). A candidate is a pair i <= j < i + max_answer_length
+ * of eligible tokens; token p of row r is eligible when mask[q] != 0 (mask NULL: ids[q] != 0), types[q] == 1 and, with
+ * sep_id >= 0, ids[q] != sep_id, q = r * stride + p (int32, device). Spans are ordered by score descending, then start,
+ * then end ascending, compared exactly in fp32; a NaN score is never a candidate. Slots past the last candidate are
+ * (-1, -1, -FLT_MAX). Every output pointer may be NULL (not written); without span pointers nothing but the logits is read.
+ * TFSC_E_INVALID unless 1 <= S <= 4096, 1 <= max_answer_length <= S and 1 <= k <= 32, and for spans ids, types and
+ * stride >= S. */
+int tfsc_k_span_head(const float* logits, const int32_t* ids, const int32_t* mask, const int32_t* types, int stride, int rows, int S,
+                     int max_answer_length, int k, int sep_id, float* start_logits, float* end_logits, int32_t* span_starts,
+                     int32_t* span_ends, float* span_scores, void* stream);
 
 #ifdef __cplusplus
 }

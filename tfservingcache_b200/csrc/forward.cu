@@ -179,7 +179,7 @@ FwdSignature read_sig(Reader* r) {
   for (uint32_t i = 0; r->ok && i < m; ++i) {
     s.output_names.push_back(r->str());
     const int32_t kind = r->i32();
-    if (kind < 0 || kind > (int32_t)OutputKind::TopKProbabilities) r->ok = false;
+    if (kind < 0 || kind > (int32_t)kLastOutputKind) r->ok = false;
     s.output_kinds.push_back(kind);
   }
   s.head_n = r->i32();

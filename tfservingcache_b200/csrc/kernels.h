@@ -76,6 +76,35 @@ struct HeadOutputs {
 };
 cudaError_t launch_classify_head(const float* logits, int rows, int n, int k, const HeadOutputs& o, cudaStream_t s);
 
+// Span head (span.cu): from per-token logits[rows, S, 2] (start, end interleaved) writes, for each non-null pointer, row r
+// of that output at ptr + r * ld (ld in 32-bit words): start logits [S], end logits [S], and the k best answer spans --
+// start indices [k], end indices [k] (int32) and scores start[i] + end[j] [k] (fp32) -- over the pairs of eligible tokens
+// with i <= j < i + L, ordered by score descending, then i, then j ascending. Token p of row r is eligible when
+// mask[q] != 0 (no mask: ids[q] != 0), types[q] == 1 and, with sep_id >= 0, ids[q] != sep_id, q = r * stride + p. Slots
+// past the last candidate hold (-1, -1, -FLT_MAX). k and the inputs count only when a span pointer is set.
+// cudaErrorInvalidValue outside span_supported (nn_limits.h).
+struct SpanInputs {
+  const int* ids = nullptr;
+  const int* mask = nullptr;
+  const int* types = nullptr;
+  int64_t stride = 0;
+  int sep_id = -1;
+};
+struct SpanOutputs {
+  float* start_logits = nullptr;
+  int64_t start_ld = 0;
+  float* end_logits = nullptr;
+  int64_t end_ld = 0;
+  int* starts = nullptr;
+  int64_t starts_ld = 0;
+  int* ends = nullptr;
+  int64_t ends_ld = 0;
+  float* scores = nullptr;
+  int64_t scores_ld = 0;
+};
+cudaError_t launch_span_head(const float* logits, const SpanInputs& in, int rows, int S, int L, int k, const SpanOutputs& o,
+                             cudaStream_t s);
+
 // wgmma 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
 bool gemm_tc_supported(const float* A, const float* B, const float* bias, const float* R, const float* C, int M, int N, int K,
                        int lda);

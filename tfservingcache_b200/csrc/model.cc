@@ -10,10 +10,14 @@ static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 size_t ModelDesc::scratch_bytes(int64_t rows) const {
   // an mlp's head reads the last layer's logits from the activation buffer that layer would have used, so only graph
-  // bundles with outputs need more: rows * head_n floats after the buffers and the im2col matrix
+  // bundles with outputs need more: the last op's rows after the buffers and the im2col matrix (N logits per row for a
+  // classify head, 2S per-token start / end logits for a span head)
   if (tmpl == Template::Mlp) return 2 * (((size_t)rows * (size_t)(max_width > 0 ? max_width : 1) * 4 + 255) & ~(size_t)255);
-  if (tmpl == Template::Graph)
-    return head_scratch_offset(rows) + (outputs.empty() ? 0 : align256((size_t)rows * (size_t)head_n * 4));
+  if (tmpl == Template::Graph) {
+    size_t last = 1;
+    for (auto v : output_shape) last *= (size_t)v;
+    return head_scratch_offset(rows) + (outputs.empty() ? 0 : align256((size_t)rows * last * 4));
+  }
   return 256;
 }
 
@@ -29,17 +33,46 @@ const char* output_kind_name(OutputKind k) {
     case OutputKind::Probabilities: return "probabilities";
     case OutputKind::Classes: return "classes";
     case OutputKind::TopKClasses: return "top_k_classes";
-    default: return "top_k_probabilities";
+    case OutputKind::TopKProbabilities: return "top_k_probabilities";
+    case OutputKind::StartLogits: return "start_logits";
+    case OutputKind::EndLogits: return "end_logits";
+    case OutputKind::SpanStarts: return "span_starts";
+    case OutputKind::SpanEnds: return "span_ends";
+    default: return "span_scores";
   }
 }
 
-int output_dtype(OutputKind k) {
-  return k == OutputKind::Classes ? TFSC_DT_INT64 : k == OutputKind::TopKClasses ? TFSC_DT_INT32 : TFSC_DT_FLOAT;
+int output_dtype(OutputKind k) { return output_form(k, 0, 0).dtype; }
+
+bool is_span_kind(OutputKind k) { return k >= OutputKind::StartLogits; }
+bool is_span_result_kind(OutputKind k) { return k >= OutputKind::SpanStarts; }
+
+OutputForm output_form(OutputKind k, int head_n, int head_k) {
+  OutputForm f;
+  switch (k) {
+    case OutputKind::Classes: f.width = 2, f.dtype = TFSC_DT_INT64, f.rank = 0; break;
+    case OutputKind::TopKClasses:
+    case OutputKind::SpanStarts:
+    case OutputKind::SpanEnds: f.width = head_k, f.dtype = TFSC_DT_INT32; break;
+    case OutputKind::TopKProbabilities:
+    case OutputKind::SpanScores: f.width = head_k; break;
+    default: f.width = head_n; break;  // logits, probabilities, start_logits, end_logits
+  }
+  f.dim = f.rank ? f.width : 1;
+  return f;
 }
 
 bool layout_outputs(ModelDesc* d, std::string* err) {
-  const bool topk = d->output(OutputKind::TopKClasses) || d->output(OutputKind::TopKProbabilities);
-  if (!head_supported(d->head_n, topk ? d->head_k : 1) || (!topk && d->head_k != 0)) {
+  if (d->span_head()) {
+    // max_answer_length is the owner's business, so only S and k decide whether a row can be laid out
+    const bool spans = d->output(OutputKind::SpanStarts) || d->output(OutputKind::SpanEnds) || d->output(OutputKind::SpanScores);
+    if (!span_supported(d->head_n, 1, spans ? d->head_k : 1) || (!spans && d->head_k != 0)) {
+      *err = "signature.outputs: no span kernel for S = " + std::to_string(d->head_n) + " and k = " + std::to_string(d->head_k) +
+             " (1 <= S <= " + std::to_string(kSpanMaxS) + ", 1 <= k <= " + std::to_string(kSpanMaxK) + ")";
+      return false;
+    }
+  } else if (const bool topk = d->output(OutputKind::TopKClasses) || d->output(OutputKind::TopKProbabilities);
+             !head_supported(d->head_n, topk ? d->head_k : 1) || (!topk && d->head_k != 0)) {
     *err = "signature.outputs: no head kernel for " + std::to_string(d->head_n) + " logits and k = " + std::to_string(d->head_k) +
            " (1 <= N <= " + std::to_string(kHeadMaxN) + ", 1 <= k <= min(N, " + std::to_string(kHeadMaxK) + "))";
     return false;
@@ -49,9 +82,7 @@ bool layout_outputs(ModelDesc* d, std::string* err) {
   int64_t off = 0;
   for (auto& o : d->outputs) {
     o.offset = off;
-    o.width = o.kind == OutputKind::Classes ? 2 : (o.kind == OutputKind::TopKClasses || o.kind == OutputKind::TopKProbabilities)
-                                                      ? d->head_k
-                                                      : d->head_n;
+    o.width = output_form(o.kind, d->head_n, d->head_k).width;
     off += o.width;
   }
   d->out_dim = off;
@@ -185,7 +216,16 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         *err = "signature.outputs must list 1 to " + std::to_string(kMaxOutputs) + " outputs";
         return false;
       }
-      int k = -1;
+      int k = -1, max_len = -1, sep_id = -1;
+      bool span_seen = false;  // a span_starts / span_ends / span_scores entry set max_len and sep_id
+      // an integer field of an output entry: 0 absent, 1 read into *v, -1 present but not an integer
+      auto int_field = [](const Json& oj, const char* key, int* v) {
+        const Json* f = oj.get(key);
+        if (!f) return 0;
+        if (f->type != Json::Num || f->num != (double)(int)f->num) return -1;
+        *v = (int)f->num;
+        return 1;
+      };
       for (auto& oj : outs->arr) {
         ModelOutput mo;
         mo.name = oj.type == Json::Obj ? oj.get_str("name", "") : "";
@@ -195,8 +235,14 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         else if (kind == "classes") mo.kind = OutputKind::Classes;
         else if (kind == "top_k_classes") mo.kind = OutputKind::TopKClasses;
         else if (kind == "top_k_probabilities") mo.kind = OutputKind::TopKProbabilities;
+        else if (kind == "start_logits") mo.kind = OutputKind::StartLogits;
+        else if (kind == "end_logits") mo.kind = OutputKind::EndLogits;
+        else if (kind == "span_starts") mo.kind = OutputKind::SpanStarts;
+        else if (kind == "span_ends") mo.kind = OutputKind::SpanEnds;
+        else if (kind == "span_scores") mo.kind = OutputKind::SpanScores;
         else {
-          *err = "signature.outputs: unknown kind '" + kind + "' (logits, probabilities, classes, top_k_classes, top_k_probabilities)";
+          *err = "signature.outputs: unknown kind '" + kind + "' (logits, probabilities, classes, top_k_classes, top_k_probabilities, "
+                 "start_logits, end_logits, span_starts, span_ends, span_scores)";
           return false;
         }
         if (mo.name.empty()) {
@@ -208,6 +254,45 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
             *err = "signature.outputs: duplicate " + std::string(o.name == mo.name ? "name '" + mo.name + "'" : "kind '" + kind + "'");
             return false;
           }
+        if (!d->outputs.empty() && is_span_kind(d->outputs.front().kind) != is_span_kind(mo.kind)) {
+          *err = "signature.outputs: span outputs (start_logits, end_logits, span_starts, span_ends, span_scores) cannot be mixed"
+                 " with classification outputs ('" + mo.name + "' is " + kind + ")";
+          return false;
+        }
+        if (is_span_kind(mo.kind)) {
+          if (!is_span_result_kind(mo.kind)) {
+            if (oj.get("k") || oj.get("max_answer_length") || oj.get("sep_id")) {
+              *err = "signature.outputs: 'k', 'max_answer_length' and 'sep_id' belong to span_starts, span_ends and span_scores ('" +
+                     mo.name + "' is " + kind + ")";
+              return false;
+            }
+          } else {
+            int v = 0;
+            int r = int_field(oj, "k", &v);
+            if (r != 1 || (span_seen && v != k)) {
+              *err = "signature.outputs: '" + mo.name + "' needs an integer 'k', the same for every span output";
+              return false;
+            }
+            k = v;
+            r = int_field(oj, "max_answer_length", &v);
+            if (r != 1 || (span_seen && v != max_len)) {
+              *err = "signature.outputs: '" + mo.name + "' needs an integer 'max_answer_length', the same for every span output";
+              return false;
+            }
+            max_len = v;
+            v = -1;
+            r = int_field(oj, "sep_id", &v);
+            if (r < 0 || (r == 1 && v < 0) || (span_seen && v != sep_id)) {
+              *err = "signature.outputs: '" + mo.name + "' has a 'sep_id' that is not a token id >= 0 or differs from the other"
+                     " span outputs' (give the same sep_id to every span output, or to none)";
+              return false;
+            }
+            sep_id = v;
+            span_seen = true;
+          }
+          d->outputs.push_back(mo);
+          continue;
+        }
         const bool topk = mo.kind == OutputKind::TopKClasses || mo.kind == OutputKind::TopKProbabilities;
         if (topk) {
           const Json* kj = oj.get("k");
@@ -222,7 +307,9 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         }
         d->outputs.push_back(mo);
       }
-      d->head_k = k < 0 ? 0 : k;
+      d->head_k = span_seen ? k : k < 0 ? 0 : k;  // a span k is always given, and a negative one is refused below
+      d->span_max_len = span_seen ? max_len : 0;
+      d->span_sep_id = sep_id;
     }
   }
   if (const Json* ex = j.get("extra_signatures")) {
@@ -448,11 +535,41 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
   }
   finish(d);
   if (!d->outputs.empty()) {
-    if (d->tmpl == Template::Affine) {
+    if (d->span_head()) {
+      // the span head reads the request's ids / mask / segment ids where the embedding does, and the per-token start / end
+      // logits [S, 1, 2] of the last op
+      if (d->tmpl != Template::Graph) {
+        *err = "signature.outputs: span outputs need a graph bundle (a BERT encoder ending in per-token start / end logits)";
+        return false;
+      }
+      if (d->ops.front().kind != OpKind::Embed) {
+        *err = "signature.outputs: span outputs need a graph bundle whose first op is 'embed'";
+        return false;
+      }
+      if (!d->input(InputRole::TypeIds)) {
+        *err = "signature.outputs: span outputs need a 'type_ids' input (the passage is segment 1)";
+        return false;
+      }
+      const int S = d->ops.front().h;
+      const GraphOp& last = d->ops.back();
+      if (last.oh != S || last.ow != 1 || last.cout != 2) {
+        *err = "signature.outputs: span outputs need a last op that writes [" + std::to_string(S) +
+               ", 1, 2] start / end logits per token (it writes [" + std::to_string(last.oh) + ", " + std::to_string(last.ow) +
+               ", " + std::to_string(last.cout) + "])";
+        return false;
+      }
+      const bool spans = d->output(OutputKind::SpanStarts) || d->output(OutputKind::SpanEnds) || d->output(OutputKind::SpanScores);
+      if (!span_supported(S, spans ? d->span_max_len : 1, spans ? d->head_k : 1)) {
+        *err = "signature.outputs: no span kernel for S = " + std::to_string(S) + ", max_answer_length = " +
+               std::to_string(d->span_max_len) + " and k = " + std::to_string(d->head_k) + " (1 <= S <= " +
+               std::to_string(kSpanMaxS) + ", 1 <= max_answer_length <= S, 1 <= k <= " + std::to_string(kSpanMaxK) + ")";
+        return false;
+      }
+    } else if (d->tmpl == Template::Affine) {
       *err = "signature.outputs needs an mlp or graph bundle (an affine bundle has no logits row)";
       return false;
     }
-    if (d->tmpl == Template::Graph && d->output_shape.size() != 1) {
+    if (!d->span_head() && d->tmpl == Template::Graph && d->output_shape.size() != 1) {
       *err = "signature.outputs needs a graph whose output is one vector of logits per row (output_shape has rank " +
              std::to_string(d->output_shape.size()) + ")";
       return false;
@@ -465,7 +582,8 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         return false;
       }
     }
-    d->head_n = d->out_dim > 0x7fffffff ? 0 : (int)d->out_dim;  // the last op's per-row width
+    // the last op's per-row width; a span head answers S start and S end logits per row
+    d->head_n = d->span_head() ? d->ops.front().h : d->out_dim > 0x7fffffff ? 0 : (int)d->out_dim;
     if (!layout_outputs(d, err)) return false;
   }
   return true;

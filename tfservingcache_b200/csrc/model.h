@@ -54,18 +54,37 @@ struct ModelInput {
   int64_t offset = 0;  // elements into the packed request row (inputs in byte-wise sorted name order, S values each)
 };
 
-// One declared output of a multi-output bundle (signature.outputs), computed from the last op's N logits by the head kernel
-// (head.cu). Per row: logits / probabilities [N] float, classes a scalar int64 (two 32-bit words, little-endian),
-// top_k_classes [k] int32, top_k_probabilities [k] float.
-enum class OutputKind { Logits, Probabilities, Classes, TopKClasses, TopKProbabilities };
+// One declared output of a multi-output bundle (signature.outputs). The classification kinds are computed from the last
+// op's N logits by the classify head (head.cu). Per row: logits / probabilities [N] float, classes a scalar int64 (two
+// 32-bit words, little-endian), top_k_classes [k] int32, top_k_probabilities [k] float. The span kinds (question answering)
+// are computed from the last op's [S, 1, 2] per-token logits by the span head (span.cu): start_logits / end_logits [S]
+// float, span_starts / span_ends [k] int32, span_scores [k] float. New kinds go at the end: the forward hop sends the
+// enum's numbers.
+enum class OutputKind {
+  Logits, Probabilities, Classes, TopKClasses, TopKProbabilities,
+  StartLogits, EndLogits, SpanStarts, SpanEnds, SpanScores
+};
+constexpr OutputKind kLastOutputKind = OutputKind::SpanScores;
 struct ModelOutput {
   std::string name;
   OutputKind kind = OutputKind::Logits;
   int64_t offset = 0;  // elements (32-bit words) into the packed response row (outputs in byte-wise sorted name order)
-  int64_t width = 0;   // words per row: N, N, 2, k, k
+  int64_t width = 0;   // words per row (output_form)
 };
 const char* output_kind_name(OutputKind k);
 int output_dtype(OutputKind k);  // TFSC_DT_FLOAT / TFSC_DT_INT64 / TFSC_DT_INT32
+// What one row of an output kind looks like, the one rule behind the packed layout, every response writer and the
+// metadata: `width` 32-bit words holding a scalar (rank 0: classes, one int64 in 2 words) or a vector of `dim` values
+// (rank 1: N or S for the logits kinds, k for the top-k and span kinds).
+struct OutputForm {
+  int64_t width = 0;
+  int dtype = TFSC_DT_FLOAT;
+  int rank = 1;
+  int64_t dim = 0;
+};
+OutputForm output_form(OutputKind k, int head_n, int head_k);
+bool is_span_kind(OutputKind k);        // start_logits .. span_scores
+bool is_span_result_kind(OutputKind k); // span_starts / span_ends / span_scores (they carry k and max_answer_length)
 constexpr int kMaxOutputs = 5;
 
 struct ModelDesc {
@@ -95,8 +114,12 @@ struct ModelDesc {
   }
   // signature.outputs, sorted by name (= packed response row order); empty for single-output bundles (output_name, out_dim
   // elements). With outputs, out_dim is the packed row width and head_n / head_k the logits width and top-k (0: none).
+  // Span outputs: head_n = S, head_k = the number of spans (0: logits only); span_max_len = max_answer_length and
+  // span_sep_id = sep_id (-1: none) are known to the owner only, the kernel's business.
   std::vector<ModelOutput> outputs;
   int head_n = 0, head_k = 0;
+  int span_max_len = 0, span_sep_id = -1;
+  bool span_head() const { return !outputs.empty() && is_span_kind(outputs.front().kind); }
   const ModelOutput* output(OutputKind k) const {
     for (auto& o : outputs)
       if (o.kind == k) return &o;

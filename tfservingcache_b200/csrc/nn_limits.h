@@ -31,4 +31,10 @@ inline bool layernorm_supported(int H) { return H >= 1 && (size_t)H * sizeof(flo
 constexpr int kHeadMaxN = 32768, kHeadMaxK = 32;
 inline bool head_supported(int N, int k) { return N >= 1 && N <= kHeadMaxN && k >= 1 && k <= kHeadMaxK && k <= N; }
 
+// Span head (span.cu): one CTA stages the start and end logits of a row of S tokens and the best end of every start in
+// shared memory (64 KB at S = 4096) and selects the k best (start, end) pairs with end - start < L by k warp argmax
+// rounds. A head with start / end logits only runs as L = k = 1.
+constexpr int kSpanMaxS = 4096, kSpanMaxK = 32;
+inline bool span_supported(int S, int L, int k) { return S >= 1 && S <= kSpanMaxS && L >= 1 && L <= S && k >= 1 && k <= kSpanMaxK; }
+
 }  // namespace tfsc

@@ -605,9 +605,31 @@ static cudaError_t run_head(const ModelDesc& d, const float* logits, int64_t row
       case OutputKind::Classes: o.classes = reinterpret_cast<int*>(p), o.classes_ld = ld; break;
       case OutputKind::TopKClasses: o.topk_idx = reinterpret_cast<int*>(p), o.topk_idx_ld = ld; break;
       case OutputKind::TopKProbabilities: o.topk_prob = p, o.topk_prob_ld = ld; break;
+      default: break;  // span kinds: run_span_head
     }
   }
   return launch_classify_head(logits, (int)rows, d.head_n, d.head_k, o, st);
+}
+
+// question-answering bundles: one span head launch reads the last op's [rows, S, 2] logits and the request's ids / mask /
+// segment ids (`in`, where the embedding reads them) and writes every declared output at its offset in the packed row
+static cudaError_t run_span_head(const ModelDesc& d, const float* logits, const SpanInputs& in, int64_t rows, char* y,
+                                 cudaStream_t st) {
+  SpanOutputs o;
+  float* yf = reinterpret_cast<float*>(y);
+  const int64_t ld = d.out_dim;
+  for (const ModelOutput& m : d.outputs) {
+    float* p = yf + m.offset;
+    switch (m.kind) {
+      case OutputKind::StartLogits: o.start_logits = p, o.start_ld = ld; break;
+      case OutputKind::EndLogits: o.end_logits = p, o.end_ld = ld; break;
+      case OutputKind::SpanStarts: o.starts = reinterpret_cast<int*>(p), o.starts_ld = ld; break;
+      case OutputKind::SpanEnds: o.ends = reinterpret_cast<int*>(p), o.ends_ld = ld; break;
+      case OutputKind::SpanScores: o.scores = p, o.scores_ld = ld; break;
+      default: break;
+    }
+  }
+  return launch_span_head(logits, in, (int)rows, d.head_n, d.span_max_len, d.head_k, o, st);
 }
 
 cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, char* y, char* scratch, void* ws,
@@ -688,6 +710,15 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
         e = launch_avgpool(src, dst, B, o.h * o.w, o.c, st);
       }
       if (e != cudaSuccess) return e;
+    }
+    if (d.span_head()) {
+      SpanInputs in;
+      in.ids = ids;
+      in.mask = d.input(InputRole::Mask) ? mask : nullptr;
+      in.types = types;
+      in.stride = stride;
+      in.sep_id = d.span_sep_id;
+      return run_span_head(d, (const float*)out, in, rows, y, st);
     }
     return d.outputs.empty() ? cudaSuccess : run_head(d, (const float*)out, rows, y, st);
   }

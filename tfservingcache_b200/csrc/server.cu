@@ -486,7 +486,8 @@ static bool plan_outputs(const ModelDesc& d, int64_t rows, const std::vector<int
     }
     p->sel.push_back(*o);
     std::vector<int64_t> sh = dims;
-    if (o->kind != OutputKind::Classes) sh.push_back(o->kind == OutputKind::Logits || o->kind == OutputKind::Probabilities ? d.head_n : d.head_k);
+    const OutputForm f = output_form(o->kind, d.head_n, d.head_k);
+    if (f.rank) sh.push_back(f.dim);
     p->shapes.push_back(sh);
   }
   return true;
@@ -1028,9 +1029,10 @@ static void write_tensor_json(const float* v, const std::vector<int64_t>& shape,
 
 // one value of a packed row as JSON: fp32 as json_float, int32 / int64 as integers
 static void json_word_value(OutputKind k, const uint32_t* w, std::string* s) {
-  if (k == OutputKind::Classes) {
+  const int dt = output_dtype(k);
+  if (dt == TFSC_DT_INT64) {
     *s += std::to_string((int64_t)((uint64_t)w[0] | ((uint64_t)w[1] << 32)));
-  } else if (k == OutputKind::TopKClasses) {
+  } else if (dt == TFSC_DT_INT32) {
     *s += std::to_string((int32_t)w[0]);
   } else {
     float f;
@@ -1069,7 +1071,7 @@ static std::string rest_multi_output_json(const OutputPlan& p, const float* pack
         json_escape(o.name, &b);
         b += ": ";
         const uint32_t* w = words + r * p.out_dim + o.offset;
-        if (o.kind == OutputKind::Classes) {
+        if (output_form(o.kind, 0, 0).rank == 0) {
           json_word_value(o.kind, w, &b);
         } else {
           int64_t idx = 0;
@@ -1089,7 +1091,7 @@ static std::string rest_multi_output_json(const OutputPlan& p, const float* pack
     json_escape(o.name, &b);
     b += ": ";
     int64_t idx = 0;
-    json_nested(o.kind, vals.data(), p.shapes[i], 0, &idx, o.kind == OutputKind::Classes ? 2 : 1, &b);
+    json_nested(o.kind, vals.data(), p.shapes[i], 0, &idx, output_dtype(o.kind) == TFSC_DT_INT64 ? 2 : 1, &b);
   }
   b += "}\n}";
   return b;
@@ -1308,13 +1310,12 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
     for (auto& mi : d.inputs)
       ins += (ins.empty() ? "" : ", ") + tensor_info(mi.name, std::to_string(d.in_dim / (int64_t)d.inputs.size()), "DT_INT32");
     if (d.inputs.empty()) ins = tensor_info(d.input_name, dim, d.input_dtype == TFSC_DT_INT32 ? "DT_INT32" : "DT_FLOAT");
-    // a multi-output model lists every output: logits / probabilities [-1, N], classes [-1] (int64), top-k [-1, k]
+    // a multi-output model lists every output: logits / probabilities [-1, N], classes [-1] (int64), top-k [-1, k],
+    // start / end logits [-1, S], spans [-1, k]
     std::string outs;
     for (auto& mo : d.outputs) {
-      const std::string last = mo.kind == OutputKind::Classes ? ""
-                               : mo.kind == OutputKind::Logits || mo.kind == OutputKind::Probabilities ? std::to_string(d.head_n)
-                                                                                                        : std::to_string(d.head_k);
-      outs += (outs.empty() ? "" : ", ") + tensor_info(mo.name, last, dtype_name(output_dtype(mo.kind)).c_str());
+      const OutputForm f = output_form(mo.kind, d.head_n, d.head_k);
+      outs += (outs.empty() ? "" : ", ") + tensor_info(mo.name, f.rank ? std::to_string(f.dim) : "", dtype_name(f.dtype).c_str());
     }
     if (d.outputs.empty()) outs = tensor_info(d.output_name, odim, "DT_FLOAT");
     std::string b = "{\n\"model_spec\": {\"name\": ";
@@ -1850,6 +1851,36 @@ int tfsc_k_classify_head(const float* logits, int rows, int n, int k, float* pro
   o.topk_prob_ld = k;
   cudaError_t e = launch_classify_head(logits, rows, n, k, o, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "classify_head: %s", cudaGetErrorString(e));
+}
+int tfsc_k_span_head(const float* logits, const int32_t* ids, const int32_t* mask, const int32_t* types, int stride, int rows, int S,
+                     int max_answer_length, int k, int sep_id, float* start_logits, float* end_logits, int32_t* span_starts,
+                     int32_t* span_ends, float* span_scores, void* stream) {
+  if (int rc = check_device()) return rc;
+  const bool spans = span_starts || span_ends || span_scores;
+  if (!logits || rows < 0 || !span_supported(S, spans ? max_answer_length : 1, spans ? k : 1))
+    return fail(TFSC_E_INVALID, "span_head: no kernel for %d rows of S = %d, max_answer_length = %d, k = %d (1 <= S <= %d, "
+                "1 <= max_answer_length <= S, 1 <= k <= %d)", rows, S, max_answer_length, k, kSpanMaxS, kSpanMaxK);
+  if (spans && (!ids || !types || stride < S))
+    return fail(TFSC_E_INVALID, "span_head: spans need the ids and the segment ids, stride >= S (%d < %d)", stride, S);
+  SpanInputs in;
+  in.ids = ids;
+  in.mask = mask;
+  in.types = types;
+  in.stride = stride;
+  in.sep_id = sep_id < 0 ? -1 : sep_id;
+  SpanOutputs o;
+  o.start_logits = start_logits;
+  o.start_ld = S;
+  o.end_logits = end_logits;
+  o.end_ld = S;
+  o.starts = span_starts;
+  o.starts_ld = k;
+  o.ends = span_ends;
+  o.ends_ld = k;
+  o.scores = span_scores;
+  o.scores_ld = k;
+  cudaError_t e = launch_span_head(logits, in, rows, S, max_answer_length, k, o, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "span_head: %s", cudaGetErrorString(e));
 }
 int tfsc_debug_gemm_trace(long long*) {
   return fail(TFSC_E_UNIMPLEMENTED, "no GEMM clock trace: the persistent GEMM kernel it timed is not part of the sm_90a build");

@@ -15,10 +15,14 @@ def _align256(x: int) -> int:
 
 
 OUTPUT_KINDS = ("logits", "probabilities", "classes", "top_k_classes", "top_k_probabilities")
+# question answering (a graph bundle ending in per-token [S, 1, 2] start / end logits, with a type_ids input); the three
+# span kinds carry the same "k" and "max_answer_length" and optionally the same "sep_id"
+SPAN_OUTPUT_KINDS = ("start_logits", "end_logits", "span_starts", "span_ends", "span_scores")
 
 
 def _signature(sig: dict, outputs):
-    """signature.outputs replaces signature.output: a list of {"name", "kind"} (+ "k" for the top-k kinds)."""
+    """signature.outputs replaces signature.output: a list of {"name", "kind"} (+ "k" for the top-k kinds, + "k",
+    "max_answer_length" [, "sep_id"] for the span kinds)."""
     if outputs is None:
         return sig
     sig = {k: v for k, v in sig.items() if k != "output"}
@@ -29,12 +33,14 @@ def _signature(sig: dict, outputs):
 def packed_output_layout(outputs, n):
     """(name, element offset, width, dtype) of every output in a packed response row, in packed order (byte-wise sorted
     names). Offsets and widths count 32-bit words: logits / probabilities n floats, classes 2 words (one little-endian
-    int64), top-k k values (int32 classes, float probabilities). n = the last op's per-row width."""
+    int64), top-k k values (int32 classes, float probabilities), start / end logits n floats, span_starts / span_ends k
+    int32, span_scores k floats. n = the last op's per-row width for the classification kinds, the sequence length S for
+    the span kinds."""
     out, off = [], 0
     for o in sorted(outputs, key=lambda o: o["name"].encode()):
         kind = o["kind"]
-        width = {"logits": n, "probabilities": n, "classes": 2}.get(kind, o.get("k"))
-        dtype = {"classes": "int64", "top_k_classes": "int32"}.get(kind, "float32")
+        width = {"logits": n, "probabilities": n, "classes": 2, "start_logits": n, "end_logits": n}.get(kind, o.get("k"))
+        dtype = {"classes": "int64", "top_k_classes": "int32", "span_starts": "int32", "span_ends": "int32"}.get(kind, "float32")
         out.append((o["name"], off, int(width), dtype))
         off += int(width)
     return out
@@ -176,7 +182,7 @@ def packed_input_order(inputs):
 
 
 def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30522, max_pos=512, labels=2, inputs=None,
-                  outputs=None):
+                  outputs=None, head="classify"):
     """BERT-base fine-tune variant (Devlin et al. 2018) as a graph bundle: token ids int32 [B, seq] -> logits
     [B, labels]. A sequence is an "image" with h = seq tokens, w = 1, c = width; dense layers are 1x1 convs.
     With inputs=None the bundle takes the ids only: the attention mask is derived from them ([PAD] = 0), token_type is 0.
@@ -184,6 +190,9 @@ def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30
     [B, seq] inputs, and the kernels read the attention mask and the segment ids from the request.
     With outputs = a list of {"name", "kind"[, "k"]} (kinds in OUTPUT_KINDS) the bundle answers those outputs, computed
     from the logits on the GPU, in place of the single "logits" output.
+    head="span" makes the question-answering variant (BertForQuestionAnswering): no pooler and no classifier, the last op
+    is the per-token qa_outputs Linear(hidden, 2), a 1x1 conv from buffer 0 writing [B, seq, 1, 2] start / end logits.
+    Its span outputs (SPAN_OUTPUT_KINDS) need inputs with a "type_ids" role.
     Buffers: 0 hidden, 1 qkv / ffn-intermediate, 2 context / post-attention, 3 dense output."""
     ops = [{"op": "embed", "src": -1, "dst": 0, "h": seq, "w": 1, "c": hidden, "vocab": vocab, "max_pos": max_pos, "eps": 1e-12}]
 
@@ -202,7 +211,10 @@ def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30
         ops.append(dense(2, 1, hidden, inter, act="gelu"))
         ops.append(dense(1, 3, inter, hidden))
         ops.append({"op": "layernorm", "src": 3, "res": 2, "dst": 0, "h": seq, "w": 1, "c": hidden, "eps": 1e-12})
-    ops.append({"op": "dense", "src": 0, "dst": 1, "h": 1, "w": 1, "c": hidden, "cout": hidden, "act": "tanh"})   # pooler on [CLS]
-    ops.append({"op": "dense", "src": 1, "dst": -2, "h": 1, "w": 1, "c": hidden, "cout": labels, "act": "none"})
+    if head == "span":
+        ops.append(dense(0, -2, hidden, 2))                                              # qa_outputs: start | end per token
+    else:
+        ops.append({"op": "dense", "src": 0, "dst": 1, "h": 1, "w": 1, "c": hidden, "cout": hidden, "act": "tanh"})  # pooler on [CLS]
+        ops.append({"op": "dense", "src": 1, "dst": -2, "h": 1, "w": 1, "c": hidden, "cout": labels, "act": "none"})
     return _graph_manifest([seq], ops, 4, input_name="input_ids", output_name="logits", input_dtype="int32", inputs=inputs,
                            outputs=outputs)
