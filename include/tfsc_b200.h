@@ -209,9 +209,10 @@ int tfsc_host_list(tfsc_server* s, int node, char* buf, size_t cap);
  * input error; nothing is launched). The same holds for _deadline, _member and _submit.
  * Outputs: a single-output model fills out[0] (DT_FLOAT; out[0].name is not looked at) and ignores out[1..n_out). A model
  * whose manifest declares signature.outputs (logits, probabilities, classes, top_k_classes, top_k_probabilities, or the
- * question-answering start_logits, end_logits, span_starts, span_ends, span_scores) fills out[i] with the output named
- * out[i].name, in the caller's order: dtype (DT_INT64 for classes, DT_INT32 for top_k_classes, span_starts and span_ends,
- * DT_FLOAT otherwise), shape (batch dims, then [N] or [S], nothing or [k]) and nbytes. A NULL, unknown or repeated
+ * question-answering start_logits, end_logits, span_starts, span_ends, span_scores, or the encoder sequence_output,
+ * pooled_output, cls_embedding, mean_embedding) fills out[i] with the output named out[i].name, in the caller's order: dtype
+ * (DT_INT64 for classes, DT_INT32 for top_k_classes, span_starts and span_ends, DT_FLOAT otherwise), shape (batch dims,
+ * then [N], [S] or [H], nothing, [k], or [S, H] for sequence_output) and nbytes. A NULL, unknown or repeated
  * name is TFSC_E_INVALID and the message lists the outputs; a buffer too small for its output is TFSC_E_BUFFER. */
 int tfsc_predict(tfsc_server* s, const char* model_name, const char* version,
                  const tfsc_tensor* in, int n_in, tfsc_tensor* out, int n_out);
@@ -264,7 +265,8 @@ int tfsc_rest_handle(tfsc_server* s, const char* method, const char* url, const 
  * y receives `rows` packed rows the same way. A multi-output model's row is the concatenation of its outputs' rows in
  * byte-wise sorted NAME order, in 32-bit words: logits / probabilities N floats, classes 2 words (the int64 index,
  * little-endian), top_k_classes k int32, top_k_probabilities k floats, start_logits / end_logits S floats, span_starts /
- * span_ends k int32, span_scores k floats; e.g. classes | logits | probabilities is 2 + 2N words per row, logits of row r at
+ * span_ends k int32, span_scores k floats, sequence_output S*H floats (token-major), pooled_output / cls_embedding /
+ * mean_embedding H floats; e.g. classes | logits | probabilities is 2 + 2N words per row, logits of row r at
  * y + r*(2+2N) + 2. A single-output model's row is its out_dim floats. */
 int tfsc_predict_device(tfsc_server* s, int node, const char* model_name, int64_t version,
                         const void* x, int64_t rows, void* y, void* stream);
@@ -381,6 +383,17 @@ int tfsc_k_classify_head(const float* logits, int rows, int n, int k, float* pro
 int tfsc_k_span_head(const float* logits, const int32_t* ids, const int32_t* mask, const int32_t* types, int stride, int rows, int S,
                      int max_answer_length, int k, int sep_id, float* start_logits, float* end_logits, int32_t* span_starts,
                      int32_t* span_ends, float* span_scores, void* stream);
+/* Encoder head of embedding bundles, one launch for the last hidden states hidden[rows, S, H] and, for pooled_output, the
+ * pooler output pooled[rows, H] (fp32, device): sequence_output[rows, S, H] and pooled_output[rows, H] (copies),
+ * cls_embedding[rows, H] = hidden[r, 0] and mean_embedding[rows, H] = sum_p m[p] hidden[r, p] / max(sum_p m[p], 1e-9),
+ * m[p] = mask[q] != 0 (mask NULL: ids[q] != 0), q = r * stride + p (int32, device). normalize_cls / normalize_mean != 0
+ * divide that output by max(||x||_2, 1e-12). The hidden states are read once and every sum runs in an order fixed by S
+ * and H, so a row's bits do not depend on the batch. Every output pointer may be NULL (not written). TFSC_E_INVALID unless
+ * 1 <= S <= 8192 and 1 <= H <= 8192, hidden is given for sequence_output / cls_embedding / mean_embedding, pooled for
+ * pooled_output, and ids with stride >= S for mean_embedding. */
+int tfsc_k_encoder_head(const float* hidden, const float* pooled, const int32_t* ids, const int32_t* mask, int stride, int rows, int S,
+                        int H, int normalize_cls, int normalize_mean, float* sequence_output, float* pooled_output,
+                        float* cls_embedding, float* mean_embedding, void* stream);
 
 #ifdef __cplusplus
 }

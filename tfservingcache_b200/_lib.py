@@ -141,6 +141,7 @@ _sig("tfsc_k_embed", C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_int, 
 _sig("tfsc_k_layernorm", C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_float, vp)
 _sig("tfsc_k_classify_head", C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp)
 _sig("tfsc_k_span_head", C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp)
+_sig("tfsc_k_encoder_head", C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp)
 
 
 class TfscError(RuntimeError):

@@ -105,6 +105,31 @@ struct SpanOutputs {
 cudaError_t launch_span_head(const float* logits, const SpanInputs& in, int rows, int S, int L, int k, const SpanOutputs& o,
                              cudaStream_t s);
 
+// Encoder head (encoder_head.cu): from the last hidden states hidden[rows, S, H] (and the pooler's pooled[rows, H]) writes,
+// for each non-null pointer, row r of that output at ptr + r * ld (ld in 32-bit words): a copy of the hidden states [S, H],
+// a copy of the pooler output [H], the hidden state of token 0 [H], and the masked mean sum_p m[p] h[p] / max(sum_p m[p],
+// 1e-9) [H] with m[p] = mask[q] != 0 (no mask: ids[q] != 0), q = r * stride + p. normalize_cls / normalize_mean divide
+// that output by max(||x||_2, 1e-12). The hidden states are read once; the sums run in an order fixed by S and H alone.
+// cudaErrorInvalidValue outside encoder_head_supported (nn_limits.h).
+struct EncoderInputs {
+  const int* ids = nullptr;
+  const int* mask = nullptr;
+  int64_t stride = 0;
+};
+struct EncoderOutputs {
+  float* sequence = nullptr;
+  int64_t sequence_ld = 0;
+  float* pooled = nullptr;
+  int64_t pooled_ld = 0;
+  float* cls = nullptr;
+  int64_t cls_ld = 0;
+  float* mean = nullptr;
+  int64_t mean_ld = 0;
+  bool normalize_cls = false, normalize_mean = false;
+};
+cudaError_t launch_encoder_head(const float* hidden, const float* pooled, const EncoderInputs& in, int rows, int S, int H,
+                                const EncoderOutputs& o, cudaStream_t s);
+
 // wgmma 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
 bool gemm_tc_supported(const float* A, const float* B, const float* bias, const float* R, const float* C, int M, int N, int K,
                        int lda);

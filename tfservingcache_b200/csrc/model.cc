@@ -38,14 +38,19 @@ const char* output_kind_name(OutputKind k) {
     case OutputKind::EndLogits: return "end_logits";
     case OutputKind::SpanStarts: return "span_starts";
     case OutputKind::SpanEnds: return "span_ends";
-    default: return "span_scores";
+    case OutputKind::SpanScores: return "span_scores";
+    case OutputKind::SequenceOutput: return "sequence_output";
+    case OutputKind::PooledOutput: return "pooled_output";
+    case OutputKind::ClsEmbedding: return "cls_embedding";
+    default: return "mean_embedding";
   }
 }
 
 int output_dtype(OutputKind k) { return output_form(k, 0, 0).dtype; }
 
-bool is_span_kind(OutputKind k) { return k >= OutputKind::StartLogits; }
-bool is_span_result_kind(OutputKind k) { return k >= OutputKind::SpanStarts; }
+bool is_span_kind(OutputKind k) { return k >= OutputKind::StartLogits && k <= OutputKind::SpanScores; }
+bool is_span_result_kind(OutputKind k) { return k >= OutputKind::SpanStarts && k <= OutputKind::SpanScores; }
+bool is_encoder_kind(OutputKind k) { return k >= OutputKind::SequenceOutput && k <= OutputKind::MeanEmbedding; }
 
 OutputForm output_form(OutputKind k, int head_n, int head_k) {
   OutputForm f;
@@ -56,14 +61,24 @@ OutputForm output_form(OutputKind k, int head_n, int head_k) {
     case OutputKind::SpanEnds: f.width = head_k, f.dtype = TFSC_DT_INT32; break;
     case OutputKind::TopKProbabilities:
     case OutputKind::SpanScores: f.width = head_k; break;
-    default: f.width = head_n; break;  // logits, probabilities, start_logits, end_logits
+    case OutputKind::SequenceOutput:  // encoder bundles: head_k = S, head_n = H
+      f.width = (int64_t)head_k * head_n, f.rank = 2, f.dims[0] = head_k, f.dims[1] = head_n;
+      return f;
+    default: f.width = head_n; break;  // logits, probabilities, start_logits, end_logits, the [H] embedding kinds
   }
-  f.dim = f.rank ? f.width : 1;
+  f.dims[0] = f.rank ? f.width : 1;
   return f;
 }
 
 bool layout_outputs(ModelDesc* d, std::string* err) {
-  if (d->span_head()) {
+  if (d->encoder_head()) {
+    if (!encoder_head_supported(d->head_k, d->head_n)) {
+      *err = "signature.outputs: no encoder head kernel for S = " + std::to_string(d->head_k) + " and H = " +
+             std::to_string(d->head_n) + " (1 <= S <= " + std::to_string(kEncoderMaxS) + ", 1 <= H <= " +
+             std::to_string(kEncoderMaxH) + ")";
+      return false;
+    }
+  } else if (d->span_head()) {
     // max_answer_length is the owner's business, so only S and k decide whether a row can be laid out
     const bool spans = d->output(OutputKind::SpanStarts) || d->output(OutputKind::SpanEnds) || d->output(OutputKind::SpanScores);
     if (!span_supported(d->head_n, 1, spans ? d->head_k : 1) || (!spans && d->head_k != 0)) {
@@ -240,9 +255,14 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         else if (kind == "span_starts") mo.kind = OutputKind::SpanStarts;
         else if (kind == "span_ends") mo.kind = OutputKind::SpanEnds;
         else if (kind == "span_scores") mo.kind = OutputKind::SpanScores;
+        else if (kind == "sequence_output") mo.kind = OutputKind::SequenceOutput;
+        else if (kind == "pooled_output") mo.kind = OutputKind::PooledOutput;
+        else if (kind == "cls_embedding") mo.kind = OutputKind::ClsEmbedding;
+        else if (kind == "mean_embedding") mo.kind = OutputKind::MeanEmbedding;
         else {
           *err = "signature.outputs: unknown kind '" + kind + "' (logits, probabilities, classes, top_k_classes, top_k_probabilities, "
-                 "start_logits, end_logits, span_starts, span_ends, span_scores)";
+                 "start_logits, end_logits, span_starts, span_ends, span_scores, sequence_output, pooled_output, cls_embedding, "
+                 "mean_embedding)";
           return false;
         }
         if (mo.name.empty()) {
@@ -254,6 +274,32 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
             *err = "signature.outputs: duplicate " + std::string(o.name == mo.name ? "name '" + mo.name + "'" : "kind '" + kind + "'");
             return false;
           }
+        if (!d->outputs.empty() && is_encoder_kind(d->outputs.front().kind) != is_encoder_kind(mo.kind)) {
+          *err = "signature.outputs: encoder outputs (sequence_output, pooled_output, cls_embedding, mean_embedding) cannot be mixed"
+                 " with classification or span outputs ('" + mo.name + "' is " + kind + ")";
+          return false;
+        }
+        const bool normalizable = mo.kind == OutputKind::ClsEmbedding || mo.kind == OutputKind::MeanEmbedding;
+        if (const Json* nj = oj.get("normalize")) {
+          if (!normalizable) {
+            *err = "signature.outputs: 'normalize' belongs to cls_embedding and mean_embedding ('" + mo.name + "' is " + kind + ")";
+            return false;
+          }
+          if (nj->type != Json::Bool) {
+            *err = "signature.outputs: '" + mo.name + "' has a 'normalize' that is not true or false";
+            return false;
+          }
+          (mo.kind == OutputKind::ClsEmbedding ? d->normalize_cls : d->normalize_mean) = nj->b;
+        }
+        if (is_encoder_kind(mo.kind)) {
+          if (oj.get("k") || oj.get("max_answer_length") || oj.get("sep_id")) {
+            *err = "signature.outputs: 'k', 'max_answer_length' and 'sep_id' do not apply to encoder outputs ('" + mo.name + "' is " +
+                   kind + ")";
+            return false;
+          }
+          d->outputs.push_back(mo);
+          continue;
+        }
         if (!d->outputs.empty() && is_span_kind(d->outputs.front().kind) != is_span_kind(mo.kind)) {
           *err = "signature.outputs: span outputs (start_logits, end_logits, span_starts, span_ends, span_scores) cannot be mixed"
                  " with classification outputs ('" + mo.name + "' is " + kind + ")";
@@ -535,7 +581,42 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
   }
   finish(d);
   if (!d->outputs.empty()) {
-    if (d->span_head()) {
+    if (d->encoder_head()) {
+      // the encoder head reads the last hidden states [S, 1, H]: what the last op writes, or, when the last op is the pooler
+      // (a tanh dense over token 0), its source buffer; and the request's ids / mask where the embedding reads them
+      if (d->tmpl != Template::Graph) {
+        *err = "signature.outputs: encoder outputs need a graph bundle (a BERT encoder ending in its hidden states or pooler)";
+        return false;
+      }
+      if (d->ops.front().kind != OpKind::Embed) {
+        *err = "signature.outputs: encoder outputs need a graph bundle whose first op is 'embed'";
+        return false;
+      }
+      const int S = d->ops.front().h, H = d->ops.front().c;
+      const GraphOp& last = d->ops.back();
+      const GraphOp* prev = d->ops.size() >= 2 ? &d->ops[d->ops.size() - 2] : nullptr;
+      const bool hidden = last.oh == S && last.ow == 1 && last.cout == H;
+      const bool pooler = last.kind == OpKind::Dense && last.act == 3 && last.c == H && last.cout == H && last.src >= 0 &&
+                          last.lda == (int64_t)S * H && prev && prev->dst == last.src &&
+                          prev->oh == S && prev->ow == 1 && prev->cout == H;
+      if (!hidden && !pooler) {
+        const std::string sh = "[" + std::to_string(S) + ", 1, " + std::to_string(H) + "]";
+        *err = "signature.outputs: encoder outputs need a last op that writes the " + sh + " hidden states, or a tanh pooler"
+               " dense over token 0 of the " + sh + " hidden states the op before it writes (it writes [" +
+               std::to_string(last.oh) + ", " + std::to_string(last.ow) + ", " + std::to_string(last.cout) + "])";
+        return false;
+      }
+      d->encoder_pooler = pooler;
+      if (d->output(OutputKind::PooledOutput) && !pooler) {
+        *err = "signature.outputs: pooled_output needs a bundle whose last op is the pooler (a tanh dense over token 0)";
+        return false;
+      }
+      if (!encoder_head_supported(S, H)) {
+        *err = "signature.outputs: no encoder head kernel for S = " + std::to_string(S) + " and H = " + std::to_string(H) +
+               " (1 <= S <= " + std::to_string(kEncoderMaxS) + ", 1 <= H <= " + std::to_string(kEncoderMaxH) + ")";
+        return false;
+      }
+    } else if (d->span_head()) {
       // the span head reads the request's ids / mask / segment ids where the embedding does, and the per-token start / end
       // logits [S, 1, 2] of the last op
       if (d->tmpl != Template::Graph) {
@@ -569,7 +650,7 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       *err = "signature.outputs needs an mlp or graph bundle (an affine bundle has no logits row)";
       return false;
     }
-    if (!d->span_head() && d->tmpl == Template::Graph && d->output_shape.size() != 1) {
+    if (!d->span_head() && !d->encoder_head() && d->tmpl == Template::Graph && d->output_shape.size() != 1) {
       *err = "signature.outputs needs a graph whose output is one vector of logits per row (output_shape has rank " +
              std::to_string(d->output_shape.size()) + ")";
       return false;
@@ -582,8 +663,10 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         return false;
       }
     }
-    // the last op's per-row width; a span head answers S start and S end logits per row
+    // the last op's per-row width; a span head answers S start and S end logits per row; an encoder head's rows are
+    // [S, H] (head_k = S) and [H] (head_n = H)
     d->head_n = d->span_head() ? d->ops.front().h : d->out_dim > 0x7fffffff ? 0 : (int)d->out_dim;
+    if (d->encoder_head()) d->head_n = d->ops.front().c, d->head_k = d->ops.front().h;
     if (!layout_outputs(d, err)) return false;
   }
   return true;

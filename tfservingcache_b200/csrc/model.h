@@ -58,13 +58,16 @@ struct ModelInput {
 // op's N logits by the classify head (head.cu). Per row: logits / probabilities [N] float, classes a scalar int64 (two
 // 32-bit words, little-endian), top_k_classes [k] int32, top_k_probabilities [k] float. The span kinds (question answering)
 // are computed from the last op's [S, 1, 2] per-token logits by the span head (span.cu): start_logits / end_logits [S]
-// float, span_starts / span_ends [k] int32, span_scores [k] float. New kinds go at the end: the forward hop sends the
-// enum's numbers.
+// float, span_starts / span_ends [k] int32, span_scores [k] float. The encoder kinds (embeddings) are computed from the
+// last hidden states [S, 1, H] (and the pooler's [H]) by the encoder head (encoder_head.cu): sequence_output [S, H] float,
+// pooled_output / cls_embedding / mean_embedding [H] float. New kinds go at the end: the forward hop sends the enum's
+// numbers.
 enum class OutputKind {
   Logits, Probabilities, Classes, TopKClasses, TopKProbabilities,
-  StartLogits, EndLogits, SpanStarts, SpanEnds, SpanScores
+  StartLogits, EndLogits, SpanStarts, SpanEnds, SpanScores,
+  SequenceOutput, PooledOutput, ClsEmbedding, MeanEmbedding
 };
-constexpr OutputKind kLastOutputKind = OutputKind::SpanScores;
+constexpr OutputKind kLastOutputKind = OutputKind::MeanEmbedding;
 struct ModelOutput {
   std::string name;
   OutputKind kind = OutputKind::Logits;
@@ -74,17 +77,19 @@ struct ModelOutput {
 const char* output_kind_name(OutputKind k);
 int output_dtype(OutputKind k);  // TFSC_DT_FLOAT / TFSC_DT_INT64 / TFSC_DT_INT32
 // What one row of an output kind looks like, the one rule behind the packed layout, every response writer and the
-// metadata: `width` 32-bit words holding a scalar (rank 0: classes, one int64 in 2 words) or a vector of `dim` values
-// (rank 1: N or S for the logits kinds, k for the top-k and span kinds).
+// metadata: `width` 32-bit words holding a scalar (rank 0: classes, one int64 in 2 words), a vector of dims[0] values
+// (rank 1: N or S for the logits kinds, k for the top-k and span kinds, H for the embedding kinds) or a dims[0] x dims[1]
+// matrix (rank 2: sequence_output, S x H).
 struct OutputForm {
   int64_t width = 0;
   int dtype = TFSC_DT_FLOAT;
   int rank = 1;
-  int64_t dim = 0;
+  int64_t dims[2] = {0, 0};
 };
 OutputForm output_form(OutputKind k, int head_n, int head_k);
 bool is_span_kind(OutputKind k);        // start_logits .. span_scores
 bool is_span_result_kind(OutputKind k); // span_starts / span_ends / span_scores (they carry k and max_answer_length)
+bool is_encoder_kind(OutputKind k);     // sequence_output, pooled_output, cls_embedding, mean_embedding
 constexpr int kMaxOutputs = 5;
 
 struct ModelDesc {
@@ -116,10 +121,14 @@ struct ModelDesc {
   // elements). With outputs, out_dim is the packed row width and head_n / head_k the logits width and top-k (0: none).
   // Span outputs: head_n = S, head_k = the number of spans (0: logits only); span_max_len = max_answer_length and
   // span_sep_id = sep_id (-1: none) are known to the owner only, the kernel's business.
+  // Encoder outputs: head_n = H, head_k = S; encoder_pooler = the last op is the pooler (it writes pooled_output, and the
+  // hidden states are its source buffer); normalize_cls / normalize_mean, like max_answer_length, are the owner's.
   std::vector<ModelOutput> outputs;
   int head_n = 0, head_k = 0;
   int span_max_len = 0, span_sep_id = -1;
+  bool encoder_pooler = false, normalize_cls = false, normalize_mean = false;
   bool span_head() const { return !outputs.empty() && is_span_kind(outputs.front().kind); }
+  bool encoder_head() const { return !outputs.empty() && is_encoder_kind(outputs.front().kind); }
   const ModelOutput* output(OutputKind k) const {
     for (auto& o : outputs)
       if (o.kind == k) return &o;

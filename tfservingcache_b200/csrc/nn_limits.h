@@ -37,4 +37,10 @@ inline bool head_supported(int N, int k) { return N >= 1 && N <= kHeadMaxN && k 
 constexpr int kSpanMaxS = 4096, kSpanMaxK = 32;
 inline bool span_supported(int S, int L, int k) { return S >= 1 && S <= kSpanMaxS && L >= 1 && L <= S && k >= 1 && k <= kSpanMaxK; }
 
+// Encoder head (encoder_head.cu): a cluster of up to 8 CTAs per row streams the [S, H] hidden states once; each CTA keeps
+// fp32 partial sums of its tokens for H columns in shared memory (32 KB at H = 8192), and in-row offsets p * H + c are
+// 32-bit (S * H <= 2^26).
+constexpr int kEncoderMaxS = 8192, kEncoderMaxH = 8192;
+inline bool encoder_head_supported(int S, int H) { return S >= 1 && S <= kEncoderMaxS && H >= 1 && H <= kEncoderMaxH; }
+
 }  // namespace tfsc

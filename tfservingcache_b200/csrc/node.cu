@@ -632,6 +632,29 @@ static cudaError_t run_span_head(const ModelDesc& d, const float* logits, const 
   return launch_span_head(logits, in, (int)rows, d.head_n, d.span_max_len, d.head_k, o, st);
 }
 
+// embedding bundles: one encoder head launch reads the last hidden states [rows, S, H] (and, with a pooler, its [rows, H]
+// output) and the request's ids / mask (`in`, where the embedding reads them), and writes every declared output at its
+// offset in the packed row
+static cudaError_t run_encoder_head(const ModelDesc& d, const float* hidden, const float* pooled, const EncoderInputs& in,
+                                    int64_t rows, char* y, cudaStream_t st) {
+  EncoderOutputs o;
+  float* yf = reinterpret_cast<float*>(y);
+  const int64_t ld = d.out_dim;
+  for (const ModelOutput& m : d.outputs) {
+    float* p = yf + m.offset;
+    switch (m.kind) {
+      case OutputKind::SequenceOutput: o.sequence = p, o.sequence_ld = ld; break;
+      case OutputKind::PooledOutput: o.pooled = p, o.pooled_ld = ld; break;
+      case OutputKind::ClsEmbedding: o.cls = p, o.cls_ld = ld; break;
+      case OutputKind::MeanEmbedding: o.mean = p, o.mean_ld = ld; break;
+      default: break;
+    }
+  }
+  o.normalize_cls = d.normalize_cls;
+  o.normalize_mean = d.normalize_mean;
+  return launch_encoder_head(hidden, pooled, in, (int)rows, d.head_k, d.head_n, o, st);
+}
+
 cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, char* y, char* scratch, void* ws,
                             size_t ws_cap, cudaStream_t st) {
   const ModelDesc& d = dm.desc;
@@ -710,6 +733,16 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
         e = launch_avgpool(src, dst, B, o.h * o.w, o.c, st);
       }
       if (e != cudaSuccess) return e;
+    }
+    if (d.encoder_head()) {
+      // with a pooler the hidden states are the pooler's source buffer and `out` holds its [rows, H] output; without one
+      // the last op wrote the hidden states to `out`
+      EncoderInputs in;
+      in.ids = ids;
+      in.mask = d.input(InputRole::Mask) ? mask : nullptr;
+      in.stride = stride ? stride : d.ops.front().h;
+      if (d.encoder_pooler) return run_encoder_head(d, (const float*)buf(d.ops.back().src), (const float*)out, in, rows, y, st);
+      return run_encoder_head(d, (const float*)out, nullptr, in, rows, y, st);
     }
     if (d.span_head()) {
       SpanInputs in;

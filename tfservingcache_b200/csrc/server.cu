@@ -487,7 +487,7 @@ static bool plan_outputs(const ModelDesc& d, int64_t rows, const std::vector<int
     p->sel.push_back(*o);
     std::vector<int64_t> sh = dims;
     const OutputForm f = output_form(o->kind, d.head_n, d.head_k);
-    if (f.rank) sh.push_back(f.dim);
+    for (int r = 0; r < f.rank; ++r) sh.push_back(f.dims[r]);
     p->shapes.push_back(sh);
   }
   return true;
@@ -1071,11 +1071,14 @@ static std::string rest_multi_output_json(const OutputPlan& p, const float* pack
         json_escape(o.name, &b);
         b += ": ";
         const uint32_t* w = words + r * p.out_dim + o.offset;
-        if (output_form(o.kind, 0, 0).rank == 0) {
+        const size_t rank = (size_t)output_form(o.kind, 0, 0).rank;
+        if (rank == 0) {
           json_word_value(o.kind, w, &b);
         } else {
+          // one row's value: the trailing `rank` dims of the plan's shape ([N], [k], [H] or sequence_output's [S, H])
+          const std::vector<int64_t>& sh = p.shapes[i];
           int64_t idx = 0;
-          json_nested(o.kind, w, {o.width}, 0, &idx, 1, &b);
+          json_nested(o.kind, w, std::vector<int64_t>(sh.end() - (ptrdiff_t)rank, sh.end()), 0, &idx, 1, &b);
         }
       }
       b += "}";
@@ -1299,25 +1302,31 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
     if (rc < 0) return fail_http(http_for(rc), err);
     std::string dim = d.tmpl == Template::Affine ? "" : std::to_string(d.in_dim);
     std::string odim = d.tmpl == Template::Affine ? "" : std::to_string(d.out_dim);
-    auto tensor_info = [](const std::string& key, const std::string& last_dim, const char* dtype) {
+    // the batch dimension -1, then `dims` (none for a scalar per row)
+    auto tensor_info = [](const std::string& key, const std::vector<std::string>& dims, const char* dtype) {
       std::string t = "\"" + key + "\": {\"dtype\": \"" + dtype + "\", \"tensor_shape\": {\"dim\": [{\"size\": \"-1\", \"name\": \"\"}";
-      if (!last_dim.empty()) t += ", {\"size\": \"" + last_dim + "\", \"name\": \"\"}";
+      for (auto& dim : dims) t += ", {\"size\": \"" + dim + "\", \"name\": \"\"}";
       t += "], \"unknown_rank\": false}, \"name\": \"" + key + ":0\"}";
       return t;
     };
     // every declared input of a multi-input model is DT_INT32 [-1, S]
     std::string ins;
     for (auto& mi : d.inputs)
-      ins += (ins.empty() ? "" : ", ") + tensor_info(mi.name, std::to_string(d.in_dim / (int64_t)d.inputs.size()), "DT_INT32");
-    if (d.inputs.empty()) ins = tensor_info(d.input_name, dim, d.input_dtype == TFSC_DT_INT32 ? "DT_INT32" : "DT_FLOAT");
+      ins += (ins.empty() ? "" : ", ") + tensor_info(mi.name, {std::to_string(d.in_dim / (int64_t)d.inputs.size())}, "DT_INT32");
+    if (d.inputs.empty())
+      ins = tensor_info(d.input_name, dim.empty() ? std::vector<std::string>{} : std::vector<std::string>{dim},
+                        d.input_dtype == TFSC_DT_INT32 ? "DT_INT32" : "DT_FLOAT");
     // a multi-output model lists every output: logits / probabilities [-1, N], classes [-1] (int64), top-k [-1, k],
-    // start / end logits [-1, S], spans [-1, k]
+    // start / end logits [-1, S], spans [-1, k], sequence_output [-1, S, H], the other encoder outputs [-1, H]
     std::string outs;
     for (auto& mo : d.outputs) {
       const OutputForm f = output_form(mo.kind, d.head_n, d.head_k);
-      outs += (outs.empty() ? "" : ", ") + tensor_info(mo.name, f.rank ? std::to_string(f.dim) : "", dtype_name(f.dtype).c_str());
+      std::vector<std::string> dims;
+      for (int r = 0; r < f.rank; ++r) dims.push_back(std::to_string(f.dims[r]));
+      outs += (outs.empty() ? "" : ", ") + tensor_info(mo.name, dims, dtype_name(f.dtype).c_str());
     }
-    if (d.outputs.empty()) outs = tensor_info(d.output_name, odim, "DT_FLOAT");
+    if (d.outputs.empty())
+      outs = tensor_info(d.output_name, odim.empty() ? std::vector<std::string>{} : std::vector<std::string>{odim}, "DT_FLOAT");
     std::string b = "{\n\"model_spec\": {\"name\": ";
     json_escape(name, &b);
     b += ", \"signature_name\": \"\", \"version\": \"" + std::to_string(id.version) + "\"},\n\"metadata\": {\"signature_def\": {\"signature_def\": {\"serving_default\": {\"inputs\": {" +
@@ -1881,6 +1890,36 @@ int tfsc_k_span_head(const float* logits, const int32_t* ids, const int32_t* mas
   o.scores_ld = k;
   cudaError_t e = launch_span_head(logits, in, rows, S, max_answer_length, k, o, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "span_head: %s", cudaGetErrorString(e));
+}
+int tfsc_k_encoder_head(const float* hidden, const float* pooled, const int32_t* ids, const int32_t* mask, int stride, int rows, int S,
+                        int H, int normalize_cls, int normalize_mean, float* sequence_output, float* pooled_output,
+                        float* cls_embedding, float* mean_embedding, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (rows < 0 || !encoder_head_supported(S, H))
+    return fail(TFSC_E_INVALID, "encoder_head: no kernel for %d rows of S = %d, H = %d (1 <= S <= %d, 1 <= H <= %d)", rows, S, H,
+                kEncoderMaxS, kEncoderMaxH);
+  if (!hidden && (sequence_output || cls_embedding || mean_embedding))
+    return fail(TFSC_E_INVALID, "encoder_head: sequence_output, cls_embedding and mean_embedding need the hidden states");
+  if (!pooled && pooled_output) return fail(TFSC_E_INVALID, "encoder_head: pooled_output needs the pooler output");
+  if (mean_embedding && (!ids || stride < S))
+    return fail(TFSC_E_INVALID, "encoder_head: mean_embedding needs the ids, stride >= S (%d < %d)", stride, S);
+  EncoderInputs in;
+  in.ids = ids;
+  in.mask = mask;
+  in.stride = stride;
+  EncoderOutputs o;
+  o.sequence = sequence_output;
+  o.sequence_ld = (int64_t)S * H;
+  o.pooled = pooled_output;
+  o.pooled_ld = H;
+  o.cls = cls_embedding;
+  o.cls_ld = H;
+  o.mean = mean_embedding;
+  o.mean_ld = H;
+  o.normalize_cls = normalize_cls != 0;
+  o.normalize_mean = normalize_mean != 0;
+  cudaError_t e = launch_encoder_head(hidden, pooled, in, rows, S, H, o, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "encoder_head: %s", cudaGetErrorString(e));
 }
 int tfsc_debug_gemm_trace(long long*) {
   return fail(TFSC_E_UNIMPLEMENTED, "no GEMM clock trace: the persistent GEMM kernel it timed is not part of the sm_90a build");

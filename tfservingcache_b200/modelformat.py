@@ -18,6 +18,9 @@ OUTPUT_KINDS = ("logits", "probabilities", "classes", "top_k_classes", "top_k_pr
 # question answering (a graph bundle ending in per-token [S, 1, 2] start / end logits, with a type_ids input); the three
 # span kinds carry the same "k" and "max_answer_length" and optionally the same "sep_id"
 SPAN_OUTPUT_KINDS = ("start_logits", "end_logits", "span_starts", "span_ends", "span_scores")
+# embeddings (a graph bundle ending in the last hidden states [S, 1, H], or in the pooler over them); cls_embedding and
+# mean_embedding may carry "normalize": true
+ENCODER_OUTPUT_KINDS = ("sequence_output", "pooled_output", "cls_embedding", "mean_embedding")
 
 
 def _signature(sig: dict, outputs):
@@ -30,32 +33,40 @@ def _signature(sig: dict, outputs):
     return sig
 
 
-def packed_output_layout(outputs, n):
+def packed_output_layout(outputs, n, seq=None):
     """(name, element offset, width, dtype) of every output in a packed response row, in packed order (byte-wise sorted
     names). Offsets and widths count 32-bit words: logits / probabilities n floats, classes 2 words (one little-endian
     int64), top-k k values (int32 classes, float probabilities), start / end logits n floats, span_starts / span_ends k
-    int32, span_scores k floats. n = the last op's per-row width for the classification kinds, the sequence length S for
-    the span kinds."""
+    int32, span_scores k floats, sequence_output seq * n floats, pooled_output / cls_embedding / mean_embedding n floats.
+    n = the last op's per-row width for the classification kinds, the sequence length S for the span kinds, the hidden
+    width H for the encoder kinds (seq = S)."""
     out, off = [], 0
     for o in sorted(outputs, key=lambda o: o["name"].encode()):
         kind = o["kind"]
-        width = {"logits": n, "probabilities": n, "classes": 2, "start_logits": n, "end_logits": n}.get(kind, o.get("k"))
+        width = {"logits": n, "probabilities": n, "classes": 2, "start_logits": n, "end_logits": n, "pooled_output": n,
+                 "cls_embedding": n, "mean_embedding": n}.get(kind, o.get("k"))
+        if kind == "sequence_output":
+            width = seq * n
         dtype = {"classes": "int64", "top_k_classes": "int32", "span_starts": "int32", "span_ends": "int32"}.get(kind, "float32")
         out.append((o["name"], off, int(width), dtype))
         off += int(width)
     return out
 
 
-def split_packed_rows(rows_words: np.ndarray, outputs, n) -> dict:
-    """{name: array} from packed rows ([rows, out_dim] of any 4-byte dtype, e.g. the float32 view of tfsc_predict_device's y)."""
+def split_packed_rows(rows_words: np.ndarray, outputs, n, seq=None) -> dict:
+    """{name: array} from packed rows ([rows, out_dim] of any 4-byte dtype, e.g. the float32 view of tfsc_predict_device's y).
+    n and seq as for packed_output_layout; sequence_output comes out as [rows, seq, n]."""
     w = np.ascontiguousarray(rows_words).view(np.uint32).reshape(len(rows_words), -1)
+    kinds = {o["name"]: o["kind"] for o in outputs}
     res = {}
-    for name, off, width, dtype in packed_output_layout(outputs, n):
+    for name, off, width, dtype in packed_output_layout(outputs, n, seq):
         part = np.ascontiguousarray(w[:, off:off + width])
         if dtype == "int64":
             res[name] = part.view("<i8").reshape(-1)
         else:
             res[name] = part.view("<i4" if dtype == "int32" else "<f4")
+        if kinds[name] == "sequence_output":
+            res[name] = res[name].reshape(len(w), seq, n)
     return res
 
 
@@ -182,7 +193,7 @@ def packed_input_order(inputs):
 
 
 def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30522, max_pos=512, labels=2, inputs=None,
-                  outputs=None, head="classify"):
+                  outputs=None, head="classify", pooler=True):
     """BERT-base fine-tune variant (Devlin et al. 2018) as a graph bundle: token ids int32 [B, seq] -> logits
     [B, labels]. A sequence is an "image" with h = seq tokens, w = 1, c = width; dense layers are 1x1 convs.
     With inputs=None the bundle takes the ids only: the attention mask is derived from them ([PAD] = 0), token_type is 0.
@@ -193,6 +204,10 @@ def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30
     head="span" makes the question-answering variant (BertForQuestionAnswering): no pooler and no classifier, the last op
     is the per-token qa_outputs Linear(hidden, 2), a 1x1 conv from buffer 0 writing [B, seq, 1, 2] start / end logits.
     Its span outputs (SPAN_OUTPUT_KINDS) need inputs with a "type_ids" role.
+    head="encoder" makes the encoder without a classifier (BertModel), answering ENCODER_OUTPUT_KINDS: with pooler=True
+    the last op is the pooler (a tanh dense over token 0 of buffer 0, writing [B, hidden]) and the hidden states are
+    buffer 0; with pooler=False (BertModel(add_pooling_layer=False)) the last LayerNorm writes the [B, seq, 1, hidden]
+    hidden states as the response.
     Buffers: 0 hidden, 1 qkv / ffn-intermediate, 2 context / post-attention, 3 dense output."""
     ops = [{"op": "embed", "src": -1, "dst": 0, "h": seq, "w": 1, "c": hidden, "vocab": vocab, "max_pos": max_pos, "eps": 1e-12}]
 
@@ -211,7 +226,12 @@ def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30
         ops.append(dense(2, 1, hidden, inter, act="gelu"))
         ops.append(dense(1, 3, inter, hidden))
         ops.append({"op": "layernorm", "src": 3, "res": 2, "dst": 0, "h": seq, "w": 1, "c": hidden, "eps": 1e-12})
-    if head == "span":
+    if head == "encoder":
+        if pooler:
+            ops.append({"op": "dense", "src": 0, "dst": -2, "h": 1, "w": 1, "c": hidden, "cout": hidden, "act": "tanh"})
+        else:
+            ops[-1]["dst"] = -2                                                          # the last LayerNorm answers
+    elif head == "span":
         ops.append(dense(0, -2, hidden, 2))                                              # qa_outputs: start | end per token
     else:
         ops.append({"op": "dense", "src": 0, "dst": 1, "h": 1, "w": 1, "c": hidden, "cout": hidden, "act": "tanh"})  # pooler on [CLS]

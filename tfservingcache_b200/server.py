@@ -92,6 +92,9 @@ class Server:
         if out_capacity_elems is None:
             lead = arrays[0].shape[0] if arrays[0].ndim > 1 else 1
             out_capacity_elems = max(sum(a.size for a in arrays) * 4 + 65536, lead * 32768 * 2)
+            if np.issubdtype(arrays[0].dtype, np.integer):
+                # token-id requests: room for an encoder's [rows, S, H] sequence_output up to H = 1024
+                out_capacity_elems = max(out_capacity_elems, arrays[0].size * 1024)
         ys, touts = [], (TfscTensor * len(outputs))()
         for t, name in zip(touts, outputs):
             y = np.empty(out_capacity_elems * 4, dtype=np.uint8)
