@@ -210,9 +210,11 @@ int tfsc_host_list(tfsc_server* s, int node, char* buf, size_t cap);
  * Outputs: a single-output model fills out[0] (DT_FLOAT; out[0].name is not looked at) and ignores out[1..n_out). A model
  * whose manifest declares signature.outputs (logits, probabilities, classes, top_k_classes, top_k_probabilities, or the
  * question-answering start_logits, end_logits, span_starts, span_ends, span_scores, or the encoder sequence_output,
- * pooled_output, cls_embedding, mean_embedding) fills out[i] with the output named out[i].name, in the caller's order: dtype
- * (DT_INT64 for classes, DT_INT32 for top_k_classes, span_starts and span_ends, DT_FLOAT otherwise), shape (batch dims,
- * then [N], [S] or [H], nothing, [k], or [S, H] for sequence_output) and nbytes. A NULL, unknown or repeated
+ * pooled_output, cls_embedding, mean_embedding, or the fill-mask masked_positions, masked_top_k_ids,
+ * masked_top_k_probabilities, masked_top_k_logits) fills out[i] with the output named out[i].name, in the caller's order:
+ * dtype (DT_INT64 for classes, DT_INT32 for top_k_classes, span_starts, span_ends, masked_positions and masked_top_k_ids,
+ * DT_FLOAT otherwise), shape (batch dims, then [N], [S], [H] or [M], nothing, [k], [S, H] for sequence_output or [M, k]
+ * for the fill-mask top-k outputs) and nbytes. A NULL, unknown or repeated
  * name is TFSC_E_INVALID and the message lists the outputs; a buffer too small for its output is TFSC_E_BUFFER. */
 int tfsc_predict(tfsc_server* s, const char* model_name, const char* version,
                  const tfsc_tensor* in, int n_in, tfsc_tensor* out, int n_out);
@@ -266,7 +268,8 @@ int tfsc_rest_handle(tfsc_server* s, const char* method, const char* url, const 
  * byte-wise sorted NAME order, in 32-bit words: logits / probabilities N floats, classes 2 words (the int64 index,
  * little-endian), top_k_classes k int32, top_k_probabilities k floats, start_logits / end_logits S floats, span_starts /
  * span_ends k int32, span_scores k floats, sequence_output S*H floats (token-major), pooled_output / cls_embedding /
- * mean_embedding H floats; e.g. classes | logits | probabilities is 2 + 2N words per row, logits of row r at
+ * mean_embedding H floats, masked_positions M int32, masked_top_k_ids M*k int32, masked_top_k_probabilities /
+ * masked_top_k_logits M*k floats (slot-major); e.g. classes | logits | probabilities is 2 + 2N words per row, logits of row r at
  * y + r*(2+2N) + 2. A single-output model's row is its out_dim floats. */
 int tfsc_predict_device(tfsc_server* s, int node, const char* model_name, int64_t version,
                         const void* x, int64_t rows, void* y, void* stream);
@@ -394,6 +397,24 @@ int tfsc_k_span_head(const float* logits, const int32_t* ids, const int32_t* mas
 int tfsc_k_encoder_head(const float* hidden, const float* pooled, const int32_t* ids, const int32_t* mask, int stride, int rows, int S,
                         int H, int normalize_cls, int normalize_mean, float* sequence_output, float* pooled_output,
                         float* cls_embedding, float* mean_embedding, void* stream);
+/* Fill-mask gather of masked-language-model bundles, one launch for rows of hidden states hidden[rows, S, H] (fp32, device):
+ * the candidates of row r are the tokens p with ids[q] == mask_token_id and, unless mask is NULL, mask[q] != 0,
+ * q = r * stride + p (int32, device). The first `slots` = M of them in ascending p fill slots 0, 1, ...: positions[r * M + s]
+ * = p and gathered[r, s, :] = hidden[r, p, :] (a bit-exact copy); empty slots hold -1 and zeros. Candidates past the
+ * first M are not served. Every output pointer may be NULL (not written). TFSC_E_INVALID unless 1 <= M <= S <= 8192,
+ * 1 <= H <= 8192, ids is given with stride >= S, and hidden is given for gathered. */
+int tfsc_k_mask_gather(const float* hidden, const int32_t* ids, const int32_t* mask, int stride, int rows, int S, int H, int slots,
+                       int mask_token_id, int32_t* positions, float* gathered, void* stream);
+/* Fill-mask head, one launch for rows of M = `slots` slots: slot s of row r reads the first `vocab` logits of the row
+ * logits + (r * M + s) * ld (fp32, device; ld >= vocab, the columns from vocab on are ignored) and the position
+ * positions[r * M + s] (int32, device). A filled slot (position >= 0) writes its top k ids (descending logit, ties to the
+ * lower id) to top_ids[r, s, :] (int32), their softmax probabilities over the vocab logits to top_probs[r, s, :] (the
+ * same bits as tfsc_k_classify_head on those logits) and their logits to top_logits[r, s, :]; an empty slot writes -1, 0
+ * and -FLT_MAX. Outputs are [rows, M, k]. Every output pointer may be NULL (not written). TFSC_E_INVALID unless
+ * 1 <= M <= 8192, 1 <= vocab <= 32768 and 1 <= k <= min(vocab, 32), and positions, and logits for a top-k output, are
+ * given. */
+int tfsc_k_fill_mask_head(const float* logits, int64_t ld, const int32_t* positions, int rows, int slots, int vocab, int k,
+                          int32_t* top_ids, float* top_probs, float* top_logits, void* stream);
 
 #ifdef __cplusplus
 }

@@ -142,6 +142,8 @@ _sig("tfsc_k_layernorm", C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_floa
 _sig("tfsc_k_classify_head", C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp)
 _sig("tfsc_k_span_head", C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp)
 _sig("tfsc_k_encoder_head", C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp)
+_sig("tfsc_k_mask_gather", C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp)
+_sig("tfsc_k_fill_mask_head", C.c_int, vp, C.c_int64, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp)
 
 
 class TfscError(RuntimeError):

@@ -16,46 +16,12 @@
 #include <cmath>
 #include <cstdlib>
 
+#include "head_select.cuh"
 #include "kernels.h"
 
 namespace tfsc {
 
 extern std::atomic<int64_t> g_launches_nn;
-
-constexpr int kHeadThreadsMax = 512;
-
-__device__ __forceinline__ bool ranks_above(float av, int ai, float bv, int bi) { return av > bv || (av == bv && ai < bi); }
-
-__device__ __forceinline__ void warp_best(float& v, int& i) {
-#pragma unroll
-  for (int o = 16; o; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, v, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, i, o);
-    if (ranks_above(ov, oi, v, i)) {
-      v = ov;
-      i = oi;
-    }
-  }
-}
-
-// this thread's best element that ranks below (lv, li); (-inf, INT_MAX) when it has none left
-__device__ __forceinline__ void local_best(const float* xs, int n, float lv, int li, float* bv, int* bi) {
-  float v0 = -INFINITY;
-  int i0 = INT_MAX;
-#pragma unroll 4
-  for (int j = threadIdx.x; j < n; j += blockDim.x) {
-    const float v = xs[j];
-    if (ranks_above(lv, li, v, j) && ranks_above(v, j, v0, i0)) {
-      v0 = v;
-      i0 = j;
-    }
-  }
-  *bv = v0;
-  *bi = i0;
-}
-
-// one expression for both probability outputs, so top_k_probabilities are the same bits as probabilities[index]
-__device__ __forceinline__ float softmax_at(float x, float m, float inv) { return expf(x - m) * inv; }
 
 __global__ void __launch_bounds__(kHeadThreadsMax) classify_head_kernel(const float* __restrict__ logits, int n, int rounds,
                                                                         HeadOutputs o) {
@@ -67,74 +33,13 @@ __global__ void __launch_bounds__(kHeadThreadsMax) classify_head_kernel(const fl
   __shared__ int s_i;
   __shared__ double s_sum;
   __shared__ int sel[kHeadMaxK];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   const int64_t row = blockIdx.x;
   // launched after a PDL dense kernel, the logits are that grid's output (a no-op without the launch attribute)
   asm volatile("griddepcontrol.wait;" ::: "memory");
-  const float* x = logits + row * n;
-  // eight independent loads in flight per thread: a 30522-wide row is 60 loads per thread, which one at a time would
-  // cost 60 round trips to HBM
-  const int T = blockDim.x;
-  int j0 = threadIdx.x;
-  for (; j0 + 7 * T < n; j0 += 8 * T) {
-    float v[8];
-#pragma unroll
-    for (int u = 0; u < 8; ++u) v[u] = __ldg(x + j0 + u * T);
-#pragma unroll
-    for (int u = 0; u < 8; ++u) xs[j0 + u * T] = v[u];
-  }
-  for (; j0 < n; j0 += T) xs[j0] = __ldg(x + j0);
-  __syncthreads();
-
-  float bv;
-  int bi;
-  local_best(xs, n, INFINITY, -1, &bv, &bi);
-  float m = 0.f;
-  for (int r = 0; r < rounds; ++r) {
-    float v = bv;
-    int i = bi;
-    warp_best(v, i);
-    if (lane == 0) {
-      wv[warp] = v;
-      wi[warp] = i;
-    }
-    __syncthreads();
-    if (warp == 0) {
-      v = lane < nwarps ? wv[lane] : -INFINITY;
-      i = lane < nwarps ? wi[lane] : INT_MAX;
-      warp_best(v, i);
-      if (lane == 0) {
-        s_v = v;
-        s_i = i;
-        sel[r] = i;
-      }
-    }
-    __syncthreads();
-    const float gv = s_v;
-    const int gi = s_i;
-    if (r == 0) m = gv;  // the row maximum
-    if (bi == gi) local_best(xs, n, gv, gi, &bv, &bi);
-  }
-
-  // softmax: max-subtracted fp32 exponentials, summed in fp64 (a 32768-wide row keeps its sum to ~1 ulp of fp32)
+  const float m = head_stage_select(logits + row * n, n, rounds, xs, wv, wi, &s_v, &s_i, sel);
+  // softmax: max-subtracted fp32 exponentials, summed in fp64
   const bool need_sum = o.probs || o.topk_prob;
-  float inv = 0.f;
-  if (need_sum) {
-    double acc = 0.0;
-    for (int j = threadIdx.x; j < n; j += blockDim.x) acc += (double)expf(xs[j] - m);
-#pragma unroll
-    for (int off = 16; off; off >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, off);
-    if (lane == 0) wsum[warp] = acc;
-    __syncthreads();
-    if (warp == 0) {
-      double a = lane < nwarps ? wsum[lane] : 0.0;
-#pragma unroll
-      for (int off = 16; off; off >>= 1) a += __shfl_xor_sync(0xffffffffu, a, off);
-      if (lane == 0) s_sum = a;
-    }
-    __syncthreads();
-    inv = (float)(1.0 / s_sum);
-  }
+  const float inv = need_sum ? head_softmax_inv(xs, n, m, wsum, &s_sum) : 0.f;
   if (o.logits) {
     float* y = o.logits + row * o.logits_ld;
     for (int j = threadIdx.x; j < n; j += blockDim.x) y[j] = xs[j];
@@ -171,11 +76,9 @@ cudaError_t launch_classify_head(const float* logits, int rows, int n, int k, co
     const char* e = getenv("TFSC_PDL");
     return !e || atoi(e) != 0;
   }();
-  // 128 threads cover a ResNet / BERT-classifier head in a few strided loads each; wide vocab heads take 512 so that
-  // every thread has at most 64 elements to load and rescan
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)rows);
-  cfg.blockDim = dim3(n > 2048 ? kHeadThreadsMax : 128);
+  cfg.blockDim = dim3(head_threads(n));
   cfg.dynamicSmemBytes = (size_t)n * sizeof(float);
   cfg.stream = s;
   cudaLaunchAttribute at[1];

@@ -130,6 +130,31 @@ struct EncoderOutputs {
 cudaError_t launch_encoder_head(const float* hidden, const float* pooled, const EncoderInputs& in, int rows, int S, int H,
                                 const EncoderOutputs& o, cudaStream_t s);
 
+// Fill-mask gather (mlm.cu): for each row r, the candidates are the tokens p < S with ids[q] == mask_token_id and, unless
+// mask is nullptr, mask[q] != 0, q = r * stride + p. The first M of them in ascending p fill slots 0, 1, ...: positions[r * M
+// + s] = p and gathered[r, s, :] = hidden[r, p, :] (a bit-exact copy); empty slots get -1 and zeros. Either output may be
+// nullptr. cudaErrorInvalidValue outside mask_gather_supported (nn_limits.h).
+cudaError_t launch_mask_gather(const float* hidden, const int* ids, const int* mask, int64_t stride, int rows, int S, int H,
+                               int M, int mask_token_id, int* positions, float* gathered, cudaStream_t s);
+
+// Fill-mask head (mlm.cu): slot s of row r reads the first `vocab` of the logits row logits + (r * M + s) * ld and, when
+// positions[r * M + s] >= 0, writes at ptr + r * ld_out + s * k (ld_out in 32-bit words) the top k ids (descending logit,
+// ties to the lower id), their softmax probabilities over the vocab logits (the same bits as launch_classify_head on that
+// row) and their logits; an empty slot writes -1, 0 and -FLT_MAX. `positions_out` receives a copy of the positions [M] per
+// row. k counts only when a top-k pointer is set. cudaErrorInvalidValue outside fill_mask_supported (nn_limits.h).
+struct FillMaskOutputs {
+  int* positions = nullptr;
+  int64_t positions_ld = 0;
+  int* ids = nullptr;
+  int64_t ids_ld = 0;
+  float* probs = nullptr;
+  int64_t probs_ld = 0;
+  float* logits = nullptr;
+  int64_t logits_ld = 0;
+};
+cudaError_t launch_fill_mask_head(const float* logits, int64_t ld, const int* positions, int rows, int M, int vocab, int k,
+                                  const FillMaskOutputs& o, cudaStream_t s);
+
 // wgmma 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
 bool gemm_tc_supported(const float* A, const float* B, const float* bias, const float* R, const float* C, int M, int N, int K,
                        int lda);

@@ -16,7 +16,9 @@ size_t ModelDesc::scratch_bytes(int64_t rows) const {
   if (tmpl == Template::Graph) {
     size_t last = 1;
     for (auto v : output_shape) last *= (size_t)v;
-    return head_scratch_offset(rows) + (outputs.empty() ? 0 : align256((size_t)rows * last * 4));
+    // a fill-mask bundle's int32 [rows, M] positions follow the head's logits
+    return head_scratch_offset(rows) + (outputs.empty() ? 0 : align256((size_t)rows * last * 4)) +
+           (mlm_head() ? align256((size_t)rows * (size_t)head_n * 4) : 0);
   }
   return 256;
 }
@@ -25,6 +27,12 @@ size_t ModelDesc::graph_buf_bytes(int64_t rows) const { return align256((size_t)
 
 size_t ModelDesc::head_scratch_offset(int64_t rows) const {
   return (size_t)n_buffers * graph_buf_bytes(rows) + align256((size_t)rows * (size_t)col_elems * 4);
+}
+
+size_t ModelDesc::mlm_positions_offset(int64_t rows) const {
+  size_t last = 1;
+  for (auto v : output_shape) last *= (size_t)v;
+  return head_scratch_offset(rows) + align256((size_t)rows * last * 4);
 }
 
 const char* output_kind_name(OutputKind k) {
@@ -42,7 +50,11 @@ const char* output_kind_name(OutputKind k) {
     case OutputKind::SequenceOutput: return "sequence_output";
     case OutputKind::PooledOutput: return "pooled_output";
     case OutputKind::ClsEmbedding: return "cls_embedding";
-    default: return "mean_embedding";
+    case OutputKind::MeanEmbedding: return "mean_embedding";
+    case OutputKind::MaskedPositions: return "masked_positions";
+    case OutputKind::MaskedTopKIds: return "masked_top_k_ids";
+    case OutputKind::MaskedTopKProbabilities: return "masked_top_k_probabilities";
+    default: return "masked_top_k_logits";
   }
 }
 
@@ -51,6 +63,7 @@ int output_dtype(OutputKind k) { return output_form(k, 0, 0).dtype; }
 bool is_span_kind(OutputKind k) { return k >= OutputKind::StartLogits && k <= OutputKind::SpanScores; }
 bool is_span_result_kind(OutputKind k) { return k >= OutputKind::SpanStarts && k <= OutputKind::SpanScores; }
 bool is_encoder_kind(OutputKind k) { return k >= OutputKind::SequenceOutput && k <= OutputKind::MeanEmbedding; }
+bool is_mlm_kind(OutputKind k) { return k >= OutputKind::MaskedPositions && k <= OutputKind::MaskedTopKLogits; }
 
 OutputForm output_form(OutputKind k, int head_n, int head_k) {
   OutputForm f;
@@ -64,6 +77,13 @@ OutputForm output_form(OutputKind k, int head_n, int head_k) {
     case OutputKind::SequenceOutput:  // encoder bundles: head_k = S, head_n = H
       f.width = (int64_t)head_k * head_n, f.rank = 2, f.dims[0] = head_k, f.dims[1] = head_n;
       return f;
+    case OutputKind::MaskedPositions: f.width = head_n, f.dtype = TFSC_DT_INT32; break;  // fill-mask: head_n = M, head_k = k
+    case OutputKind::MaskedTopKIds:
+    case OutputKind::MaskedTopKProbabilities:
+    case OutputKind::MaskedTopKLogits:
+      f.width = (int64_t)head_n * head_k, f.rank = 2, f.dims[0] = head_n, f.dims[1] = head_k;
+      if (k == OutputKind::MaskedTopKIds) f.dtype = TFSC_DT_INT32;
+      return f;
     default: f.width = head_n; break;  // logits, probabilities, start_logits, end_logits, the [H] embedding kinds
   }
   f.dims[0] = f.rank ? f.width : 1;
@@ -71,7 +91,17 @@ OutputForm output_form(OutputKind k, int head_n, int head_k) {
 }
 
 bool layout_outputs(ModelDesc* d, std::string* err) {
-  if (d->encoder_head()) {
+  if (d->mlm_head()) {
+    // vocab is the owner's business, so only M and k decide whether a row can be laid out
+    const bool topk = d->output(OutputKind::MaskedTopKIds) || d->output(OutputKind::MaskedTopKProbabilities) ||
+                      d->output(OutputKind::MaskedTopKLogits);
+    if (!fill_mask_supported(d->head_n, kHeadMaxN, topk ? d->head_k : 1) || (!topk && d->head_k != 0)) {
+      *err = "signature.outputs: no fill-mask head for M = " + std::to_string(d->head_n) + " slots and k = " +
+             std::to_string(d->head_k) + " (1 <= M <= " + std::to_string(kMaskGatherMaxS) + ", 1 <= k <= " +
+             std::to_string(kHeadMaxK) + ")";
+      return false;
+    }
+  } else if (d->encoder_head()) {
     if (!encoder_head_supported(d->head_k, d->head_n)) {
       *err = "signature.outputs: no encoder head kernel for S = " + std::to_string(d->head_k) + " and H = " +
              std::to_string(d->head_n) + " (1 <= S <= " + std::to_string(kEncoderMaxS) + ", 1 <= H <= " +
@@ -259,10 +289,14 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         else if (kind == "pooled_output") mo.kind = OutputKind::PooledOutput;
         else if (kind == "cls_embedding") mo.kind = OutputKind::ClsEmbedding;
         else if (kind == "mean_embedding") mo.kind = OutputKind::MeanEmbedding;
+        else if (kind == "masked_positions") mo.kind = OutputKind::MaskedPositions;
+        else if (kind == "masked_top_k_ids") mo.kind = OutputKind::MaskedTopKIds;
+        else if (kind == "masked_top_k_probabilities") mo.kind = OutputKind::MaskedTopKProbabilities;
+        else if (kind == "masked_top_k_logits") mo.kind = OutputKind::MaskedTopKLogits;
         else {
           *err = "signature.outputs: unknown kind '" + kind + "' (logits, probabilities, classes, top_k_classes, top_k_probabilities, "
                  "start_logits, end_logits, span_starts, span_ends, span_scores, sequence_output, pooled_output, cls_embedding, "
-                 "mean_embedding)";
+                 "mean_embedding, masked_positions, masked_top_k_ids, masked_top_k_probabilities, masked_top_k_logits)";
           return false;
         }
         if (mo.name.empty()) {
@@ -274,6 +308,35 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
             *err = "signature.outputs: duplicate " + std::string(o.name == mo.name ? "name '" + mo.name + "'" : "kind '" + kind + "'");
             return false;
           }
+        if (!d->outputs.empty() && is_mlm_kind(d->outputs.front().kind) != is_mlm_kind(mo.kind)) {
+          *err = "signature.outputs: fill-mask outputs (masked_positions, masked_top_k_ids, masked_top_k_probabilities,"
+                 " masked_top_k_logits) cannot be mixed with classification, span or encoder outputs ('" + mo.name + "' is " +
+                 kind + ")";
+          return false;
+        }
+        if (is_mlm_kind(mo.kind)) {
+          if (oj.get("normalize") || oj.get("max_answer_length") || oj.get("sep_id")) {
+            *err = "signature.outputs: 'normalize', 'max_answer_length' and 'sep_id' do not apply to fill-mask outputs ('" +
+                   mo.name + "' is " + kind + ")";
+            return false;
+          }
+          if (mo.kind == OutputKind::MaskedPositions) {
+            if (oj.get("k")) {
+              *err = "signature.outputs: 'k' belongs to masked_top_k_ids, masked_top_k_probabilities and masked_top_k_logits ('" +
+                     mo.name + "' is masked_positions)";
+              return false;
+            }
+          } else {
+            int v = 0;
+            if (int_field(oj, "k", &v) != 1 || v < 1 || (k >= 0 && v != k)) {
+              *err = "signature.outputs: '" + mo.name + "' needs an integer 'k' >= 1, the same for every fill-mask top-k output";
+              return false;
+            }
+            k = v;
+          }
+          d->outputs.push_back(mo);
+          continue;
+        }
         if (!d->outputs.empty() && is_encoder_kind(d->outputs.front().kind) != is_encoder_kind(mo.kind)) {
           *err = "signature.outputs: encoder outputs (sequence_output, pooled_output, cls_embedding, mean_embedding) cannot be mixed"
                  " with classification or span outputs ('" + mo.name + "' is " + kind + ")";
@@ -438,6 +501,7 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       else if (kind == "embed") o.kind = OpKind::Embed;
       else if (kind == "layernorm") o.kind = OpKind::LayerNorm;
       else if (kind == "attention") o.kind = OpKind::Attention;
+      else if (kind == "mask_gather") o.kind = OpKind::MaskGather;
       else {
         *err = "graph manifest: unknown op '" + kind + "'";
         return false;
@@ -464,6 +528,10 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       o.eps = (float)oj.get_num("eps", 1e-12);
       o.w_off = (size_t)oj.get_int("w_offset", 0);
       o.b_off = (size_t)oj.get_int("b_offset", 0);
+      if (o.kind == OpKind::MaskGather) {
+        o.oh = (int)oj.get_int("slots", 0);
+        o.mask_token_id = (int)oj.get_int("mask_token_id", 0);
+      }
       if (o.h < 1 || o.w < 1 || o.c < 1 || o.kh < 1 || o.kw < 1 || o.stride < 1 || o.pad < 0 || o.cout < 1) {
         *err = "graph manifest: bad op geometry";
         return false;
@@ -490,6 +558,15 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
           *err = "graph manifest: no attention kernel for S = " + std::to_string(o.h) + ", hidden " + std::to_string(o.cout) + ", " +
                  std::to_string(o.heads) + " heads (head width d % 4 == 0 and d <= 128 runs at every S; other widths only while"
                  " K and V of a head fit in shared memory)";
+          return false;
+        }
+      } else if (o.kind == OpKind::MaskGather) {
+        // [S, 1, H] -> [M, 1, H]; the shapes are checked with the fill-mask outputs below
+        o.ow = 1;
+        o.cout = o.c;
+        if (o.oh < 1 || o.oh > o.h) {
+          *err = "graph manifest: mask_gather needs 1 <= slots <= h (slots = " + std::to_string(o.oh) + ", h = " +
+                 std::to_string(o.h) + ")";
           return false;
         }
       } else if (o.kind == OpKind::AvgPool) {
@@ -580,8 +657,65 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
     for (size_t i = 0; i < d->inputs.size(); ++i) d->inputs[i].offset = (int64_t)i * S;
   }
   finish(d);
+  int gathers = 0;
+  for (auto& o : d->ops) gathers += o.kind == OpKind::MaskGather;
+  if (gathers && !d->mlm_head()) {
+    *err = "graph manifest: a mask_gather op needs fill-mask outputs (masked_positions, masked_top_k_ids, "
+           "masked_top_k_probabilities, masked_top_k_logits)";
+    return false;
+  }
   if (!d->outputs.empty()) {
-    if (d->encoder_head()) {
+    if (d->mlm_head()) {
+      // the gather reads the request's ids / mask where the embedding reads them and the encoder's [S, 1, H] hidden states;
+      // the ops after it run on its M slots and the last one writes [M, 1, Vp] vocabulary logits
+      if (d->tmpl != Template::Graph) {
+        *err = "signature.outputs: fill-mask outputs need a graph bundle (a BERT encoder, a mask_gather op and the MLM head)";
+        return false;
+      }
+      if (d->ops.front().kind != OpKind::Embed) {
+        *err = "signature.outputs: fill-mask outputs need a graph bundle whose first op is 'embed'";
+        return false;
+      }
+      if (gathers != 1) {
+        *err = "signature.outputs: fill-mask outputs need exactly one mask_gather op (the bundle has " + std::to_string(gathers) + ")";
+        return false;
+      }
+      const GraphOp& emb = d->ops.front();
+      const int S = emb.h, H = emb.c, V = emb.vocab;
+      const GraphOp* g = nullptr;
+      for (auto& o : d->ops)
+        if (o.kind == OpKind::MaskGather) g = &o;
+      const int M = g->oh;
+      if (g->src < 0 || g->h != S || g->w != 1 || g->c != H) {
+        *err = "signature.outputs: the mask_gather op needs the [" + std::to_string(S) + ", 1, " + std::to_string(H) +
+               "] hidden states of a scratch buffer (it reads [" + std::to_string(g->h) + ", " + std::to_string(g->w) + ", " +
+               std::to_string(g->c) + "] of buffer " + std::to_string(g->src) + ")";
+        return false;
+      }
+      if (g->mask_token_id < 1 || g->mask_token_id >= V) {
+        *err = "signature.outputs: mask_token_id " + std::to_string(g->mask_token_id) + " is not a token id in [1, " +
+               std::to_string(V) + ")";
+        return false;
+      }
+      const GraphOp& last = d->ops.back();
+      if (last.oh != M || last.ow != 1 || last.cout < V) {
+        *err = "signature.outputs: fill-mask outputs need a last op that writes [" + std::to_string(M) + ", 1, Vp] logits, Vp >= " +
+               std::to_string(V) + " (it writes [" + std::to_string(last.oh) + ", " + std::to_string(last.ow) + ", " +
+               std::to_string(last.cout) + "])";
+        return false;
+      }
+      const bool topk = d->output(OutputKind::MaskedTopKIds) || d->output(OutputKind::MaskedTopKProbabilities) ||
+                        d->output(OutputKind::MaskedTopKLogits);
+      if (!mask_gather_supported(S, H, M) || !fill_mask_supported(M, V, topk ? d->head_k : 1)) {
+        *err = "signature.outputs: no fill-mask kernels for S = " + std::to_string(S) + ", H = " + std::to_string(H) + ", M = " +
+               std::to_string(M) + ", vocab = " + std::to_string(V) + " and k = " + std::to_string(d->head_k) + " (1 <= M <= S <= " +
+               std::to_string(kMaskGatherMaxS) + ", H <= " + std::to_string(kMaskGatherMaxH) + ", 1 <= vocab <= " +
+               std::to_string(kHeadMaxN) + ", 1 <= k <= min(vocab, " + std::to_string(kHeadMaxK) + "))";
+        return false;
+      }
+      d->mlm_vocab = V;
+      d->mlm_mask_token_id = g->mask_token_id;
+    } else if (d->encoder_head()) {
       // the encoder head reads the last hidden states [S, 1, H]: what the last op writes, or, when the last op is the pooler
       // (a tanh dense over token 0), its source buffer; and the request's ids / mask where the embedding reads them
       if (d->tmpl != Template::Graph) {
@@ -650,7 +784,7 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       *err = "signature.outputs needs an mlp or graph bundle (an affine bundle has no logits row)";
       return false;
     }
-    if (!d->span_head() && !d->encoder_head() && d->tmpl == Template::Graph && d->output_shape.size() != 1) {
+    if (!d->span_head() && !d->encoder_head() && !d->mlm_head() && d->tmpl == Template::Graph && d->output_shape.size() != 1) {
       *err = "signature.outputs needs a graph whose output is one vector of logits per row (output_shape has rank " +
              std::to_string(d->output_shape.size()) + ")";
       return false;
@@ -667,6 +801,8 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
     // [S, H] (head_k = S) and [H] (head_n = H)
     d->head_n = d->span_head() ? d->ops.front().h : d->out_dim > 0x7fffffff ? 0 : (int)d->out_dim;
     if (d->encoder_head()) d->head_n = d->ops.front().c, d->head_k = d->ops.front().h;
+    // a fill-mask head's rows are [M] positions and [M, k] top-k (head_k as declared, 0: positions only)
+    if (d->mlm_head()) d->head_n = d->ops.back().oh;
     if (!layout_outputs(d, err)) return false;
   }
   return true;

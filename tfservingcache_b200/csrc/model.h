@@ -17,7 +17,10 @@ enum class Template { Affine, Mlp, Graph };
 // One node of a "graph" bundle (conv nets): activations are NHWC fp32, `src`/`dst`/`res` index scratch
 // activation buffers (-1 = the request tensor, -2 = the response tensor). Weights: conv/dense kernel
 // flattened to [kh*kw*c, cout] row-major (= TF HWIO / dense layout) at w_off, bias (folded BN) at b_off.
-enum class OpKind { Conv, MaxPool, AvgPool, Dense, Embed, LayerNorm, Attention };
+// MaskGather (fill-mask bundles): from the [S, 1, H] hidden states in `src`, copies those of the first `slots` = M tokens
+// whose id is mask_token_id (and whose mask is set, with a mask input) to dst [M, 1, H], ascending position, zeros for
+// empty slots, and writes their positions (int32 [M], -1 empty) to the executor's positions scratch for the head.
+enum class OpKind { Conv, MaxPool, AvgPool, Dense, Embed, LayerNorm, Attention, MaskGather };
 struct GraphOp {
   OpKind kind = OpKind::Conv;
   int src = -1, dst = 0, res = -100;  // res = -100: no residual input
@@ -30,6 +33,7 @@ struct GraphOp {
   size_t word_off = 0, pos_off = 0, type_off = 0;  // Embed tables [vocab,c], [max_pos,c], [2,c]
   float eps = 1e-12f;
   int64_t lda = 0;                    // Dense: elements per image of the source (> c selects the first token)
+  int mask_token_id = 0;              // MaskGather (slots = oh)
 };
 
 struct DenseLayer {
@@ -60,14 +64,17 @@ struct ModelInput {
 // are computed from the last op's [S, 1, 2] per-token logits by the span head (span.cu): start_logits / end_logits [S]
 // float, span_starts / span_ends [k] int32, span_scores [k] float. The encoder kinds (embeddings) are computed from the
 // last hidden states [S, 1, H] (and the pooler's [H]) by the encoder head (encoder_head.cu): sequence_output [S, H] float,
-// pooled_output / cls_embedding / mean_embedding [H] float. New kinds go at the end: the forward hop sends the enum's
-// numbers.
+// pooled_output / cls_embedding / mean_embedding [H] float. The fill-mask kinds (masked-language-model prediction) are
+// computed from the [M, 1, Vp] vocabulary logits of the M [MASK] slots a mask_gather op selected, by the fill-mask head
+// (mlm.cu): masked_positions [M] int32, masked_top_k_ids [M, k] int32, masked_top_k_probabilities / masked_top_k_logits
+// [M, k] float. New kinds go at the end: the forward hop sends the enum's numbers.
 enum class OutputKind {
   Logits, Probabilities, Classes, TopKClasses, TopKProbabilities,
   StartLogits, EndLogits, SpanStarts, SpanEnds, SpanScores,
-  SequenceOutput, PooledOutput, ClsEmbedding, MeanEmbedding
+  SequenceOutput, PooledOutput, ClsEmbedding, MeanEmbedding,
+  MaskedPositions, MaskedTopKIds, MaskedTopKProbabilities, MaskedTopKLogits
 };
-constexpr OutputKind kLastOutputKind = OutputKind::MeanEmbedding;
+constexpr OutputKind kLastOutputKind = OutputKind::MaskedTopKLogits;
 struct ModelOutput {
   std::string name;
   OutputKind kind = OutputKind::Logits;
@@ -79,7 +86,7 @@ int output_dtype(OutputKind k);  // TFSC_DT_FLOAT / TFSC_DT_INT64 / TFSC_DT_INT3
 // What one row of an output kind looks like, the one rule behind the packed layout, every response writer and the
 // metadata: `width` 32-bit words holding a scalar (rank 0: classes, one int64 in 2 words), a vector of dims[0] values
 // (rank 1: N or S for the logits kinds, k for the top-k and span kinds, H for the embedding kinds) or a dims[0] x dims[1]
-// matrix (rank 2: sequence_output, S x H).
+// matrix (rank 2: sequence_output, S x H; the fill-mask top-k kinds, M x k).
 struct OutputForm {
   int64_t width = 0;
   int dtype = TFSC_DT_FLOAT;
@@ -90,6 +97,7 @@ OutputForm output_form(OutputKind k, int head_n, int head_k);
 bool is_span_kind(OutputKind k);        // start_logits .. span_scores
 bool is_span_result_kind(OutputKind k); // span_starts / span_ends / span_scores (they carry k and max_answer_length)
 bool is_encoder_kind(OutputKind k);     // sequence_output, pooled_output, cls_embedding, mean_embedding
+bool is_mlm_kind(OutputKind k);         // masked_positions, masked_top_k_ids / _probabilities / _logits
 constexpr int kMaxOutputs = 5;
 
 struct ModelDesc {
@@ -126,9 +134,13 @@ struct ModelDesc {
   std::vector<ModelOutput> outputs;
   int head_n = 0, head_k = 0;
   int span_max_len = 0, span_sep_id = -1;
+  // Fill-mask outputs: head_n = M (the mask_gather op's slots), head_k = k (0: masked_positions only); mlm_vocab (the embed
+  // op's vocab, the logits the head reads of each Vp-wide row) and mlm_mask_token_id are the owner's.
   bool encoder_pooler = false, normalize_cls = false, normalize_mean = false;
+  int mlm_vocab = 0, mlm_mask_token_id = 0;
   bool span_head() const { return !outputs.empty() && is_span_kind(outputs.front().kind); }
   bool encoder_head() const { return !outputs.empty() && is_encoder_kind(outputs.front().kind); }
+  bool mlm_head() const { return !outputs.empty() && is_mlm_kind(outputs.front().kind); }
   const ModelOutput* output(OutputKind k) const {
     for (auto& o : outputs)
       if (o.kind == k) return &o;
@@ -146,6 +158,8 @@ struct ModelDesc {
   size_t graph_buf_bytes(int64_t rows) const;
   // offset of the head's logits in that scratch (graph bundles with outputs: after the buffers and the im2col matrix)
   size_t head_scratch_offset(int64_t rows) const;
+  // fill-mask bundles: offset of the mask_gather op's int32 positions [rows, M] in that scratch, after the head's logits
+  size_t mlm_positions_offset(int64_t rows) const;
 };
 
 // Sort d->outputs by name, set their offsets and widths from d->head_n / d->head_k and d->out_dim to the packed row width.

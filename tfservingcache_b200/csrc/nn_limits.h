@@ -43,4 +43,16 @@ inline bool span_supported(int S, int L, int k) { return S >= 1 && S <= kSpanMax
 constexpr int kEncoderMaxS = 8192, kEncoderMaxH = 8192;
 inline bool encoder_head_supported(int S, int H) { return S >= 1 && S <= kEncoderMaxS && H >= 1 && H <= kEncoderMaxH; }
 
+// Fill-mask (mlm.cu). The gather: one CTA per row scans S tokens for [MASK] and copies the hidden states of up to M of them
+// (1 <= M <= S <= 8192, H <= 8192, M positions in shared memory). The head: one CTA per (row, slot) stages the first `vocab`
+// logits of its slot like the classification head (128 KB at vocab = 32768) and selects the top k of them. A head with
+// masked_positions only runs as k = 1.
+constexpr int kMaskGatherMaxS = 8192, kMaskGatherMaxH = 8192;
+inline bool mask_gather_supported(int S, int H, int M) {
+  return S >= 1 && S <= kMaskGatherMaxS && H >= 1 && H <= kMaskGatherMaxH && M >= 1 && M <= S;
+}
+inline bool fill_mask_supported(int M, int vocab, int k) {
+  return M >= 1 && M <= kMaskGatherMaxS && vocab >= 1 && vocab <= kHeadMaxN && k >= 1 && k <= kHeadMaxK && k <= vocab;
+}
+
 }  // namespace tfsc

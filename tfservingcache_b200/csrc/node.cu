@@ -576,11 +576,15 @@ size_t Node::model_ws_bytes(const ModelDesc& d) {
     size_t w = dense_workspace_bytes(kMaxRowsPerLaunch, L.in, L.out);
     if (w > m) m = w;
   }
-  for (auto& o : d.ops)  // graph bundles: plain dense heads (ResNet fc) run on the weight-streaming dense kernels
-    if (o.kind == OpKind::Dense) {
+  bool after_gather = false;
+  for (auto& o : d.ops) {  // graph bundles: plain dense heads (ResNet fc) run on the weight-streaming dense kernels
+    // and so does a fill-mask bundle's vocabulary projection on a few rows (run_model)
+    if (o.kind == OpKind::Dense || (after_gather && o.kind == OpKind::Conv)) {
       size_t w = dense_workspace_bytes(kMaxRowsPerLaunch, o.c, o.cout);
       if (w > m) m = w;
     }
+    after_gather = after_gather || o.kind == OpKind::MaskGather;
+  }
   return m;
 }
 
@@ -655,6 +659,26 @@ static cudaError_t run_encoder_head(const ModelDesc& d, const float* hidden, con
   return launch_encoder_head(hidden, pooled, in, (int)rows, d.head_k, d.head_n, o, st);
 }
 
+// fill-mask bundles: one head launch reads the last op's [rows, M, Vp] vocabulary logits and the gather's positions
+// [rows, M], and writes every declared output at its offset in the packed row
+static cudaError_t run_fill_mask_head(const ModelDesc& d, const float* logits, const int* positions, int64_t rows, char* y,
+                                      cudaStream_t st) {
+  FillMaskOutputs o;
+  float* yf = reinterpret_cast<float*>(y);
+  const int64_t ld = d.out_dim;
+  for (const ModelOutput& m : d.outputs) {
+    float* p = yf + m.offset;
+    switch (m.kind) {
+      case OutputKind::MaskedPositions: o.positions = reinterpret_cast<int*>(p), o.positions_ld = ld; break;
+      case OutputKind::MaskedTopKIds: o.ids = reinterpret_cast<int*>(p), o.ids_ld = ld; break;
+      case OutputKind::MaskedTopKProbabilities: o.probs = p, o.probs_ld = ld; break;
+      case OutputKind::MaskedTopKLogits: o.logits = p, o.logits_ld = ld; break;
+      default: break;
+    }
+  }
+  return launch_fill_mask_head(logits, d.ops.back().cout, positions, (int)rows, d.head_n, d.mlm_vocab, d.head_k, o, st);
+}
+
 cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, char* y, char* scratch, void* ws,
                             size_t ws_cap, cudaStream_t st) {
   const ModelDesc& d = dm.desc;
@@ -685,6 +709,9 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
       types = ti ? (const int*)x + ti->offset : nullptr;
       stride = (int)d.in_dim;
     }
+    // fill-mask bundles: the mask_gather op writes the [MASK] positions here, and the head reads them
+    int* positions = d.mlm_head() ? reinterpret_cast<int*>(scratch + d.mlm_positions_offset(rows)) : nullptr;
+    bool after_gather = false;
     for (const GraphOp& o : d.ops) {
       const float* src = (const float*)buf(o.src);
       float* dst = (float*)buf(o.dst);
@@ -697,6 +724,15 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
         if (o.kind == OpKind::Dense && !res && o.act <= 1 && (int)o.lda == K && B < 64) {
           // a classifier head on a handful of rows is the tenant-MLP problem (HBM-bound weight streaming), not a GEMM tile
           e = launch_dense(src, W, bias, dst, B, K, o.cout, o.act == 1, ws, ws_cap, st);
+          if (e != cudaSuccess) return e;
+          continue;
+        }
+        if (after_gather && o.kind == OpKind::Conv && o.dst == -2 && !res && o.act <= 1 && o.kh == 1 && o.kw == 1 &&
+            o.stride == 1 && o.pad == 0 && o.cout % 32 == 0 && B * o.oh * o.ow < 64) {
+          // a fill-mask vocabulary projection, padded to Vp % 32 == 0, on fewer than 64 slots (one [MASK] per row at the
+          // default batch of 8): too few rows for the tensor-core GEMM, so it streams the [H, Vp] weights once (DESIGN §4);
+          // an unpadded decoder keeps the GEMM path
+          e = launch_dense(src, W, bias, dst, B * o.oh * o.ow, K, o.cout, o.act == 1, ws, ws_cap, st);
           if (e != cudaSuccess) return e;
           continue;
         }
@@ -729,11 +765,16 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
                              (const float*)(dm.dptr + o.w_off), (const float*)(dm.dptr + o.b_off), dst, B * o.h, o.h, o.c, 0, o.eps, st);
       } else if (o.kind == OpKind::Attention) {
         e = launch_attention(src, mask, stride ? stride : o.h, dst, B, o.h, o.cout, o.heads, st);
+      } else if (o.kind == OpKind::MaskGather) {
+        e = launch_mask_gather(src, ids, d.input(InputRole::Mask) ? mask : nullptr, stride ? stride : o.h, B, o.h, o.c, o.oh,
+                               o.mask_token_id, positions, dst, st);
+        after_gather = true;
       } else {
         e = launch_avgpool(src, dst, B, o.h * o.w, o.c, st);
       }
       if (e != cudaSuccess) return e;
     }
+    if (d.mlm_head()) return run_fill_mask_head(d, (const float*)out, positions, rows, y, st);
     if (d.encoder_head()) {
       // with a pooler the hidden states are the pooler's source buffer and `out` holds its [rows, H] output; without one
       // the last op wrote the hidden states to `out`

@@ -1317,7 +1317,8 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
       ins = tensor_info(d.input_name, dim.empty() ? std::vector<std::string>{} : std::vector<std::string>{dim},
                         d.input_dtype == TFSC_DT_INT32 ? "DT_INT32" : "DT_FLOAT");
     // a multi-output model lists every output: logits / probabilities [-1, N], classes [-1] (int64), top-k [-1, k],
-    // start / end logits [-1, S], spans [-1, k], sequence_output [-1, S, H], the other encoder outputs [-1, H]
+    // start / end logits [-1, S], spans [-1, k], sequence_output [-1, S, H], the other encoder outputs [-1, H],
+    // masked_positions [-1, M], the fill-mask top-k outputs [-1, M, k]
     std::string outs;
     for (auto& mo : d.outputs) {
       const OutputForm f = output_form(mo.kind, d.head_n, d.head_k);
@@ -1920,6 +1921,36 @@ int tfsc_k_encoder_head(const float* hidden, const float* pooled, const int32_t*
   o.normalize_mean = normalize_mean != 0;
   cudaError_t e = launch_encoder_head(hidden, pooled, in, rows, S, H, o, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "encoder_head: %s", cudaGetErrorString(e));
+}
+int tfsc_k_mask_gather(const float* hidden, const int32_t* ids, const int32_t* mask, int stride, int rows, int S, int H, int slots,
+                       int mask_token_id, int32_t* positions, float* gathered, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (rows < 0 || !mask_gather_supported(S, H, slots))
+    return fail(TFSC_E_INVALID, "mask_gather: no kernel for %d rows of S = %d, H = %d, M = %d (1 <= M <= S <= %d, 1 <= H <= %d)",
+                rows, S, H, slots, kMaskGatherMaxS, kMaskGatherMaxH);
+  if (!ids || stride < S) return fail(TFSC_E_INVALID, "mask_gather: needs the ids, stride >= S (%d < %d)", stride, S);
+  if (gathered && !hidden) return fail(TFSC_E_INVALID, "mask_gather: the gathered rows need the hidden states");
+  cudaError_t e = launch_mask_gather(hidden, ids, mask, stride, rows, S, H, slots, mask_token_id, positions, gathered,
+                                     (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "mask_gather: %s", cudaGetErrorString(e));
+}
+int tfsc_k_fill_mask_head(const float* logits, int64_t ld, const int32_t* positions, int rows, int slots, int vocab, int k,
+                          int32_t* top_ids, float* top_probs, float* top_logits, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (rows < 0 || !fill_mask_supported(slots, vocab, k))
+    return fail(TFSC_E_INVALID, "fill_mask_head: no kernel for %d rows of M = %d, vocab = %d, k = %d (1 <= M <= %d, 1 <= vocab <= %d, "
+                "1 <= k <= min(vocab, %d))", rows, slots, vocab, k, kMaskGatherMaxS, kHeadMaxN, kHeadMaxK);
+  if (!positions || ((top_ids || top_probs || top_logits) && (!logits || ld < vocab)))
+    return fail(TFSC_E_INVALID, "fill_mask_head: needs the positions and the logits, ld >= vocab (%lld < %d)", (long long)ld, vocab);
+  FillMaskOutputs o;
+  o.ids = top_ids;
+  o.ids_ld = (int64_t)slots * k;
+  o.probs = top_probs;
+  o.probs_ld = (int64_t)slots * k;
+  o.logits = top_logits;
+  o.logits_ld = (int64_t)slots * k;
+  cudaError_t e = launch_fill_mask_head(logits, ld, positions, rows, slots, vocab, k, o, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "fill_mask_head: %s", cudaGetErrorString(e));
 }
 int tfsc_debug_gemm_trace(long long*) {
   return fail(TFSC_E_UNIMPLEMENTED, "no GEMM clock trace: the persistent GEMM kernel it timed is not part of the sm_90a build");

@@ -21,6 +21,10 @@ SPAN_OUTPUT_KINDS = ("start_logits", "end_logits", "span_starts", "span_ends", "
 # embeddings (a graph bundle ending in the last hidden states [S, 1, H], or in the pooler over them); cls_embedding and
 # mean_embedding may carry "normalize": true
 ENCODER_OUTPUT_KINDS = ("sequence_output", "pooled_output", "cls_embedding", "mean_embedding")
+# fill-mask (a graph bundle with a mask_gather op over the [MASK] tokens, ending in [M, 1, Vp] vocabulary logits); the three
+# top-k kinds carry the same "k"
+MLM_OUTPUT_KINDS = ("masked_positions", "masked_top_k_ids", "masked_top_k_probabilities", "masked_top_k_logits")
+_MLM_TOPK = MLM_OUTPUT_KINDS[1:]
 
 
 def _signature(sig: dict, outputs):
@@ -37,17 +41,21 @@ def packed_output_layout(outputs, n, seq=None):
     """(name, element offset, width, dtype) of every output in a packed response row, in packed order (byte-wise sorted
     names). Offsets and widths count 32-bit words: logits / probabilities n floats, classes 2 words (one little-endian
     int64), top-k k values (int32 classes, float probabilities), start / end logits n floats, span_starts / span_ends k
-    int32, span_scores k floats, sequence_output seq * n floats, pooled_output / cls_embedding / mean_embedding n floats.
+    int32, span_scores k floats, sequence_output seq * n floats, pooled_output / cls_embedding / mean_embedding n floats,
+    masked_positions n int32, masked_top_k_ids n * k int32, masked_top_k_probabilities / masked_top_k_logits n * k floats.
     n = the last op's per-row width for the classification kinds, the sequence length S for the span kinds, the hidden
-    width H for the encoder kinds (seq = S)."""
+    width H for the encoder kinds (seq = S), the mask_gather op's slots M for the fill-mask kinds."""
     out, off = [], 0
     for o in sorted(outputs, key=lambda o: o["name"].encode()):
         kind = o["kind"]
         width = {"logits": n, "probabilities": n, "classes": 2, "start_logits": n, "end_logits": n, "pooled_output": n,
-                 "cls_embedding": n, "mean_embedding": n}.get(kind, o.get("k"))
+                 "cls_embedding": n, "mean_embedding": n, "masked_positions": n}.get(kind, o.get("k"))
         if kind == "sequence_output":
             width = seq * n
-        dtype = {"classes": "int64", "top_k_classes": "int32", "span_starts": "int32", "span_ends": "int32"}.get(kind, "float32")
+        elif kind in _MLM_TOPK:
+            width = n * o["k"]
+        dtype = {"classes": "int64", "top_k_classes": "int32", "span_starts": "int32", "span_ends": "int32",
+                 "masked_positions": "int32", "masked_top_k_ids": "int32"}.get(kind, "float32")
         out.append((o["name"], off, int(width), dtype))
         off += int(width)
     return out
@@ -55,7 +63,8 @@ def packed_output_layout(outputs, n, seq=None):
 
 def split_packed_rows(rows_words: np.ndarray, outputs, n, seq=None) -> dict:
     """{name: array} from packed rows ([rows, out_dim] of any 4-byte dtype, e.g. the float32 view of tfsc_predict_device's y).
-    n and seq as for packed_output_layout; sequence_output comes out as [rows, seq, n]."""
+    n and seq as for packed_output_layout; sequence_output comes out as [rows, seq, n], the fill-mask top-k kinds as
+    [rows, n, k]."""
     w = np.ascontiguousarray(rows_words).view(np.uint32).reshape(len(rows_words), -1)
     kinds = {o["name"]: o["kind"] for o in outputs}
     res = {}
@@ -67,6 +76,8 @@ def split_packed_rows(rows_words: np.ndarray, outputs, n, seq=None) -> dict:
             res[name] = part.view("<i4" if dtype == "int32" else "<f4")
         if kinds[name] == "sequence_output":
             res[name] = res[name].reshape(len(w), seq, n)
+        elif kinds[name] in _MLM_TOPK:
+            res[name] = res[name].reshape(len(w), n, -1)
     return res
 
 
@@ -193,7 +204,7 @@ def packed_input_order(inputs):
 
 
 def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30522, max_pos=512, labels=2, inputs=None,
-                  outputs=None, head="classify", pooler=True):
+                  outputs=None, head="classify", pooler=True, slots=1, mask_token_id=103):
     """BERT-base fine-tune variant (Devlin et al. 2018) as a graph bundle: token ids int32 [B, seq] -> logits
     [B, labels]. A sequence is an "image" with h = seq tokens, w = 1, c = width; dense layers are 1x1 convs.
     With inputs=None the bundle takes the ids only: the attention mask is derived from them ([PAD] = 0), token_type is 0.
@@ -208,6 +219,11 @@ def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30
     the last op is the pooler (a tanh dense over token 0 of buffer 0, writing [B, hidden]) and the hidden states are
     buffer 0; with pooler=False (BertModel(add_pooling_layer=False)) the last LayerNorm writes the [B, seq, 1, hidden]
     hidden states as the response.
+    head="mlm" makes the masked-language-model variant (BertForMaskedLM), answering MLM_OUTPUT_KINDS: after the encoder a
+    mask_gather op copies the hidden states of the first `slots` = M tokens whose id is mask_token_id to buffer 1
+    ([B, M, 1, hidden]), then the prediction head runs on those M slots: the transform (a 1x1 conv hidden -> hidden with
+    GELU), its LayerNorm, and the decoder (a 1x1 conv hidden -> Vp writing [B, M, 1, Vp] logits), Vp = vocab rounded up
+    to a multiple of 32 so that the projection runs on the tensor-core GEMM; its columns from vocab on are zero padding.
     Buffers: 0 hidden, 1 qkv / ffn-intermediate, 2 context / post-attention, 3 dense output."""
     ops = [{"op": "embed", "src": -1, "dst": 0, "h": seq, "w": 1, "c": hidden, "vocab": vocab, "max_pos": max_pos, "eps": 1e-12}]
 
@@ -231,6 +247,17 @@ def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30
             ops.append({"op": "dense", "src": 0, "dst": -2, "h": 1, "w": 1, "c": hidden, "cout": hidden, "act": "tanh"})
         else:
             ops[-1]["dst"] = -2                                                          # the last LayerNorm answers
+    elif head == "mlm":
+        M, vp = slots, (vocab + 31) // 32 * 32
+        ops.append({"op": "mask_gather", "src": 0, "dst": 1, "h": seq, "w": 1, "c": hidden, "slots": M,
+                    "mask_token_id": mask_token_id})
+
+        def slot_dense(src, dst, cout, act="none"):
+            return {"op": "conv", "src": src, "dst": dst, "h": M, "w": 1, "c": hidden, "kh": 1, "kw": 1, "stride": 1, "pad": 0,
+                    "cout": cout, "act": act}
+        ops.append(slot_dense(1, 2, hidden, act="gelu"))                                # cls.predictions.transform.dense
+        ops.append({"op": "layernorm", "src": 2, "dst": 3, "h": M, "w": 1, "c": hidden, "eps": 1e-12})
+        ops.append(slot_dense(3, -2, vp))                                                # decoder (tied to word_embeddings)
     elif head == "span":
         ops.append(dense(0, -2, hidden, 2))                                              # qa_outputs: start | end per token
     else:
