@@ -252,6 +252,7 @@ void FwdSignature::to_desc(ModelDesc* d) const {
   std::string err;
   if (!d->outputs.empty() && !layout_outputs(d, &err)) {  // unusable: no front-end can size a response for 0 words per row
     d->outputs.clear();
+    d->head = HeadKind::None;
     d->out_dim = 0;
   }
 }

@@ -18,7 +18,7 @@ size_t ModelDesc::scratch_bytes(int64_t rows) const {
     for (auto v : output_shape) last *= (size_t)v;
     // a fill-mask bundle's int32 [rows, M] positions follow the head's logits
     return head_scratch_offset(rows) + (outputs.empty() ? 0 : align256((size_t)rows * last * 4)) +
-           (mlm_head() ? align256((size_t)rows * (size_t)head_n * 4) : 0);
+           (head == HeadKind::FillMask ? align256((size_t)rows * (size_t)head_n * 4) : 0);
   }
   return 256;
 }
@@ -35,92 +35,110 @@ size_t ModelDesc::mlm_positions_offset(int64_t rows) const {
   return head_scratch_offset(rows) + align256((size_t)rows * last * 4);
 }
 
-const char* output_kind_name(OutputKind k) {
-  switch (k) {
-    case OutputKind::Logits: return "logits";
-    case OutputKind::Probabilities: return "probabilities";
-    case OutputKind::Classes: return "classes";
-    case OutputKind::TopKClasses: return "top_k_classes";
-    case OutputKind::TopKProbabilities: return "top_k_probabilities";
-    case OutputKind::StartLogits: return "start_logits";
-    case OutputKind::EndLogits: return "end_logits";
-    case OutputKind::SpanStarts: return "span_starts";
-    case OutputKind::SpanEnds: return "span_ends";
-    case OutputKind::SpanScores: return "span_scores";
-    case OutputKind::SequenceOutput: return "sequence_output";
-    case OutputKind::PooledOutput: return "pooled_output";
-    case OutputKind::ClsEmbedding: return "cls_embedding";
-    case OutputKind::MeanEmbedding: return "mean_embedding";
-    case OutputKind::MaskedPositions: return "masked_positions";
-    case OutputKind::MaskedTopKIds: return "masked_top_k_ids";
-    case OutputKind::MaskedTopKProbabilities: return "masked_top_k_probabilities";
-    default: return "masked_top_k_logits";
-  }
-}
+// ------------------------------------------------------------------------------------------------ output kinds ----
+// A row of an output kind in the bundle's head_n / head_k (ModelDesc): one int64 scalar (2 words), a vector of head_n or
+// head_k values, or a head_k x head_n / head_n x head_k matrix
+enum class Rows { Int64, N, K, KxN, NxK };
+// The entry fields a kind takes besides name and kind: "k"; "k", "max_answer_length" and "sep_id"; or "normalize"
+enum class Fields { None, K, Span, Normalize };
+struct OutputKindInfo {
+  const char* name;
+  HeadKind head;
+  int dtype;
+  Rows rows;
+  Fields fields;
+};
+// One row per OutputKind, in enum order. head_n / head_k per head: see ModelDesc::outputs.
+static constexpr OutputKindInfo kOutputKinds[] = {
+    {"logits", HeadKind::Classify, TFSC_DT_FLOAT, Rows::N, Fields::None},
+    {"probabilities", HeadKind::Classify, TFSC_DT_FLOAT, Rows::N, Fields::None},
+    {"classes", HeadKind::Classify, TFSC_DT_INT64, Rows::Int64, Fields::None},
+    {"top_k_classes", HeadKind::Classify, TFSC_DT_INT32, Rows::K, Fields::K},
+    {"top_k_probabilities", HeadKind::Classify, TFSC_DT_FLOAT, Rows::K, Fields::K},
+    {"start_logits", HeadKind::Span, TFSC_DT_FLOAT, Rows::N, Fields::None},
+    {"end_logits", HeadKind::Span, TFSC_DT_FLOAT, Rows::N, Fields::None},
+    {"span_starts", HeadKind::Span, TFSC_DT_INT32, Rows::K, Fields::Span},
+    {"span_ends", HeadKind::Span, TFSC_DT_INT32, Rows::K, Fields::Span},
+    {"span_scores", HeadKind::Span, TFSC_DT_FLOAT, Rows::K, Fields::Span},
+    {"sequence_output", HeadKind::Encoder, TFSC_DT_FLOAT, Rows::KxN, Fields::None},
+    {"pooled_output", HeadKind::Encoder, TFSC_DT_FLOAT, Rows::N, Fields::None},
+    {"cls_embedding", HeadKind::Encoder, TFSC_DT_FLOAT, Rows::N, Fields::Normalize},
+    {"mean_embedding", HeadKind::Encoder, TFSC_DT_FLOAT, Rows::N, Fields::Normalize},
+    {"masked_positions", HeadKind::FillMask, TFSC_DT_INT32, Rows::N, Fields::None},
+    {"masked_top_k_ids", HeadKind::FillMask, TFSC_DT_INT32, Rows::NxK, Fields::K},
+    {"masked_top_k_probabilities", HeadKind::FillMask, TFSC_DT_FLOAT, Rows::NxK, Fields::K},
+    {"masked_top_k_logits", HeadKind::FillMask, TFSC_DT_FLOAT, Rows::NxK, Fields::K},
+};
+static_assert(sizeof(kOutputKinds) / sizeof(kOutputKinds[0]) == (size_t)kLastOutputKind + 1, "one row per OutputKind");
 
-int output_dtype(OutputKind k) { return output_form(k, 0, 0).dtype; }
+static const OutputKindInfo& kind_info(OutputKind k) { return kOutputKinds[(int)k]; }
+static bool takes_k(OutputKind k) { return kind_info(k).fields == Fields::K || kind_info(k).fields == Fields::Span; }
 
-bool is_span_kind(OutputKind k) { return k >= OutputKind::StartLogits && k <= OutputKind::SpanScores; }
-bool is_span_result_kind(OutputKind k) { return k >= OutputKind::SpanStarts && k <= OutputKind::SpanScores; }
-bool is_encoder_kind(OutputKind k) { return k >= OutputKind::SequenceOutput && k <= OutputKind::MeanEmbedding; }
-bool is_mlm_kind(OutputKind k) { return k >= OutputKind::MaskedPositions && k <= OutputKind::MaskedTopKLogits; }
+const char* output_kind_name(OutputKind k) { return kind_info(k).name; }
+int output_dtype(OutputKind k) { return kind_info(k).dtype; }
 
 OutputForm output_form(OutputKind k, int head_n, int head_k) {
   OutputForm f;
-  switch (k) {
-    case OutputKind::Classes: f.width = 2, f.dtype = TFSC_DT_INT64, f.rank = 0; break;
-    case OutputKind::TopKClasses:
-    case OutputKind::SpanStarts:
-    case OutputKind::SpanEnds: f.width = head_k, f.dtype = TFSC_DT_INT32; break;
-    case OutputKind::TopKProbabilities:
-    case OutputKind::SpanScores: f.width = head_k; break;
-    case OutputKind::SequenceOutput:  // encoder bundles: head_k = S, head_n = H
-      f.width = (int64_t)head_k * head_n, f.rank = 2, f.dims[0] = head_k, f.dims[1] = head_n;
-      return f;
-    case OutputKind::MaskedPositions: f.width = head_n, f.dtype = TFSC_DT_INT32; break;  // fill-mask: head_n = M, head_k = k
-    case OutputKind::MaskedTopKIds:
-    case OutputKind::MaskedTopKProbabilities:
-    case OutputKind::MaskedTopKLogits:
-      f.width = (int64_t)head_n * head_k, f.rank = 2, f.dims[0] = head_n, f.dims[1] = head_k;
-      if (k == OutputKind::MaskedTopKIds) f.dtype = TFSC_DT_INT32;
-      return f;
-    default: f.width = head_n; break;  // logits, probabilities, start_logits, end_logits, the [H] embedding kinds
+  f.dtype = kind_info(k).dtype;
+  switch (kind_info(k).rows) {
+    case Rows::Int64: f.width = 2, f.rank = 0, f.dims[0] = 1; break;
+    case Rows::N: f.width = f.dims[0] = head_n; break;
+    case Rows::K: f.width = f.dims[0] = head_k; break;
+    case Rows::KxN: f.rank = 2, f.dims[0] = head_k, f.dims[1] = head_n, f.width = (int64_t)head_k * head_n; break;
+    case Rows::NxK: f.rank = 2, f.dims[0] = head_n, f.dims[1] = head_k, f.width = (int64_t)head_n * head_k; break;
   }
-  f.dims[0] = f.rank ? f.width : 1;
   return f;
 }
 
+// the head of a bundle's outputs is the first one's (the loader refuses a mix)
+static void set_head(ModelDesc* d) { d->head = d->outputs.empty() ? HeadKind::None : kind_info(d->outputs.front().kind).head; }
+
+// a top-k or span result output: without one, a bundle's head_k must be 0
+static bool declares_k(const ModelDesc& d) {
+  for (auto& o : d.outputs)
+    if (takes_k(o.kind)) return true;
+  return false;
+}
+
+// Each head's limits on a row, checked by the loader on the bundle and by layout_outputs on what the forward hop carries
+static bool classify_fits(int n, int k, bool with_k) { return head_supported(n, with_k ? k : 1) && (with_k || k == 0); }
+static bool span_fits(int S, int L, int k, bool with_k) { return span_supported(S, with_k ? L : 1, with_k ? k : 1) && (with_k || k == 0); }
+static bool fill_mask_fits(int M, int V, int k, bool with_k) { return fill_mask_supported(M, V, with_k ? k : 1) && (with_k || k == 0); }
+static bool encoder_fits(int S, int H, std::string* err) {
+  if (encoder_head_supported(S, H)) return true;
+  *err = "signature.outputs: no encoder head kernel for S = " + std::to_string(S) + " and H = " + std::to_string(H) +
+         " (1 <= S <= " + std::to_string(kEncoderMaxS) + ", 1 <= H <= " + std::to_string(kEncoderMaxH) + ")";
+  return false;
+}
+
 bool layout_outputs(ModelDesc* d, std::string* err) {
-  if (d->mlm_head()) {
-    // vocab is the owner's business, so only M and k decide whether a row can be laid out
-    const bool topk = d->output(OutputKind::MaskedTopKIds) || d->output(OutputKind::MaskedTopKProbabilities) ||
-                      d->output(OutputKind::MaskedTopKLogits);
-    if (!fill_mask_supported(d->head_n, kHeadMaxN, topk ? d->head_k : 1) || (!topk && d->head_k != 0)) {
-      *err = "signature.outputs: no fill-mask head for M = " + std::to_string(d->head_n) + " slots and k = " +
-             std::to_string(d->head_k) + " (1 <= M <= " + std::to_string(kMaskGatherMaxS) + ", 1 <= k <= " +
-             std::to_string(kHeadMaxK) + ")";
-      return false;
-    }
-  } else if (d->encoder_head()) {
-    if (!encoder_head_supported(d->head_k, d->head_n)) {
-      *err = "signature.outputs: no encoder head kernel for S = " + std::to_string(d->head_k) + " and H = " +
-             std::to_string(d->head_n) + " (1 <= S <= " + std::to_string(kEncoderMaxS) + ", 1 <= H <= " +
-             std::to_string(kEncoderMaxH) + ")";
-      return false;
-    }
-  } else if (d->span_head()) {
-    // max_answer_length is the owner's business, so only S and k decide whether a row can be laid out
-    const bool spans = d->output(OutputKind::SpanStarts) || d->output(OutputKind::SpanEnds) || d->output(OutputKind::SpanScores);
-    if (!span_supported(d->head_n, 1, spans ? d->head_k : 1) || (!spans && d->head_k != 0)) {
-      *err = "signature.outputs: no span kernel for S = " + std::to_string(d->head_n) + " and k = " + std::to_string(d->head_k) +
-             " (1 <= S <= " + std::to_string(kSpanMaxS) + ", 1 <= k <= " + std::to_string(kSpanMaxK) + ")";
-      return false;
-    }
-  } else if (const bool topk = d->output(OutputKind::TopKClasses) || d->output(OutputKind::TopKProbabilities);
-             !head_supported(d->head_n, topk ? d->head_k : 1) || (!topk && d->head_k != 0)) {
-    *err = "signature.outputs: no head kernel for " + std::to_string(d->head_n) + " logits and k = " + std::to_string(d->head_k) +
-           " (1 <= N <= " + std::to_string(kHeadMaxN) + ", 1 <= k <= min(N, " + std::to_string(kHeadMaxK) + "))";
-    return false;
+  set_head(d);
+  const bool with_k = declares_k(*d);
+  switch (d->head) {
+    case HeadKind::FillMask:  // vocab is the owner's business, so only M and k decide whether a row can be laid out
+      if (!fill_mask_fits(d->head_n, kHeadMaxN, d->head_k, with_k)) {
+        *err = "signature.outputs: no fill-mask head for M = " + std::to_string(d->head_n) + " slots and k = " +
+               std::to_string(d->head_k) + " (1 <= M <= " + std::to_string(kMaskGatherMaxS) + ", 1 <= k <= " +
+               std::to_string(kHeadMaxK) + ")";
+        return false;
+      }
+      break;
+    case HeadKind::Encoder:
+      if (!encoder_fits(d->head_k, d->head_n, err)) return false;
+      break;
+    case HeadKind::Span:  // max_answer_length is the owner's business, so only S and k decide whether a row can be laid out
+      if (!span_fits(d->head_n, 1, d->head_k, with_k)) {
+        *err = "signature.outputs: no span kernel for S = " + std::to_string(d->head_n) + " and k = " + std::to_string(d->head_k) +
+               " (1 <= S <= " + std::to_string(kSpanMaxS) + ", 1 <= k <= " + std::to_string(kSpanMaxK) + ")";
+        return false;
+      }
+      break;
+    default:
+      if (!classify_fits(d->head_n, d->head_k, with_k)) {
+        *err = "signature.outputs: no head kernel for " + std::to_string(d->head_n) + " logits and k = " + std::to_string(d->head_k) +
+               " (1 <= N <= " + std::to_string(kHeadMaxN) + ", 1 <= k <= min(N, " + std::to_string(kHeadMaxK) + "))";
+        return false;
+      }
   }
   // the packed row holds the outputs in byte-wise name order, so a rank can split a response without the manifest
   std::sort(d->outputs.begin(), d->outputs.end(), [](const ModelOutput& a, const ModelOutput& b) { return a.name < b.name; });
@@ -197,6 +215,271 @@ ModelDesc make_affine_desc() {
   return d;
 }
 
+// signature.outputs, one entry at a time. An entry is refused for, in this order: an unknown kind, no name, a duplicate, a
+// mix of heads (fill-mask, then encoder, then span: the message names the later entry's head), a 'normalize' on a kind
+// without one, and then the fields its head takes. Sets d->head.
+static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
+  int k = -1, max_len = -1, sep_id = -1;
+  bool span_seen = false;  // a span_starts / span_ends / span_scores entry set max_len and sep_id
+  // an integer field of an output entry: 0 absent, 1 read into *v, -1 present but not an integer
+  auto int_field = [](const Json& oj, const char* key, int* v) {
+    const Json* f = oj.get(key);
+    if (!f) return 0;
+    if (f->type != Json::Num || f->num != (double)(int)f->num) return -1;
+    *v = (int)f->num;
+    return 1;
+  };
+  for (auto& oj : outs.arr) {
+    ModelOutput mo;
+    mo.name = oj.type == Json::Obj ? oj.get_str("name", "") : "";
+    const std::string kind = oj.type == Json::Obj ? oj.get_str("kind", "") : "";
+    const OutputKindInfo* ki = nullptr;
+    for (auto& i : kOutputKinds)
+      if (kind == i.name) ki = &i;
+    if (!ki) {
+      *err = "signature.outputs: unknown kind '" + kind + "' (";
+      for (auto& i : kOutputKinds) *err += std::string(&i == kOutputKinds ? "" : ", ") + i.name;
+      *err += ")";
+      return false;
+    }
+    mo.kind = (OutputKind)(ki - kOutputKinds);
+    if (mo.name.empty()) {
+      *err = "signature.outputs: every output needs a name";
+      return false;
+    }
+    for (auto& o : d->outputs)
+      if (o.name == mo.name || o.kind == mo.kind) {
+        *err = "signature.outputs: duplicate " + std::string(o.name == mo.name ? "name '" + mo.name + "'" : "kind '" + kind + "'");
+        return false;
+      }
+    const HeadKind h = ki->head, first = d->outputs.empty() ? h : kind_info(d->outputs.front().kind).head;
+    const std::string is = " ('" + mo.name + "' is " + kind + ")";
+    if ((h == HeadKind::FillMask) != (first == HeadKind::FillMask)) {
+      *err = "signature.outputs: fill-mask outputs (masked_positions, masked_top_k_ids, masked_top_k_probabilities,"
+             " masked_top_k_logits) cannot be mixed with classification, span or encoder outputs" + is;
+      return false;
+    }
+    if (h != HeadKind::FillMask) {
+      if ((h == HeadKind::Encoder) != (first == HeadKind::Encoder)) {
+        *err = "signature.outputs: encoder outputs (sequence_output, pooled_output, cls_embedding, mean_embedding) cannot be mixed"
+               " with classification or span outputs" + is;
+        return false;
+      }
+      if (const Json* nj = oj.get("normalize")) {
+        if (ki->fields != Fields::Normalize) {
+          *err = "signature.outputs: 'normalize' belongs to cls_embedding and mean_embedding" + is;
+          return false;
+        }
+        if (nj->type != Json::Bool) {
+          *err = "signature.outputs: '" + mo.name + "' has a 'normalize' that is not true or false";
+          return false;
+        }
+        (mo.kind == OutputKind::ClsEmbedding ? d->normalize_cls : d->normalize_mean) = nj->b;
+      }
+      if (h != HeadKind::Encoder && (h == HeadKind::Span) != (first == HeadKind::Span)) {
+        *err = "signature.outputs: span outputs (start_logits, end_logits, span_starts, span_ends, span_scores) cannot be mixed"
+               " with classification outputs" + is;
+        return false;
+      }
+    }
+    const bool span_fields = oj.get("max_answer_length") || oj.get("sep_id");
+    int v = 0;
+    switch (h) {
+      case HeadKind::FillMask:
+        if (oj.get("normalize") || span_fields) {
+          *err = "signature.outputs: 'normalize', 'max_answer_length' and 'sep_id' do not apply to fill-mask outputs" + is;
+          return false;
+        }
+        if (!takes_k(mo.kind) && oj.get("k")) {
+          *err = "signature.outputs: 'k' belongs to masked_top_k_ids, masked_top_k_probabilities and masked_top_k_logits" + is;
+          return false;
+        }
+        if (takes_k(mo.kind) && (int_field(oj, "k", &v) != 1 || v < 1 || (k >= 0 && v != k))) {
+          *err = "signature.outputs: '" + mo.name + "' needs an integer 'k' >= 1, the same for every fill-mask top-k output";
+          return false;
+        }
+        if (takes_k(mo.kind)) k = v;
+        break;
+      case HeadKind::Encoder:
+        if (oj.get("k") || span_fields) {
+          *err = "signature.outputs: 'k', 'max_answer_length' and 'sep_id' do not apply to encoder outputs" + is;
+          return false;
+        }
+        break;
+      case HeadKind::Span:
+        if (!takes_k(mo.kind)) {
+          if (oj.get("k") || span_fields) {
+            *err = "signature.outputs: 'k', 'max_answer_length' and 'sep_id' belong to span_starts, span_ends and span_scores" + is;
+            return false;
+          }
+          break;
+        }
+        if (int_field(oj, "k", &v) != 1 || (span_seen && v != k)) {
+          *err = "signature.outputs: '" + mo.name + "' needs an integer 'k', the same for every span output";
+          return false;
+        }
+        k = v;
+        if (int_field(oj, "max_answer_length", &v) != 1 || (span_seen && v != max_len)) {
+          *err = "signature.outputs: '" + mo.name + "' needs an integer 'max_answer_length', the same for every span output";
+          return false;
+        }
+        max_len = v;
+        v = -1;
+        if (const int r = int_field(oj, "sep_id", &v); r < 0 || (r == 1 && v < 0) || (span_seen && v != sep_id)) {
+          *err = "signature.outputs: '" + mo.name + "' has a 'sep_id' that is not a token id >= 0 or differs from the other"
+                 " span outputs' (give the same sep_id to every span output, or to none)";
+          return false;
+        }
+        sep_id = v;
+        span_seen = true;
+        break;
+      default:  // classification: 'k' on the top-k kinds only; max_answer_length and sep_id are ignored
+        if (!takes_k(mo.kind) && oj.get("k")) {
+          *err = "signature.outputs: 'k' belongs to the top-k outputs only" + is;
+          return false;
+        }
+        if (takes_k(mo.kind) && (int_field(oj, "k", &v) != 1 || (k >= 0 && v != k))) {
+          *err = "signature.outputs: '" + mo.name + "' needs an integer 'k', the same for both top-k outputs";
+          return false;
+        }
+        if (takes_k(mo.kind)) k = v;
+    }
+    d->outputs.push_back(mo);
+  }
+  d->head_k = span_seen ? k : k < 0 ? 0 : k;  // a span k is always given, and a negative one is refused by span_fits
+  d->span_max_len = span_seen ? max_len : 0;
+  d->span_sep_id = sep_id;
+  set_head(d);
+  return true;
+}
+
+// ------------------------------------------------------------------- the bundle each head's outputs need ----
+// The span, encoder and fill-mask heads read the request's ids / mask / segment ids where the embedding reads them
+static bool embed_graph(const ModelDesc& d, const std::string& outputs, const char* bundle, std::string* err) {
+  if (d.tmpl != Template::Graph) {
+    *err = "signature.outputs: " + outputs + " outputs need a graph bundle (" + bundle + ")";
+    return false;
+  }
+  if (d.ops.front().kind != OpKind::Embed) {
+    *err = "signature.outputs: " + outputs + " outputs need a graph bundle whose first op is 'embed'";
+    return false;
+  }
+  return true;
+}
+
+// the classify head reads the last op's (or the mlp's last layer's) N logits: head_n = N
+static bool check_classify_bundle(ModelDesc* d, std::string* err) {
+  if (d->tmpl == Template::Affine) {
+    *err = "signature.outputs needs an mlp or graph bundle (an affine bundle has no logits row)";
+    return false;
+  }
+  if (d->tmpl == Template::Graph && d->output_shape.size() != 1) {
+    *err = "signature.outputs needs a graph whose output is one vector of logits per row (output_shape has rank " +
+           std::to_string(d->output_shape.size()) + ")";
+    return false;
+  }
+  d->head_n = d->out_dim > 0x7fffffff ? 0 : (int)d->out_dim;
+  return true;
+}
+
+// the span head reads the per-token start / end logits [S, 1, 2] of the last op: head_n = S
+static bool check_span_bundle(ModelDesc* d, std::string* err) {
+  if (!embed_graph(*d, "span", "a BERT encoder ending in per-token start / end logits", err)) return false;
+  if (!d->input(InputRole::TypeIds)) {
+    *err = "signature.outputs: span outputs need a 'type_ids' input (the passage is segment 1)";
+    return false;
+  }
+  const int S = d->ops.front().h;
+  const GraphOp& last = d->ops.back();
+  if (last.oh != S || last.ow != 1 || last.cout != 2) {
+    *err = "signature.outputs: span outputs need a last op that writes [" + std::to_string(S) +
+           ", 1, 2] start / end logits per token (it writes [" + std::to_string(last.oh) + ", " + std::to_string(last.ow) +
+           ", " + std::to_string(last.cout) + "])";
+    return false;
+  }
+  if (!span_fits(S, d->span_max_len, d->head_k, declares_k(*d))) {
+    *err = "signature.outputs: no span kernel for S = " + std::to_string(S) + ", max_answer_length = " +
+           std::to_string(d->span_max_len) + " and k = " + std::to_string(d->head_k) + " (1 <= S <= " +
+           std::to_string(kSpanMaxS) + ", 1 <= max_answer_length <= S, 1 <= k <= " + std::to_string(kSpanMaxK) + ")";
+    return false;
+  }
+  d->head_n = S;
+  return true;
+}
+
+// the encoder head reads the last hidden states [S, 1, H]: what the last op writes, or, when the last op is the pooler (a
+// tanh dense over token 0), its source buffer: head_n = H, head_k = S
+static bool check_encoder_bundle(ModelDesc* d, std::string* err) {
+  if (!embed_graph(*d, "encoder", "a BERT encoder ending in its hidden states or pooler", err)) return false;
+  const int S = d->ops.front().h, H = d->ops.front().c;
+  const GraphOp& last = d->ops.back();
+  const GraphOp* prev = d->ops.size() >= 2 ? &d->ops[d->ops.size() - 2] : nullptr;
+  const bool hidden = last.oh == S && last.ow == 1 && last.cout == H;
+  const bool pooler = last.kind == OpKind::Dense && last.act == 3 && last.c == H && last.cout == H && last.src >= 0 &&
+                      last.lda == (int64_t)S * H && prev && prev->dst == last.src && prev->oh == S && prev->ow == 1 &&
+                      prev->cout == H;
+  if (!hidden && !pooler) {
+    const std::string sh = "[" + std::to_string(S) + ", 1, " + std::to_string(H) + "]";
+    *err = "signature.outputs: encoder outputs need a last op that writes the " + sh + " hidden states, or a tanh pooler"
+           " dense over token 0 of the " + sh + " hidden states the op before it writes (it writes [" +
+           std::to_string(last.oh) + ", " + std::to_string(last.ow) + ", " + std::to_string(last.cout) + "])";
+    return false;
+  }
+  d->encoder_pooler = pooler;
+  if (d->output(OutputKind::PooledOutput) && !pooler) {
+    *err = "signature.outputs: pooled_output needs a bundle whose last op is the pooler (a tanh dense over token 0)";
+    return false;
+  }
+  if (!encoder_fits(S, H, err)) return false;
+  d->head_n = H, d->head_k = S;
+  return true;
+}
+
+// the fill-mask head: one mask_gather op reads the encoder's [S, 1, H] hidden states, the ops after it run on its M slots
+// and the last one writes [M, 1, Vp] vocabulary logits: head_n = M
+static bool check_fill_mask_bundle(ModelDesc* d, int gathers, std::string* err) {
+  if (!embed_graph(*d, "fill-mask", "a BERT encoder, a mask_gather op and the MLM head", err)) return false;
+  if (gathers != 1) {
+    *err = "signature.outputs: fill-mask outputs need exactly one mask_gather op (the bundle has " + std::to_string(gathers) + ")";
+    return false;
+  }
+  const GraphOp& emb = d->ops.front();
+  const int S = emb.h, H = emb.c, V = emb.vocab;
+  const GraphOp* g = nullptr;
+  for (auto& o : d->ops)
+    if (o.kind == OpKind::MaskGather) g = &o;
+  const int M = g->oh;
+  if (g->src < 0 || g->h != S || g->w != 1 || g->c != H) {
+    *err = "signature.outputs: the mask_gather op needs the [" + std::to_string(S) + ", 1, " + std::to_string(H) +
+           "] hidden states of a scratch buffer (it reads [" + std::to_string(g->h) + ", " + std::to_string(g->w) + ", " +
+           std::to_string(g->c) + "] of buffer " + std::to_string(g->src) + ")";
+    return false;
+  }
+  if (g->mask_token_id < 1 || g->mask_token_id >= V) {
+    *err = "signature.outputs: mask_token_id " + std::to_string(g->mask_token_id) + " is not a token id in [1, " +
+           std::to_string(V) + ")";
+    return false;
+  }
+  const GraphOp& last = d->ops.back();
+  if (last.oh != M || last.ow != 1 || last.cout < V) {
+    *err = "signature.outputs: fill-mask outputs need a last op that writes [" + std::to_string(M) + ", 1, Vp] logits, Vp >= " +
+           std::to_string(V) + " (it writes [" + std::to_string(last.oh) + ", " + std::to_string(last.ow) + ", " +
+           std::to_string(last.cout) + "])";
+    return false;
+  }
+  if (!mask_gather_supported(S, H, M) || !fill_mask_fits(M, V, d->head_k, declares_k(*d))) {
+    *err = "signature.outputs: no fill-mask kernels for S = " + std::to_string(S) + ", H = " + std::to_string(H) + ", M = " +
+           std::to_string(M) + ", vocab = " + std::to_string(V) + " and k = " + std::to_string(d->head_k) + " (1 <= M <= S <= " +
+           std::to_string(kMaskGatherMaxS) + ", H <= " + std::to_string(kMaskGatherMaxH) + ", 1 <= vocab <= " +
+           std::to_string(kHeadMaxN) + ", 1 <= k <= min(vocab, " + std::to_string(kHeadMaxK) + "))";
+    return false;
+  }
+  d->mlm_vocab = V;
+  d->mlm_mask_token_id = g->mask_token_id;
+  d->head_n = M;
+  return true;
+}
+
 bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
   if (j.type != Json::Obj) {
     *err = "manifest is not a JSON object";
@@ -261,164 +544,7 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         *err = "signature.outputs must list 1 to " + std::to_string(kMaxOutputs) + " outputs";
         return false;
       }
-      int k = -1, max_len = -1, sep_id = -1;
-      bool span_seen = false;  // a span_starts / span_ends / span_scores entry set max_len and sep_id
-      // an integer field of an output entry: 0 absent, 1 read into *v, -1 present but not an integer
-      auto int_field = [](const Json& oj, const char* key, int* v) {
-        const Json* f = oj.get(key);
-        if (!f) return 0;
-        if (f->type != Json::Num || f->num != (double)(int)f->num) return -1;
-        *v = (int)f->num;
-        return 1;
-      };
-      for (auto& oj : outs->arr) {
-        ModelOutput mo;
-        mo.name = oj.type == Json::Obj ? oj.get_str("name", "") : "";
-        const std::string kind = oj.type == Json::Obj ? oj.get_str("kind", "") : "";
-        if (kind == "logits") mo.kind = OutputKind::Logits;
-        else if (kind == "probabilities") mo.kind = OutputKind::Probabilities;
-        else if (kind == "classes") mo.kind = OutputKind::Classes;
-        else if (kind == "top_k_classes") mo.kind = OutputKind::TopKClasses;
-        else if (kind == "top_k_probabilities") mo.kind = OutputKind::TopKProbabilities;
-        else if (kind == "start_logits") mo.kind = OutputKind::StartLogits;
-        else if (kind == "end_logits") mo.kind = OutputKind::EndLogits;
-        else if (kind == "span_starts") mo.kind = OutputKind::SpanStarts;
-        else if (kind == "span_ends") mo.kind = OutputKind::SpanEnds;
-        else if (kind == "span_scores") mo.kind = OutputKind::SpanScores;
-        else if (kind == "sequence_output") mo.kind = OutputKind::SequenceOutput;
-        else if (kind == "pooled_output") mo.kind = OutputKind::PooledOutput;
-        else if (kind == "cls_embedding") mo.kind = OutputKind::ClsEmbedding;
-        else if (kind == "mean_embedding") mo.kind = OutputKind::MeanEmbedding;
-        else if (kind == "masked_positions") mo.kind = OutputKind::MaskedPositions;
-        else if (kind == "masked_top_k_ids") mo.kind = OutputKind::MaskedTopKIds;
-        else if (kind == "masked_top_k_probabilities") mo.kind = OutputKind::MaskedTopKProbabilities;
-        else if (kind == "masked_top_k_logits") mo.kind = OutputKind::MaskedTopKLogits;
-        else {
-          *err = "signature.outputs: unknown kind '" + kind + "' (logits, probabilities, classes, top_k_classes, top_k_probabilities, "
-                 "start_logits, end_logits, span_starts, span_ends, span_scores, sequence_output, pooled_output, cls_embedding, "
-                 "mean_embedding, masked_positions, masked_top_k_ids, masked_top_k_probabilities, masked_top_k_logits)";
-          return false;
-        }
-        if (mo.name.empty()) {
-          *err = "signature.outputs: every output needs a name";
-          return false;
-        }
-        for (auto& o : d->outputs)
-          if (o.name == mo.name || o.kind == mo.kind) {
-            *err = "signature.outputs: duplicate " + std::string(o.name == mo.name ? "name '" + mo.name + "'" : "kind '" + kind + "'");
-            return false;
-          }
-        if (!d->outputs.empty() && is_mlm_kind(d->outputs.front().kind) != is_mlm_kind(mo.kind)) {
-          *err = "signature.outputs: fill-mask outputs (masked_positions, masked_top_k_ids, masked_top_k_probabilities,"
-                 " masked_top_k_logits) cannot be mixed with classification, span or encoder outputs ('" + mo.name + "' is " +
-                 kind + ")";
-          return false;
-        }
-        if (is_mlm_kind(mo.kind)) {
-          if (oj.get("normalize") || oj.get("max_answer_length") || oj.get("sep_id")) {
-            *err = "signature.outputs: 'normalize', 'max_answer_length' and 'sep_id' do not apply to fill-mask outputs ('" +
-                   mo.name + "' is " + kind + ")";
-            return false;
-          }
-          if (mo.kind == OutputKind::MaskedPositions) {
-            if (oj.get("k")) {
-              *err = "signature.outputs: 'k' belongs to masked_top_k_ids, masked_top_k_probabilities and masked_top_k_logits ('" +
-                     mo.name + "' is masked_positions)";
-              return false;
-            }
-          } else {
-            int v = 0;
-            if (int_field(oj, "k", &v) != 1 || v < 1 || (k >= 0 && v != k)) {
-              *err = "signature.outputs: '" + mo.name + "' needs an integer 'k' >= 1, the same for every fill-mask top-k output";
-              return false;
-            }
-            k = v;
-          }
-          d->outputs.push_back(mo);
-          continue;
-        }
-        if (!d->outputs.empty() && is_encoder_kind(d->outputs.front().kind) != is_encoder_kind(mo.kind)) {
-          *err = "signature.outputs: encoder outputs (sequence_output, pooled_output, cls_embedding, mean_embedding) cannot be mixed"
-                 " with classification or span outputs ('" + mo.name + "' is " + kind + ")";
-          return false;
-        }
-        const bool normalizable = mo.kind == OutputKind::ClsEmbedding || mo.kind == OutputKind::MeanEmbedding;
-        if (const Json* nj = oj.get("normalize")) {
-          if (!normalizable) {
-            *err = "signature.outputs: 'normalize' belongs to cls_embedding and mean_embedding ('" + mo.name + "' is " + kind + ")";
-            return false;
-          }
-          if (nj->type != Json::Bool) {
-            *err = "signature.outputs: '" + mo.name + "' has a 'normalize' that is not true or false";
-            return false;
-          }
-          (mo.kind == OutputKind::ClsEmbedding ? d->normalize_cls : d->normalize_mean) = nj->b;
-        }
-        if (is_encoder_kind(mo.kind)) {
-          if (oj.get("k") || oj.get("max_answer_length") || oj.get("sep_id")) {
-            *err = "signature.outputs: 'k', 'max_answer_length' and 'sep_id' do not apply to encoder outputs ('" + mo.name + "' is " +
-                   kind + ")";
-            return false;
-          }
-          d->outputs.push_back(mo);
-          continue;
-        }
-        if (!d->outputs.empty() && is_span_kind(d->outputs.front().kind) != is_span_kind(mo.kind)) {
-          *err = "signature.outputs: span outputs (start_logits, end_logits, span_starts, span_ends, span_scores) cannot be mixed"
-                 " with classification outputs ('" + mo.name + "' is " + kind + ")";
-          return false;
-        }
-        if (is_span_kind(mo.kind)) {
-          if (!is_span_result_kind(mo.kind)) {
-            if (oj.get("k") || oj.get("max_answer_length") || oj.get("sep_id")) {
-              *err = "signature.outputs: 'k', 'max_answer_length' and 'sep_id' belong to span_starts, span_ends and span_scores ('" +
-                     mo.name + "' is " + kind + ")";
-              return false;
-            }
-          } else {
-            int v = 0;
-            int r = int_field(oj, "k", &v);
-            if (r != 1 || (span_seen && v != k)) {
-              *err = "signature.outputs: '" + mo.name + "' needs an integer 'k', the same for every span output";
-              return false;
-            }
-            k = v;
-            r = int_field(oj, "max_answer_length", &v);
-            if (r != 1 || (span_seen && v != max_len)) {
-              *err = "signature.outputs: '" + mo.name + "' needs an integer 'max_answer_length', the same for every span output";
-              return false;
-            }
-            max_len = v;
-            v = -1;
-            r = int_field(oj, "sep_id", &v);
-            if (r < 0 || (r == 1 && v < 0) || (span_seen && v != sep_id)) {
-              *err = "signature.outputs: '" + mo.name + "' has a 'sep_id' that is not a token id >= 0 or differs from the other"
-                     " span outputs' (give the same sep_id to every span output, or to none)";
-              return false;
-            }
-            sep_id = v;
-            span_seen = true;
-          }
-          d->outputs.push_back(mo);
-          continue;
-        }
-        const bool topk = mo.kind == OutputKind::TopKClasses || mo.kind == OutputKind::TopKProbabilities;
-        if (topk) {
-          const Json* kj = oj.get("k");
-          if (!kj || kj->type != Json::Num || kj->num != (double)(int)kj->num || (k >= 0 && (int)kj->num != k)) {
-            *err = "signature.outputs: '" + mo.name + "' needs an integer 'k', the same for both top-k outputs";
-            return false;
-          }
-          k = (int)kj->num;
-        } else if (oj.get("k")) {
-          *err = "signature.outputs: 'k' belongs to the top-k outputs only ('" + mo.name + "' is " + kind + ")";
-          return false;
-        }
-        d->outputs.push_back(mo);
-      }
-      d->head_k = span_seen ? k : k < 0 ? 0 : k;  // a span k is always given, and a negative one is refused below
-      d->span_max_len = span_seen ? max_len : 0;
-      d->span_sep_id = sep_id;
+      if (!parse_outputs(*outs, d, err)) return false;
     }
   }
   if (const Json* ex = j.get("extra_signatures")) {
@@ -659,153 +785,29 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
   finish(d);
   int gathers = 0;
   for (auto& o : d->ops) gathers += o.kind == OpKind::MaskGather;
-  if (gathers && !d->mlm_head()) {
+  if (gathers && d->head != HeadKind::FillMask) {
     *err = "graph manifest: a mask_gather op needs fill-mask outputs (masked_positions, masked_top_k_ids, "
            "masked_top_k_probabilities, masked_top_k_logits)";
     return false;
   }
-  if (!d->outputs.empty()) {
-    if (d->mlm_head()) {
-      // the gather reads the request's ids / mask where the embedding reads them and the encoder's [S, 1, H] hidden states;
-      // the ops after it run on its M slots and the last one writes [M, 1, Vp] vocabulary logits
-      if (d->tmpl != Template::Graph) {
-        *err = "signature.outputs: fill-mask outputs need a graph bundle (a BERT encoder, a mask_gather op and the MLM head)";
-        return false;
-      }
-      if (d->ops.front().kind != OpKind::Embed) {
-        *err = "signature.outputs: fill-mask outputs need a graph bundle whose first op is 'embed'";
-        return false;
-      }
-      if (gathers != 1) {
-        *err = "signature.outputs: fill-mask outputs need exactly one mask_gather op (the bundle has " + std::to_string(gathers) + ")";
-        return false;
-      }
-      const GraphOp& emb = d->ops.front();
-      const int S = emb.h, H = emb.c, V = emb.vocab;
-      const GraphOp* g = nullptr;
-      for (auto& o : d->ops)
-        if (o.kind == OpKind::MaskGather) g = &o;
-      const int M = g->oh;
-      if (g->src < 0 || g->h != S || g->w != 1 || g->c != H) {
-        *err = "signature.outputs: the mask_gather op needs the [" + std::to_string(S) + ", 1, " + std::to_string(H) +
-               "] hidden states of a scratch buffer (it reads [" + std::to_string(g->h) + ", " + std::to_string(g->w) + ", " +
-               std::to_string(g->c) + "] of buffer " + std::to_string(g->src) + ")";
-        return false;
-      }
-      if (g->mask_token_id < 1 || g->mask_token_id >= V) {
-        *err = "signature.outputs: mask_token_id " + std::to_string(g->mask_token_id) + " is not a token id in [1, " +
-               std::to_string(V) + ")";
-        return false;
-      }
-      const GraphOp& last = d->ops.back();
-      if (last.oh != M || last.ow != 1 || last.cout < V) {
-        *err = "signature.outputs: fill-mask outputs need a last op that writes [" + std::to_string(M) + ", 1, Vp] logits, Vp >= " +
-               std::to_string(V) + " (it writes [" + std::to_string(last.oh) + ", " + std::to_string(last.ow) + ", " +
-               std::to_string(last.cout) + "])";
-        return false;
-      }
-      const bool topk = d->output(OutputKind::MaskedTopKIds) || d->output(OutputKind::MaskedTopKProbabilities) ||
-                        d->output(OutputKind::MaskedTopKLogits);
-      if (!mask_gather_supported(S, H, M) || !fill_mask_supported(M, V, topk ? d->head_k : 1)) {
-        *err = "signature.outputs: no fill-mask kernels for S = " + std::to_string(S) + ", H = " + std::to_string(H) + ", M = " +
-               std::to_string(M) + ", vocab = " + std::to_string(V) + " and k = " + std::to_string(d->head_k) + " (1 <= M <= S <= " +
-               std::to_string(kMaskGatherMaxS) + ", H <= " + std::to_string(kMaskGatherMaxH) + ", 1 <= vocab <= " +
-               std::to_string(kHeadMaxN) + ", 1 <= k <= min(vocab, " + std::to_string(kHeadMaxK) + "))";
-        return false;
-      }
-      d->mlm_vocab = V;
-      d->mlm_mask_token_id = g->mask_token_id;
-    } else if (d->encoder_head()) {
-      // the encoder head reads the last hidden states [S, 1, H]: what the last op writes, or, when the last op is the pooler
-      // (a tanh dense over token 0), its source buffer; and the request's ids / mask where the embedding reads them
-      if (d->tmpl != Template::Graph) {
-        *err = "signature.outputs: encoder outputs need a graph bundle (a BERT encoder ending in its hidden states or pooler)";
-        return false;
-      }
-      if (d->ops.front().kind != OpKind::Embed) {
-        *err = "signature.outputs: encoder outputs need a graph bundle whose first op is 'embed'";
-        return false;
-      }
-      const int S = d->ops.front().h, H = d->ops.front().c;
-      const GraphOp& last = d->ops.back();
-      const GraphOp* prev = d->ops.size() >= 2 ? &d->ops[d->ops.size() - 2] : nullptr;
-      const bool hidden = last.oh == S && last.ow == 1 && last.cout == H;
-      const bool pooler = last.kind == OpKind::Dense && last.act == 3 && last.c == H && last.cout == H && last.src >= 0 &&
-                          last.lda == (int64_t)S * H && prev && prev->dst == last.src &&
-                          prev->oh == S && prev->ow == 1 && prev->cout == H;
-      if (!hidden && !pooler) {
-        const std::string sh = "[" + std::to_string(S) + ", 1, " + std::to_string(H) + "]";
-        *err = "signature.outputs: encoder outputs need a last op that writes the " + sh + " hidden states, or a tanh pooler"
-               " dense over token 0 of the " + sh + " hidden states the op before it writes (it writes [" +
-               std::to_string(last.oh) + ", " + std::to_string(last.ow) + ", " + std::to_string(last.cout) + "])";
-        return false;
-      }
-      d->encoder_pooler = pooler;
-      if (d->output(OutputKind::PooledOutput) && !pooler) {
-        *err = "signature.outputs: pooled_output needs a bundle whose last op is the pooler (a tanh dense over token 0)";
-        return false;
-      }
-      if (!encoder_head_supported(S, H)) {
-        *err = "signature.outputs: no encoder head kernel for S = " + std::to_string(S) + " and H = " + std::to_string(H) +
-               " (1 <= S <= " + std::to_string(kEncoderMaxS) + ", 1 <= H <= " + std::to_string(kEncoderMaxH) + ")";
-        return false;
-      }
-    } else if (d->span_head()) {
-      // the span head reads the request's ids / mask / segment ids where the embedding does, and the per-token start / end
-      // logits [S, 1, 2] of the last op
-      if (d->tmpl != Template::Graph) {
-        *err = "signature.outputs: span outputs need a graph bundle (a BERT encoder ending in per-token start / end logits)";
-        return false;
-      }
-      if (d->ops.front().kind != OpKind::Embed) {
-        *err = "signature.outputs: span outputs need a graph bundle whose first op is 'embed'";
-        return false;
-      }
-      if (!d->input(InputRole::TypeIds)) {
-        *err = "signature.outputs: span outputs need a 'type_ids' input (the passage is segment 1)";
-        return false;
-      }
-      const int S = d->ops.front().h;
-      const GraphOp& last = d->ops.back();
-      if (last.oh != S || last.ow != 1 || last.cout != 2) {
-        *err = "signature.outputs: span outputs need a last op that writes [" + std::to_string(S) +
-               ", 1, 2] start / end logits per token (it writes [" + std::to_string(last.oh) + ", " + std::to_string(last.ow) +
-               ", " + std::to_string(last.cout) + "])";
-        return false;
-      }
-      const bool spans = d->output(OutputKind::SpanStarts) || d->output(OutputKind::SpanEnds) || d->output(OutputKind::SpanScores);
-      if (!span_supported(S, spans ? d->span_max_len : 1, spans ? d->head_k : 1)) {
-        *err = "signature.outputs: no span kernel for S = " + std::to_string(S) + ", max_answer_length = " +
-               std::to_string(d->span_max_len) + " and k = " + std::to_string(d->head_k) + " (1 <= S <= " +
-               std::to_string(kSpanMaxS) + ", 1 <= max_answer_length <= S, 1 <= k <= " + std::to_string(kSpanMaxK) + ")";
-        return false;
-      }
-    } else if (d->tmpl == Template::Affine) {
-      *err = "signature.outputs needs an mlp or graph bundle (an affine bundle has no logits row)";
-      return false;
-    }
-    if (!d->span_head() && !d->encoder_head() && !d->mlm_head() && d->tmpl == Template::Graph && d->output_shape.size() != 1) {
-      *err = "signature.outputs needs a graph whose output is one vector of logits per row (output_shape has rank " +
-             std::to_string(d->output_shape.size()) + ")";
-      return false;
-    }
-    for (auto& o : d->outputs) {
-      bool clash = d->inputs.empty() && o.name == d->input_name;
-      for (auto& i : d->inputs) clash = clash || o.name == i.name;
-      if (clash) {
-        *err = "signature.outputs: '" + o.name + "' is also an input name";
-        return false;
-      }
-    }
-    // the last op's per-row width; a span head answers S start and S end logits per row; an encoder head's rows are
-    // [S, H] (head_k = S) and [H] (head_n = H)
-    d->head_n = d->span_head() ? d->ops.front().h : d->out_dim > 0x7fffffff ? 0 : (int)d->out_dim;
-    if (d->encoder_head()) d->head_n = d->ops.front().c, d->head_k = d->ops.front().h;
-    // a fill-mask head's rows are [M] positions and [M, k] top-k (head_k as declared, 0: positions only)
-    if (d->mlm_head()) d->head_n = d->ops.back().oh;
-    if (!layout_outputs(d, err)) return false;
+  if (d->outputs.empty()) return true;
+  bool ok = false;
+  switch (d->head) {
+    case HeadKind::FillMask: ok = check_fill_mask_bundle(d, gathers, err); break;
+    case HeadKind::Encoder: ok = check_encoder_bundle(d, err); break;
+    case HeadKind::Span: ok = check_span_bundle(d, err); break;
+    default: ok = check_classify_bundle(d, err);
   }
-  return true;
+  if (!ok) return false;
+  for (auto& o : d->outputs) {
+    bool clash = d->inputs.empty() && o.name == d->input_name;
+    for (auto& i : d->inputs) clash = clash || o.name == i.name;
+    if (clash) {
+      *err = "signature.outputs: '" + o.name + "' is also an input name";
+      return false;
+    }
+  }
+  return layout_outputs(d, err);
 }
 
 }  // namespace tfsc

@@ -58,16 +58,15 @@ struct ModelInput {
   int64_t offset = 0;  // elements into the packed request row (inputs in byte-wise sorted name order, S values each)
 };
 
-// One declared output of a multi-output bundle (signature.outputs). The classification kinds are computed from the last
-// op's N logits by the classify head (head.cu). Per row: logits / probabilities [N] float, classes a scalar int64 (two
-// 32-bit words, little-endian), top_k_classes [k] int32, top_k_probabilities [k] float. The span kinds (question answering)
-// are computed from the last op's [S, 1, 2] per-token logits by the span head (span.cu): start_logits / end_logits [S]
-// float, span_starts / span_ends [k] int32, span_scores [k] float. The encoder kinds (embeddings) are computed from the
-// last hidden states [S, 1, H] (and the pooler's [H]) by the encoder head (encoder_head.cu): sequence_output [S, H] float,
-// pooled_output / cls_embedding / mean_embedding [H] float. The fill-mask kinds (masked-language-model prediction) are
-// computed from the [M, 1, Vp] vocabulary logits of the M [MASK] slots a mask_gather op selected, by the fill-mask head
-// (mlm.cu): masked_positions [M] int32, masked_top_k_ids [M, k] int32, masked_top_k_probabilities / masked_top_k_logits
-// [M, k] float. New kinds go at the end: the forward hop sends the enum's numbers.
+// The head that computes a bundle's signature.outputs; every output of a bundle belongs to the same one (None: no outputs).
+// Classify: the last op's N logits (head.cu). Span (question answering): the last op's [S, 1, 2] per-token start / end
+// logits (span.cu). Encoder (embeddings): the last hidden states [S, 1, H] and the pooler's [H] (encoder_head.cu).
+// FillMask (masked-language-model prediction): the [M, 1, Vp] vocabulary logits of the M [MASK] slots a mask_gather op
+// selected (mlm.cu).
+enum class HeadKind { None, Classify, Span, Encoder, FillMask };
+
+// One declared output of a multi-output bundle (signature.outputs). Its name, head, dtype and per-row shape are in the
+// kind table (model.cc). New kinds go at the end: the forward hop sends the enum's numbers.
 enum class OutputKind {
   Logits, Probabilities, Classes, TopKClasses, TopKProbabilities,
   StartLogits, EndLogits, SpanStarts, SpanEnds, SpanScores,
@@ -85,8 +84,7 @@ const char* output_kind_name(OutputKind k);
 int output_dtype(OutputKind k);  // TFSC_DT_FLOAT / TFSC_DT_INT64 / TFSC_DT_INT32
 // What one row of an output kind looks like, the one rule behind the packed layout, every response writer and the
 // metadata: `width` 32-bit words holding a scalar (rank 0: classes, one int64 in 2 words), a vector of dims[0] values
-// (rank 1: N or S for the logits kinds, k for the top-k and span kinds, H for the embedding kinds) or a dims[0] x dims[1]
-// matrix (rank 2: sequence_output, S x H; the fill-mask top-k kinds, M x k).
+// (rank 1) or a dims[0] x dims[1] matrix (rank 2), in terms of the bundle's head_n / head_k (ModelDesc).
 struct OutputForm {
   int64_t width = 0;
   int dtype = TFSC_DT_FLOAT;
@@ -94,10 +92,6 @@ struct OutputForm {
   int64_t dims[2] = {0, 0};
 };
 OutputForm output_form(OutputKind k, int head_n, int head_k);
-bool is_span_kind(OutputKind k);        // start_logits .. span_scores
-bool is_span_result_kind(OutputKind k); // span_starts / span_ends / span_scores (they carry k and max_answer_length)
-bool is_encoder_kind(OutputKind k);     // sequence_output, pooled_output, cls_embedding, mean_embedding
-bool is_mlm_kind(OutputKind k);         // masked_positions, masked_top_k_ids / _probabilities / _logits
 constexpr int kMaxOutputs = 5;
 
 struct ModelDesc {
@@ -126,21 +120,22 @@ struct ModelDesc {
     return nullptr;
   }
   // signature.outputs, sorted by name (= packed response row order); empty for single-output bundles (output_name, out_dim
-  // elements). With outputs, out_dim is the packed row width and head_n / head_k the logits width and top-k (0: none).
-  // Span outputs: head_n = S, head_k = the number of spans (0: logits only); span_max_len = max_answer_length and
-  // span_sep_id = sep_id (-1: none) are known to the owner only, the kernel's business.
-  // Encoder outputs: head_n = H, head_k = S; encoder_pooler = the last op is the pooler (it writes pooled_output, and the
-  // hidden states are its source buffer); normalize_cls / normalize_mean, like max_answer_length, are the owner's.
+  // elements). With outputs, out_dim is the packed row width, `head` the head that computes them, and head_n / head_k
+  // the two numbers every output's row shape is given in (output_form), which the forward hop carries:
+  //   Classify: head_n = N logits, head_k = the top-k k (0: no top-k output).
+  //   Span:     head_n = S, head_k = the number of spans (0: logits only).
+  //   Encoder:  head_n = H, head_k = S.
+  //   FillMask: head_n = M (the mask_gather op's slots), head_k = k (0: masked_positions only).
+  // The rest is known to the owner only, the kernels' business: a span head's span_max_len = max_answer_length and
+  // span_sep_id = sep_id (-1: none); an encoder head's encoder_pooler (the last op is the pooler: it writes pooled_output,
+  // and the hidden states are its source buffer) and normalize_cls / normalize_mean; a fill-mask head's mlm_vocab (the
+  // embed op's vocab, the logits the head reads of each Vp-wide row) and mlm_mask_token_id.
   std::vector<ModelOutput> outputs;
+  HeadKind head = HeadKind::None;
   int head_n = 0, head_k = 0;
   int span_max_len = 0, span_sep_id = -1;
-  // Fill-mask outputs: head_n = M (the mask_gather op's slots), head_k = k (0: masked_positions only); mlm_vocab (the embed
-  // op's vocab, the logits the head reads of each Vp-wide row) and mlm_mask_token_id are the owner's.
   bool encoder_pooler = false, normalize_cls = false, normalize_mean = false;
   int mlm_vocab = 0, mlm_mask_token_id = 0;
-  bool span_head() const { return !outputs.empty() && is_span_kind(outputs.front().kind); }
-  bool encoder_head() const { return !outputs.empty() && is_encoder_kind(outputs.front().kind); }
-  bool mlm_head() const { return !outputs.empty() && is_mlm_kind(outputs.front().kind); }
   const ModelOutput* output(OutputKind k) const {
     for (auto& o : outputs)
       if (o.kind == k) return &o;
@@ -162,8 +157,8 @@ struct ModelDesc {
   size_t mlm_positions_offset(int64_t rows) const;
 };
 
-// Sort d->outputs by name, set their offsets and widths from d->head_n / d->head_k and d->out_dim to the packed row width.
-// Fails on a shape the head kernel cannot run (head_supported).
+// Set d->head from the first output's kind, sort d->outputs by name, set their offsets and widths from d->head_n / d->head_k
+// and d->out_dim to the packed row width. Fails on a shape the head kernel cannot run (head_supported and its kin).
 bool layout_outputs(ModelDesc* d, std::string* err);
 // "'classes' (int64), 'logits' (float), ..." for error messages
 std::string expected_outputs(const ModelDesc& d);

@@ -596,87 +596,83 @@ static bool conv_tc_enabled() {  // TFSC_CONV_TC=0: explicit im2col + GEMM (the 
   return v;
 }
 
-// multi-output bundles: one head launch writes every declared output of a row at its offset in the packed row (out_dim words)
-static cudaError_t run_head(const ModelDesc& d, const float* logits, int64_t rows, char* y, cudaStream_t st) {
-  HeadOutputs o;
+// multi-output bundles: one launch of the bundle's head writes every declared output of a row at its offset in the packed
+// row (out_dim words). `out` is what the last op (or the mlp's last layer) wrote: N logits (classify), [S, 2] start / end
+// logits (span), the [S, H] hidden states or, under a pooler, its [H] output (encoder), [M, Vp] vocabulary logits
+// (fill-mask). The graph heads read the request's ids / mask / segment ids where the embedding reads them (`in`), an
+// encoder under a pooler its source buffer (`hidden`), a fill-mask head the mask_gather op's [rows, M] `positions`.
+static cudaError_t run_head(const ModelDesc& d, const float* out, const SpanInputs& in, const float* hidden, const int* positions,
+                            int64_t rows, char* y, cudaStream_t st) {
   float* yf = reinterpret_cast<float*>(y);
   const int64_t ld = d.out_dim;
-  for (const ModelOutput& m : d.outputs) {
-    float* p = yf + m.offset;
-    switch (m.kind) {
-      case OutputKind::Logits: o.logits = p, o.logits_ld = ld; break;
-      case OutputKind::Probabilities: o.probs = p, o.probs_ld = ld; break;
-      case OutputKind::Classes: o.classes = reinterpret_cast<int*>(p), o.classes_ld = ld; break;
-      case OutputKind::TopKClasses: o.topk_idx = reinterpret_cast<int*>(p), o.topk_idx_ld = ld; break;
-      case OutputKind::TopKProbabilities: o.topk_prob = p, o.topk_prob_ld = ld; break;
-      default: break;  // span kinds: run_span_head
+  switch (d.head) {
+    case HeadKind::Span: {
+      SpanOutputs o;
+      for (const ModelOutput& m : d.outputs) {
+        float* p = yf + m.offset;
+        switch (m.kind) {
+          case OutputKind::StartLogits: o.start_logits = p, o.start_ld = ld; break;
+          case OutputKind::EndLogits: o.end_logits = p, o.end_ld = ld; break;
+          case OutputKind::SpanStarts: o.starts = reinterpret_cast<int*>(p), o.starts_ld = ld; break;
+          case OutputKind::SpanEnds: o.ends = reinterpret_cast<int*>(p), o.ends_ld = ld; break;
+          case OutputKind::SpanScores: o.scores = p, o.scores_ld = ld; break;
+          default: break;
+        }
+      }
+      return launch_span_head(out, in, (int)rows, d.head_n, d.span_max_len, d.head_k, o, st);
     }
-  }
-  return launch_classify_head(logits, (int)rows, d.head_n, d.head_k, o, st);
-}
-
-// question-answering bundles: one span head launch reads the last op's [rows, S, 2] logits and the request's ids / mask /
-// segment ids (`in`, where the embedding reads them) and writes every declared output at its offset in the packed row
-static cudaError_t run_span_head(const ModelDesc& d, const float* logits, const SpanInputs& in, int64_t rows, char* y,
-                                 cudaStream_t st) {
-  SpanOutputs o;
-  float* yf = reinterpret_cast<float*>(y);
-  const int64_t ld = d.out_dim;
-  for (const ModelOutput& m : d.outputs) {
-    float* p = yf + m.offset;
-    switch (m.kind) {
-      case OutputKind::StartLogits: o.start_logits = p, o.start_ld = ld; break;
-      case OutputKind::EndLogits: o.end_logits = p, o.end_ld = ld; break;
-      case OutputKind::SpanStarts: o.starts = reinterpret_cast<int*>(p), o.starts_ld = ld; break;
-      case OutputKind::SpanEnds: o.ends = reinterpret_cast<int*>(p), o.ends_ld = ld; break;
-      case OutputKind::SpanScores: o.scores = p, o.scores_ld = ld; break;
-      default: break;
+    case HeadKind::Encoder: {
+      EncoderOutputs o;
+      for (const ModelOutput& m : d.outputs) {
+        float* p = yf + m.offset;
+        switch (m.kind) {
+          case OutputKind::SequenceOutput: o.sequence = p, o.sequence_ld = ld; break;
+          case OutputKind::PooledOutput: o.pooled = p, o.pooled_ld = ld; break;
+          case OutputKind::ClsEmbedding: o.cls = p, o.cls_ld = ld; break;
+          case OutputKind::MeanEmbedding: o.mean = p, o.mean_ld = ld; break;
+          default: break;
+        }
+      }
+      o.normalize_cls = d.normalize_cls;
+      o.normalize_mean = d.normalize_mean;
+      EncoderInputs e;
+      e.ids = in.ids;
+      e.mask = in.mask;
+      e.stride = in.stride ? in.stride : d.ops.front().h;
+      return launch_encoder_head(d.encoder_pooler ? hidden : out, d.encoder_pooler ? out : nullptr, e, (int)rows, d.head_k,
+                                 d.head_n, o, st);
     }
-  }
-  return launch_span_head(logits, in, (int)rows, d.head_n, d.span_max_len, d.head_k, o, st);
-}
-
-// embedding bundles: one encoder head launch reads the last hidden states [rows, S, H] (and, with a pooler, its [rows, H]
-// output) and the request's ids / mask (`in`, where the embedding reads them), and writes every declared output at its
-// offset in the packed row
-static cudaError_t run_encoder_head(const ModelDesc& d, const float* hidden, const float* pooled, const EncoderInputs& in,
-                                    int64_t rows, char* y, cudaStream_t st) {
-  EncoderOutputs o;
-  float* yf = reinterpret_cast<float*>(y);
-  const int64_t ld = d.out_dim;
-  for (const ModelOutput& m : d.outputs) {
-    float* p = yf + m.offset;
-    switch (m.kind) {
-      case OutputKind::SequenceOutput: o.sequence = p, o.sequence_ld = ld; break;
-      case OutputKind::PooledOutput: o.pooled = p, o.pooled_ld = ld; break;
-      case OutputKind::ClsEmbedding: o.cls = p, o.cls_ld = ld; break;
-      case OutputKind::MeanEmbedding: o.mean = p, o.mean_ld = ld; break;
-      default: break;
+    case HeadKind::FillMask: {
+      FillMaskOutputs o;
+      for (const ModelOutput& m : d.outputs) {
+        float* p = yf + m.offset;
+        switch (m.kind) {
+          case OutputKind::MaskedPositions: o.positions = reinterpret_cast<int*>(p), o.positions_ld = ld; break;
+          case OutputKind::MaskedTopKIds: o.ids = reinterpret_cast<int*>(p), o.ids_ld = ld; break;
+          case OutputKind::MaskedTopKProbabilities: o.probs = p, o.probs_ld = ld; break;
+          case OutputKind::MaskedTopKLogits: o.logits = p, o.logits_ld = ld; break;
+          default: break;
+        }
+      }
+      return launch_fill_mask_head(out, d.ops.back().cout, positions, (int)rows, d.head_n, d.mlm_vocab, d.head_k, o, st);
     }
-  }
-  o.normalize_cls = d.normalize_cls;
-  o.normalize_mean = d.normalize_mean;
-  return launch_encoder_head(hidden, pooled, in, (int)rows, d.head_k, d.head_n, o, st);
-}
-
-// fill-mask bundles: one head launch reads the last op's [rows, M, Vp] vocabulary logits and the gather's positions
-// [rows, M], and writes every declared output at its offset in the packed row
-static cudaError_t run_fill_mask_head(const ModelDesc& d, const float* logits, const int* positions, int64_t rows, char* y,
-                                      cudaStream_t st) {
-  FillMaskOutputs o;
-  float* yf = reinterpret_cast<float*>(y);
-  const int64_t ld = d.out_dim;
-  for (const ModelOutput& m : d.outputs) {
-    float* p = yf + m.offset;
-    switch (m.kind) {
-      case OutputKind::MaskedPositions: o.positions = reinterpret_cast<int*>(p), o.positions_ld = ld; break;
-      case OutputKind::MaskedTopKIds: o.ids = reinterpret_cast<int*>(p), o.ids_ld = ld; break;
-      case OutputKind::MaskedTopKProbabilities: o.probs = p, o.probs_ld = ld; break;
-      case OutputKind::MaskedTopKLogits: o.logits = p, o.logits_ld = ld; break;
-      default: break;
+    case HeadKind::Classify: {
+      HeadOutputs o;
+      for (const ModelOutput& m : d.outputs) {
+        float* p = yf + m.offset;
+        switch (m.kind) {
+          case OutputKind::Logits: o.logits = p, o.logits_ld = ld; break;
+          case OutputKind::Probabilities: o.probs = p, o.probs_ld = ld; break;
+          case OutputKind::Classes: o.classes = reinterpret_cast<int*>(p), o.classes_ld = ld; break;
+          case OutputKind::TopKClasses: o.topk_idx = reinterpret_cast<int*>(p), o.topk_idx_ld = ld; break;
+          case OutputKind::TopKProbabilities: o.topk_prob = p, o.topk_prob_ld = ld; break;
+          default: break;
+        }
+      }
+      return launch_classify_head(out, (int)rows, d.head_n, d.head_k, o, st);
     }
+    default: return cudaSuccess;  // a single-output bundle: the last op wrote y
   }
-  return launch_fill_mask_head(logits, d.ops.back().cout, positions, (int)rows, d.head_n, d.mlm_vocab, d.head_k, o, st);
 }
 
 cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, char* y, char* scratch, void* ws,
@@ -710,7 +706,7 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
       stride = (int)d.in_dim;
     }
     // fill-mask bundles: the mask_gather op writes the [MASK] positions here, and the head reads them
-    int* positions = d.mlm_head() ? reinterpret_cast<int*>(scratch + d.mlm_positions_offset(rows)) : nullptr;
+    int* positions = d.head == HeadKind::FillMask ? reinterpret_cast<int*>(scratch + d.mlm_positions_offset(rows)) : nullptr;
     bool after_gather = false;
     for (const GraphOp& o : d.ops) {
       const float* src = (const float*)buf(o.src);
@@ -774,27 +770,15 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
       }
       if (e != cudaSuccess) return e;
     }
-    if (d.mlm_head()) return run_fill_mask_head(d, (const float*)out, positions, rows, y, st);
-    if (d.encoder_head()) {
-      // with a pooler the hidden states are the pooler's source buffer and `out` holds its [rows, H] output; without one
-      // the last op wrote the hidden states to `out`
-      EncoderInputs in;
-      in.ids = ids;
-      in.mask = d.input(InputRole::Mask) ? mask : nullptr;
-      in.stride = stride ? stride : d.ops.front().h;
-      if (d.encoder_pooler) return run_encoder_head(d, (const float*)buf(d.ops.back().src), (const float*)out, in, rows, y, st);
-      return run_encoder_head(d, (const float*)out, nullptr, in, rows, y, st);
-    }
-    if (d.span_head()) {
-      SpanInputs in;
-      in.ids = ids;
-      in.mask = d.input(InputRole::Mask) ? mask : nullptr;
-      in.types = types;
-      in.stride = stride;
-      in.sep_id = d.span_sep_id;
-      return run_span_head(d, (const float*)out, in, rows, y, st);
-    }
-    return d.outputs.empty() ? cudaSuccess : run_head(d, (const float*)out, rows, y, st);
+    SpanInputs in;
+    in.ids = ids;
+    in.mask = d.input(InputRole::Mask) ? mask : nullptr;
+    in.types = types;
+    in.stride = stride;
+    in.sep_id = d.span_sep_id;
+    // with a pooler the hidden states are the pooler's source buffer and `out` holds its [rows, H] output
+    const float* hidden = d.encoder_pooler ? (const float*)buf(d.ops.back().src) : nullptr;
+    return run_head(d, (const float*)out, in, hidden, positions, rows, y, st);
   }
   char* act0 = scratch;
   char* act1 = scratch + d.scratch_bytes(rows) / 2;
@@ -808,7 +792,7 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
     if (e != cudaSuccess) return e;
     in = out;
   }
-  return d.outputs.empty() ? cudaSuccess : run_head(d, (const float*)in, rows, y, st);
+  return run_head(d, (const float*)in, SpanInputs(), nullptr, nullptr, rows, y, st);
 }
 
 size_t Node::row_in_bytes(const ModelDesc& d) { return d.tmpl == Template::Affine ? 4 : (size_t)d.in_dim * 4; }

@@ -5,6 +5,7 @@ dense layer W[in,out] row-major fp32 (the TF dense-kernel layout) then b[out], e
 from __future__ import annotations
 
 import json
+import math
 import os
 
 import numpy as np
@@ -14,17 +15,23 @@ def _align256(x: int) -> int:
     return (x + 255) & ~255
 
 
-OUTPUT_KINDS = ("logits", "probabilities", "classes", "top_k_classes", "top_k_probabilities")
-# question answering (a graph bundle ending in per-token [S, 1, 2] start / end logits, with a type_ids input); the three
-# span kinds carry the same "k" and "max_answer_length" and optionally the same "sep_id"
-SPAN_OUTPUT_KINDS = ("start_logits", "end_logits", "span_starts", "span_ends", "span_scores")
-# embeddings (a graph bundle ending in the last hidden states [S, 1, H], or in the pooler over them); cls_embedding and
-# mean_embedding may carry "normalize": true
-ENCODER_OUTPUT_KINDS = ("sequence_output", "pooled_output", "cls_embedding", "mean_embedding")
-# fill-mask (a graph bundle with a mask_gather op over the [MASK] tokens, ending in [M, 1, Vp] vocabulary logits); the three
-# top-k kinds carry the same "k"
-MLM_OUTPUT_KINDS = ("masked_positions", "masked_top_k_ids", "masked_top_k_probabilities", "masked_top_k_logits")
-_MLM_TOPK = MLM_OUTPUT_KINDS[1:]
+# signature.outputs kinds as the loader's kind table (csrc/model.cc) has them: kind -> (head, dtype, per-row dims in n and
+# k). n is the last op's per-row width (classify), S (span), H (encoder) or the mask_gather op's slots M (fill-mask); k is
+# the entries' "k" (the same on every top-k or span result entry), or S for an encoder. The span result kinds also carry
+# "max_answer_length" and optionally "sep_id" (a graph bundle with a type_ids input, ending in [S, 1, 2] start / end
+# logits); cls_embedding and mean_embedding may carry "normalize": true; classes is one int64 (2 words).
+OUTPUT_KIND_TABLE = {
+    "logits": ("classify", "float32", "n"), "probabilities": ("classify", "float32", "n"), "classes": ("classify", "int64", ""),
+    "top_k_classes": ("classify", "int32", "k"), "top_k_probabilities": ("classify", "float32", "k"),
+    "start_logits": ("span", "float32", "n"), "end_logits": ("span", "float32", "n"), "span_starts": ("span", "int32", "k"),
+    "span_ends": ("span", "int32", "k"), "span_scores": ("span", "float32", "k"),
+    "sequence_output": ("encoder", "float32", "kn"), "pooled_output": ("encoder", "float32", "n"),
+    "cls_embedding": ("encoder", "float32", "n"), "mean_embedding": ("encoder", "float32", "n"),
+    "masked_positions": ("fill_mask", "int32", "n"), "masked_top_k_ids": ("fill_mask", "int32", "nk"),
+    "masked_top_k_probabilities": ("fill_mask", "float32", "nk"), "masked_top_k_logits": ("fill_mask", "float32", "nk"),
+}
+OUTPUT_KINDS, SPAN_OUTPUT_KINDS, ENCODER_OUTPUT_KINDS, MLM_OUTPUT_KINDS = (
+    tuple(k for k, v in OUTPUT_KIND_TABLE.items() if v[0] == head) for head in ("classify", "span", "encoder", "fill_mask"))
 
 
 def _signature(sig: dict, outputs):
@@ -37,36 +44,30 @@ def _signature(sig: dict, outputs):
     return sig
 
 
+def _dims(o, n, seq):
+    head, _dtype, dims = OUTPUT_KIND_TABLE[o["kind"]]
+    return [int(n if d == "n" else seq if head == "encoder" else o.get("k")) for d in dims]
+
+
 def packed_output_layout(outputs, n, seq=None):
     """(name, element offset, width, dtype) of every output in a packed response row, in packed order (byte-wise sorted
-    names). Offsets and widths count 32-bit words: logits / probabilities n floats, classes 2 words (one little-endian
-    int64), top-k k values (int32 classes, float probabilities), start / end logits n floats, span_starts / span_ends k
-    int32, span_scores k floats, sequence_output seq * n floats, pooled_output / cls_embedding / mean_embedding n floats,
-    masked_positions n int32, masked_top_k_ids n * k int32, masked_top_k_probabilities / masked_top_k_logits n * k floats.
-    n = the last op's per-row width for the classification kinds, the sequence length S for the span kinds, the hidden
-    width H for the encoder kinds (seq = S), the mask_gather op's slots M for the fill-mask kinds."""
+    names). Offsets and widths count 32-bit words: a kind's per-row dims (OUTPUT_KIND_TABLE) in n, the entry's "k" and,
+    for the encoder kinds, seq = S; classes is one little-endian int64 in 2 words."""
     out, off = [], 0
     for o in sorted(outputs, key=lambda o: o["name"].encode()):
-        kind = o["kind"]
-        width = {"logits": n, "probabilities": n, "classes": 2, "start_logits": n, "end_logits": n, "pooled_output": n,
-                 "cls_embedding": n, "mean_embedding": n, "masked_positions": n}.get(kind, o.get("k"))
-        if kind == "sequence_output":
-            width = seq * n
-        elif kind in _MLM_TOPK:
-            width = n * o["k"]
-        dtype = {"classes": "int64", "top_k_classes": "int32", "span_starts": "int32", "span_ends": "int32",
-                 "masked_positions": "int32", "masked_top_k_ids": "int32"}.get(kind, "float32")
-        out.append((o["name"], off, int(width), dtype))
-        off += int(width)
+        dtype = OUTPUT_KIND_TABLE[o["kind"]][1]
+        width = math.prod(_dims(o, n, seq)) * (2 if dtype == "int64" else 1)
+        out.append((o["name"], off, width, dtype))
+        off += width
     return out
 
 
 def split_packed_rows(rows_words: np.ndarray, outputs, n, seq=None) -> dict:
     """{name: array} from packed rows ([rows, out_dim] of any 4-byte dtype, e.g. the float32 view of tfsc_predict_device's y).
-    n and seq as for packed_output_layout; sequence_output comes out as [rows, seq, n], the fill-mask top-k kinds as
-    [rows, n, k]."""
+    n and seq as for packed_output_layout; the rank-2 kinds come out as [rows, *dims]: sequence_output [rows, seq, n], the
+    fill-mask top-k kinds [rows, n, k]."""
     w = np.ascontiguousarray(rows_words).view(np.uint32).reshape(len(rows_words), -1)
-    kinds = {o["name"]: o["kind"] for o in outputs}
+    dims = {o["name"]: _dims(o, n, seq) for o in outputs}
     res = {}
     for name, off, width, dtype in packed_output_layout(outputs, n, seq):
         part = np.ascontiguousarray(w[:, off:off + width])
@@ -74,10 +75,8 @@ def split_packed_rows(rows_words: np.ndarray, outputs, n, seq=None) -> dict:
             res[name] = part.view("<i8").reshape(-1)
         else:
             res[name] = part.view("<i4" if dtype == "int32" else "<f4")
-        if kinds[name] == "sequence_output":
-            res[name] = res[name].reshape(len(w), seq, n)
-        elif kinds[name] in _MLM_TOPK:
-            res[name] = res[name].reshape(len(w), n, -1)
+        if len(dims[name]) == 2:
+            res[name] = res[name].reshape(len(w), *dims[name])
     return res
 
 
