@@ -327,7 +327,9 @@ typedef struct tfsc_copy_seg {
 } tfsc_copy_seg;
 int tfsc_k_copy_segments(const tfsc_copy_seg* segs, int n, void* stream);
 
-/* X4/X5 building blocks of the graph executor (conv nets), fp32, row-major / NHWC. act: 0 none, 1 relu, 2 gelu.
+/* X4/X5 building blocks of the graph executor (conv nets), fp32, row-major / NHWC. act: 0 none, 1 relu, 2 gelu, 3 tanh,
+ * 4 relu6 (min(max(x, 0), 6)), 5 silu (x / (1 + exp(-x))), 6 sigmoid (1 / (1 + exp(-x))); the same on tfsc_k_gemm_tc and
+ * tfsc_k_conv_tc.
  * C[M,N] = act(A[M,K] (row stride lda) * B[K,N] + bias[N] (+ R[M,N])); bias / R may be NULL. */
 int tfsc_k_gemm(const float* a, const float* b, const float* bias, const float* r, float* c, int m, int n, int k, int lda,
                 int act, void* stream);
@@ -347,6 +349,17 @@ int tfsc_k_im2col(const float* x, float* col, int batch, int h, int w, int c, in
                   void* stream);
 int tfsc_k_maxpool(const float* x, float* y, int batch, int h, int w, int c, int kh, int kw, int stride, int pad, void* stream);
 int tfsc_k_avgpool(const float* x, float* y, int batch, int hw, int c, void* stream);
+/* MobileNet / EfficientNet building blocks (fp32, device, NHWC). Depthwise convolution: y[b, oy, ox, ch] = act(sum_i sum_j
+ * x[b, oy*stride - pad + i, ox*stride - pad + j, ch] * w[i, j, ch] + bias[ch]) with zero padding, OH = (h + 2 pad - kh) /
+ * stride + 1 (OW likewise), w [kh, kw, c] (TF's [kh, kw, c, 1] depthwise layout), bias [c]. act: 0 none, 1 relu, 4 relu6,
+ * 5 silu, 6 sigmoid. The taps are summed in the same order at every batch size and alignment, so a row's bits depend on
+ * neither. TFSC_E_INVALID unless kh, kw in 1..7, stride in 1..2, pad <= kh / 2 and kw / 2, h * w * c < 2^31, and every
+ * pointer is given. */
+int tfsc_k_depthwise_conv(const float* x, const float* w, const float* bias, float* y, int batch, int h, int wd, int c, int kh, int kw,
+                          int stride, int pad, int act, void* stream);
+/* Squeeze-and-excitation gate: y[b, p, ch] = x[b, p, ch] * gate[b, ch] over hw positions p. TFSC_E_INVALID unless
+ * hw * c < 2^31. */
+int tfsc_k_channel_scale(const float* x, const float* gate, float* y, int batch, int hw, int c, void* stream);
 /* X5 building blocks of the transformer graphs. Multi-head self-attention: qkv[batch, seq, 3*hidden] (q | k | v of every
  * token), ctx[batch, seq, hidden]; head width d = hidden / heads, scores scaled by 1/sqrt(d). ids[batch, seq] may be NULL;
  * a key whose id is 0 ([PAD]) gets the additive mask -10000 unless every key of its sequence is [PAD]. Every seq runs for

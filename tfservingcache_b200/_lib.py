@@ -135,6 +135,8 @@ _sig("tfsc_k_conv_tc", C.c_int, vp, vp, vp, vp, vp, *([C.c_int] * 10), vp)
 _sig("tfsc_k_im2col", C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp)
 _sig("tfsc_k_maxpool", C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp)
 _sig("tfsc_k_avgpool", C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, vp)
+_sig("tfsc_k_depthwise_conv", C.c_int, vp, vp, vp, vp, *([C.c_int] * 9), vp)
+_sig("tfsc_k_channel_scale", C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp)
 _sig("tfsc_k_attention", C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp)
 _sig("tfsc_k_attention_mask", C.c_int, vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp)
 _sig("tfsc_k_embed", C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp)

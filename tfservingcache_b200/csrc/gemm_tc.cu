@@ -16,7 +16,7 @@
 //     have separate accumulators (the tensor core's fp32 accumulate truncates).
 //   * two consumer warpgroups: for BN = 128 each owns 64 columns x 128 rows (wgmma N = 128), for BN = 64 each owns the 64
 //     columns x 64 rows. The epilogue parks the tile in shared memory and stores it row-contiguous with bias (+ residual)
-//     and ReLU / GELU(erf) / tanh.
+//     and ReLU / GELU(erf) / tanh / ReLU6 / SiLU / sigmoid.
 // One CTA per 128 x BN output tile; small grids (late ResNet stages: M = 392, K = 4608; BERT's K = 3072 projection) split K
 // over a thread-block cluster of 2 / 4 / 8 CTAs along grid.z: every CTA parks its partial tile in its own shared memory
 // and each CTA folds 128/S rows of the tile over distributed shared memory in fixed rank order (deterministic), then
@@ -31,6 +31,7 @@
 #include <mutex>
 #include <unordered_map>
 
+#include "act.cuh"
 #include "kernels.h"
 #include "tc_ptx.cuh"
 
@@ -77,13 +78,19 @@ __device__ __forceinline__ void tma_load_im2col_4d(void* dst, const CUtensorMap*
 }
 
 __device__ __forceinline__ float gelu_erf_tc(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752440f)); }
-// run-time activation with REAL branches (noinline bodies cannot be if-converted into the caller's store loop)
-__device__ __noinline__ float4 act_gelu4(float4 v) { return make_float4(gelu_erf_tc(v.x), gelu_erf_tc(v.y), gelu_erf_tc(v.z), gelu_erf_tc(v.w)); }
-__device__ __noinline__ float4 act_tanh4(float4 v) { return make_float4(tanhf(v.x), tanhf(v.y), tanhf(v.z), tanhf(v.w)); }
+// run-time activation with REAL branches (a noinline body cannot be if-converted into the caller's store loop); every
+// activation but ReLU shares one call site, so the store loop of act 0 / 1 carries a single extra compare
+__device__ __noinline__ float4 act_call4(float4 v, int act) {
+  if (act == 2) return make_float4(gelu_erf_tc(v.x), gelu_erf_tc(v.y), gelu_erf_tc(v.z), gelu_erf_tc(v.w));
+  if (act == 3) return make_float4(tanhf(v.x), tanhf(v.y), tanhf(v.z), tanhf(v.w));
+  if (act == 4) return make_float4(relu6f(v.x), relu6f(v.y), relu6f(v.z), relu6f(v.w));
+  if (act == 5) return make_float4(siluf(v.x), siluf(v.y), siluf(v.z), siluf(v.w));
+  if (act == 6) return make_float4(sigmoidf(v.x), sigmoidf(v.y), sigmoidf(v.z), sigmoidf(v.w));
+  return v;
+}
 __device__ __forceinline__ float4 apply_act_rt(float4 v, int act) {
   if (act == 1) return make_float4(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f), fmaxf(v.z, 0.f), fmaxf(v.w, 0.f));
-  if (act == 2) return act_gelu4(v);
-  if (act == 3) return act_tanh4(v);
+  if (act >= 2) return act_call4(v, act);
   return v;
 }
 template <int BN, bool IM2COL>

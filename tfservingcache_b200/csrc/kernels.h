@@ -38,7 +38,7 @@ cudaError_t launch_dense_cluster(const float* x, const float* w, const float* bi
 // grid of the cluster kernel on the current device: co-resident 2-CTA clusters and the strip width chosen for n columns
 cudaError_t dense_cluster_grid(int rows, int n, int* active_clusters, int* strip_cols);
 
-// X4/X5 building blocks (nn_kernels.cu): act 0 none / 1 relu / 2 gelu(erf)
+// X4/X5 building blocks (nn_kernels.cu): act 0 none / 1 relu / 2 gelu(erf) / 3 tanh / 4 relu6 / 5 silu / 6 sigmoid
 cudaError_t launch_gemm(const float* A, const float* B, const float* bias, const float* R, float* C, int M, int N, int K,
                         int lda, int act, cudaStream_t s);
 cudaError_t launch_im2col(const float* x, float* col, int Bn, int H, int W, int C, int KH, int KW, int stride, int pad,
@@ -46,6 +46,13 @@ cudaError_t launch_im2col(const float* x, float* col, int Bn, int H, int W, int 
 cudaError_t launch_maxpool(const float* x, float* y, int Bn, int H, int W, int C, int KH, int KW, int stride, int pad, int OH,
                            int OW, cudaStream_t s);
 cudaError_t launch_avgpool(const float* x, float* y, int Bn, int HW, int C, cudaStream_t s);
+// MobileNet / EfficientNet blocks (depthwise.cu). y[b, oy, ox, ch] = act(sum_ij x[b, oy*stride - pad + i, ox*stride - pad +
+// j, ch] * w[i, j, ch] + bias[ch]), w [KH, KW, C], act 0 none / 1 relu / 4 relu6 / 5 silu / 6 sigmoid; cudaErrorInvalidValue
+// outside depthwise_supported (nn_limits.h), for another act or a null pointer.
+cudaError_t launch_depthwise_conv(const float* x, const float* w, const float* bias, float* y, int Bn, int H, int W, int C, int KH,
+                                  int KW, int stride, int pad, int act, cudaStream_t s);
+// y[b, p, ch] = x[b, p, ch] * gate[b, ch] over HW positions p (the squeeze-and-excitation gate)
+cudaError_t launch_channel_scale(const float* x, const float* gate, float* y, int Bn, int HW, int C, cudaStream_t s);
 // y = LayerNorm(x (+res)) or, with ids != nullptr, LayerNorm(word[id] + pos[s] + type[t]) (BERT embeddings): token
 // b*S + s reads ids[b*stride + s] and, unless types is nullptr (segment 0), t = clamp(types[b*stride + s], 0, 1)
 cudaError_t launch_layernorm(const float* x, const float* res, const int* ids, const int* types, int stride, const float* word,

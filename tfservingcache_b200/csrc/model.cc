@@ -628,6 +628,8 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       else if (kind == "layernorm") o.kind = OpKind::LayerNorm;
       else if (kind == "attention") o.kind = OpKind::Attention;
       else if (kind == "mask_gather") o.kind = OpKind::MaskGather;
+      else if (kind == "depthwise_conv") o.kind = OpKind::DepthwiseConv;
+      else if (kind == "channel_scale") o.kind = OpKind::ChannelScale;
       else {
         *err = "graph manifest: unknown op '" + kind + "'";
         return false;
@@ -644,7 +646,16 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       o.pad = (int)oj.get_int("pad", 0);
       o.cout = (int)oj.get_int("cout", o.c);
       const std::string act = oj.get_str("act", "none");
-      o.act = act == "relu" ? 1 : act == "gelu" ? 2 : act == "tanh" ? 3 : 0;
+      o.act = act == "relu" ? 1 : act == "gelu" ? 2 : act == "tanh" ? 3 : act == "relu6" ? 4 : act == "silu" ? 5 : act == "sigmoid" ? 6 : 0;
+      // the older ops read an unknown act string as none; the depthwise and gate ops refuse it
+      if (o.kind == OpKind::DepthwiseConv && !(act == "none" || o.act == 1 || o.act >= 4)) {
+        *err = "graph manifest: depthwise_conv act '" + act + "' is not none, relu, relu6, silu or sigmoid";
+        return false;
+      }
+      if (o.kind == OpKind::ChannelScale && act != "none") {
+        *err = "graph manifest: channel_scale takes no activation (act '" + act + "')";
+        return false;
+      }
       o.heads = (int)oj.get_int("heads", 1);
       o.vocab = (int)oj.get_int("vocab", 0);
       o.max_pos = (int)oj.get_int("max_pos", 0);
@@ -698,6 +709,33 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       } else if (o.kind == OpKind::AvgPool) {
         o.oh = o.ow = 1;
         o.cout = o.c;
+      } else if (o.kind == OpKind::ChannelScale) {
+        o.oh = o.h;
+        o.ow = o.w;
+        o.cout = o.c;
+        o.gate = (int)oj.get_int("gate", -100);
+        if (o.res != -100) {
+          *err = "graph manifest: channel_scale takes no residual input";
+          return false;
+        }
+      } else if (o.kind == OpKind::DepthwiseConv) {
+        if (o.cout != o.c) {
+          *err = "graph manifest: depthwise_conv writes its c = " + std::to_string(o.c) + " channels (cout " + std::to_string(o.cout) + ")";
+          return false;
+        }
+        if (o.res != -100) {
+          *err = "graph manifest: depthwise_conv takes no residual input";
+          return false;
+        }
+        if (!depthwise_supported(o.h, o.w, o.c, o.kh, o.kw, o.stride, o.pad)) {
+          *err = "graph manifest: no depthwise_conv kernel for " + std::to_string(o.h) + " x " + std::to_string(o.w) + " x " +
+                 std::to_string(o.c) + ", kernel " + std::to_string(o.kh) + " x " + std::to_string(o.kw) + ", stride " +
+                 std::to_string(o.stride) + ", pad " + std::to_string(o.pad) + " (kernel <= " + std::to_string(kDepthwiseMaxK) +
+                 ", stride <= " + std::to_string(kDepthwiseMaxStride) + ", pad <= kernel / 2, h * w * c < 2^31)";
+          return false;
+        }
+        o.oh = (o.h + 2 * o.pad - o.kh) / o.stride + 1;
+        o.ow = (o.w + 2 * o.pad - o.kw) / o.stride + 1;
       } else if (o.kind == OpKind::Dense) {
         o.oh = o.ow = 1;
         o.kh = o.kw = 1;
@@ -716,6 +754,22 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       }
       const int64_t have = o.src == -1 ? in_elems : written[o.src];
       o.lda = have;
+      if (o.kind == OpKind::ChannelScale) {
+        if (o.gate == o.dst) {
+          *err = "graph manifest: channel_scale cannot write its gate buffer (gate == dst == " + std::to_string(o.dst) + ")";
+          return false;
+        }
+        if (o.gate < 0 || o.gate >= d->n_buffers || written[o.gate] != o.c) {
+          *err = "graph manifest: channel_scale needs a gate that an earlier op wrote to a scratch buffer with c = " +
+                 std::to_string(o.c) + " values per image (gate " + std::to_string(o.gate) + ")";
+          return false;
+        }
+        if (have != in_e) {
+          *err = "graph manifest: channel_scale reads " + std::to_string(have) + " values per image, not h * w * c = " +
+                 std::to_string(in_e);
+          return false;
+        }
+      }
       const bool size_ok = o.kind == OpKind::Dense ? have >= in_e : have == in_e;  // Dense may read the first token only
       if (o.kind == OpKind::Embed && (o.src != -1 || o.vocab < 1 || o.max_pos < o.h || (o.word_off & 255) || (o.pos_off & 255) ||
                                       (o.type_off & 255) || o.word_off + (size_t)o.vocab * o.c * 4 > d->weights_bytes ||
@@ -733,14 +787,14 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         *err = "graph manifest: op input size does not match its producer";
         return false;
       }
-      if (o.kind == OpKind::Conv || o.kind == OpKind::Dense) {
-        const size_t wbytes = (size_t)o.kh * o.kw * o.c * o.cout * 4;
+      if (o.kind == OpKind::Conv || o.kind == OpKind::Dense || o.kind == OpKind::DepthwiseConv) {
+        const size_t wbytes = (size_t)o.kh * o.kw * o.c * (o.kind == OpKind::DepthwiseConv ? 1 : o.cout) * 4;
         if ((o.w_off & 255) || (o.b_off & 255) || o.w_off + wbytes > d->weights_bytes || o.b_off + (size_t)o.cout * 4 > d->weights_bytes) {
           *err = "graph manifest: weights out of range or misaligned";
           return false;
         }
         const bool direct = o.kh == 1 && o.kw == 1 && o.stride == 1 && o.pad == 0;
-        if (!direct) {
+        if (!direct && o.kind != OpKind::DepthwiseConv) {
           const int64_t ldc = ((int64_t)o.kh * o.kw * o.c + 3) / 4 * 4;
           d->col_elems = std::max<int64_t>(d->col_elems, (int64_t)o.oh * o.ow * ldc);
         }

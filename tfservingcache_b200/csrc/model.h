@@ -20,13 +20,17 @@ enum class Template { Affine, Mlp, Graph };
 // MaskGather (fill-mask bundles): from the [S, 1, H] hidden states in `src`, copies those of the first `slots` = M tokens
 // whose id is mask_token_id (and whose mask is set, with a mask input) to dst [M, 1, H], ascending position, zeros for
 // empty slots, and writes their positions (int32 [M], -1 empty) to the executor's positions scratch for the head.
-enum class OpKind { Conv, MaxPool, AvgPool, Dense, Embed, LayerNorm, Attention, MaskGather };
+// DepthwiseConv (MobileNet / EfficientNet): one kh x kw filter per channel, kernel [kh, kw, c] (TF's [kh, kw, c, 1]) at
+// w_off, bias [c] at b_off, cout = c. ChannelScale (squeeze-and-excitation): dst[b, p, ch] = src[b, p, ch] * gate[b, ch],
+// where `gate` is a scratch buffer an earlier op wrote with c values per image.
+enum class OpKind { Conv, MaxPool, AvgPool, Dense, Embed, LayerNorm, Attention, MaskGather, DepthwiseConv, ChannelScale };
 struct GraphOp {
   OpKind kind = OpKind::Conv;
   int src = -1, dst = 0, res = -100;  // res = -100: no residual input
+  int gate = -100;                    // ChannelScale: the buffer holding the [c] gate of each image
   int h = 1, w = 1, c = 1;            // input H, W, C per image
   int kh = 1, kw = 1, stride = 1, pad = 0, cout = 1, oh = 1, ow = 1;
-  int act = 0;                        // 0 none, 1 relu, 2 gelu(erf), 3 tanh
+  int act = 0;                        // 0 none, 1 relu, 2 gelu(erf), 3 tanh, 4 relu6, 5 silu, 6 sigmoid
   size_t w_off = 0, b_off = 0;        // kernel / bias; LayerNorm + Embed: gamma / beta
   // transformer ops (a "image" is a sequence: h = S tokens, w = 1, c = hidden width)
   int heads = 1, vocab = 0, max_pos = 0;

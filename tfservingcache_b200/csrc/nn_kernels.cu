@@ -11,6 +11,7 @@
 #include <cfloat>
 #include <cstdlib>
 
+#include "act.cuh"
 #include "kernels.h"
 
 namespace tfsc {
@@ -128,6 +129,9 @@ gemm_f32_kernel(const float* __restrict__ A, const float* __restrict__ B, const 
       if (act == 1) v = fmaxf(v, 0.f);
       else if (act == 2) v = gelu_erf(v);
       else if (act == 3) v = tanhf(v);
+      else if (act == 4) v = relu6f(v);
+      else if (act == 5) v = siluf(v);
+      else if (act == 6) v = sigmoidf(v);
       C[(size_t)gm * N + gn] = v;
     }
   }

@@ -55,4 +55,14 @@ inline bool fill_mask_supported(int M, int vocab, int k) {
   return M >= 1 && M <= kMaskGatherMaxS && vocab >= 1 && vocab <= kHeadMaxN && k >= 1 && k <= kHeadMaxK && k <= vocab;
 }
 
+// Depthwise convolution (depthwise.cu): a thread runs the kh x kw taps of one output pixel for 4 channels (1 on the scalar
+// path). Kernels up to 7 x 7, stride 1 or 2 and padding up to k / 2 cover MobileNetV2 and EfficientNet B0-B7 (3 x 3 and
+// 5 x 5, stride <= 2) with margin; offsets within an image are 32-bit (H * W * C < 2^31).
+constexpr int kDepthwiseMaxK = 7, kDepthwiseMaxStride = 2;
+inline bool depthwise_supported(int H, int W, int C, int KH, int KW, int stride, int pad) {
+  return H >= 1 && W >= 1 && C >= 1 && KH >= 1 && KH <= kDepthwiseMaxK && KW >= 1 && KW <= kDepthwiseMaxK && stride >= 1 &&
+         stride <= kDepthwiseMaxStride && pad >= 0 && pad <= KH / 2 && pad <= KW / 2 && H + 2 * pad >= KH && W + 2 * pad >= KW &&
+         (long long)H * W * C <= 0x7fffffffLL;
+}
+
 }  // namespace tfsc

@@ -765,6 +765,11 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
         e = launch_mask_gather(src, ids, d.input(InputRole::Mask) ? mask : nullptr, stride ? stride : o.h, B, o.h, o.c, o.oh,
                                o.mask_token_id, positions, dst, st);
         after_gather = true;
+      } else if (o.kind == OpKind::DepthwiseConv) {
+        e = launch_depthwise_conv(src, (const float*)(dm.dptr + o.w_off), (const float*)(dm.dptr + o.b_off), dst, B, o.h, o.w, o.c,
+                                  o.kh, o.kw, o.stride, o.pad, o.act, st);
+      } else if (o.kind == OpKind::ChannelScale) {
+        e = launch_channel_scale(src, (const float*)buf(o.gate), dst, B, o.h * o.w, o.c, st);
       } else {
         e = launch_avgpool(src, dst, B, o.h * o.w, o.c, st);
       }

@@ -281,6 +281,10 @@ std::shared_ptr<HostModel> SyntheticModelProvider::load_model(const std::string&
         const uint64_t fan_in = (uint64_t)o.kh * o.kw * o.c;
         fill(base + o.w_off / 4, seed, t0, fan_in * o.cout, (float)std::sqrt(3.0 / (double)fan_in), threads_);
         fill(base + o.b_off / 4, seed, t0 + 1, (uint64_t)o.cout, 0.1f, 1);
+      } else if (o.kind == OpKind::DepthwiseConv) {  // one kh x kw filter per channel: fan-in kh * kw
+        const uint64_t fan_in = (uint64_t)o.kh * o.kw;
+        fill(base + o.w_off / 4, seed, t0, fan_in * o.c, (float)std::sqrt(3.0 / (double)fan_in), threads_);
+        fill(base + o.b_off / 4, seed, t0 + 1, (uint64_t)o.c, 0.1f, 1);
       } else if (o.kind == OpKind::LayerNorm || o.kind == OpKind::Embed) {
         float* g = base + o.w_off / 4;
         fill(g, seed, t0, (uint64_t)o.c, 0.1f, 1);

@@ -1805,6 +1805,25 @@ int tfsc_k_avgpool(const float* x, float* y, int batch, int hw, int c, void* str
   cudaError_t e = launch_avgpool(x, y, batch, hw, c, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "avgpool: %s", cudaGetErrorString(e));
 }
+int tfsc_k_depthwise_conv(const float* x, const float* w, const float* bias, float* y, int batch, int h, int wd, int c, int kh, int kw,
+                          int stride, int pad, int act, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (!x || !w || !bias || !y || batch < 0 || !depthwise_supported(h, wd, c, kh, kw, stride, pad))
+    return fail(TFSC_E_INVALID, "depthwise_conv: no kernel for batch %d, %d x %d x %d, kernel %d x %d, stride %d, pad %d (kernel <= %d, "
+                "stride <= %d, pad <= kernel / 2, h * w * c < 2^31)", batch, h, wd, c, kh, kw, stride, pad, kDepthwiseMaxK,
+                kDepthwiseMaxStride);
+  if (!(act == 0 || act == 1 || (act >= 4 && act <= 6)))
+    return fail(TFSC_E_INVALID, "depthwise_conv: act %d is not 0 none, 1 relu, 4 relu6, 5 silu or 6 sigmoid", act);
+  cudaError_t e = launch_depthwise_conv(x, w, bias, y, batch, h, wd, c, kh, kw, stride, pad, act, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "depthwise_conv: %s", cudaGetErrorString(e));
+}
+int tfsc_k_channel_scale(const float* x, const float* gate, float* y, int batch, int hw, int c, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (!x || !gate || !y || batch < 0 || hw < 1 || c < 1 || (int64_t)hw * c > 0x7fffffff)
+    return fail(TFSC_E_INVALID, "channel_scale: no kernel for batch %d, hw %d, c %d (hw * c < 2^31)", batch, hw, c);
+  cudaError_t e = launch_channel_scale(x, gate, y, batch, hw, c, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "channel_scale: %s", cudaGetErrorString(e));
+}
 int tfsc_k_attention(const float* qkv, const int* ids, float* ctx, int batch, int seq, int hidden, int heads, void* stream) {
   if (int rc = check_device()) return rc;
   const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;

@@ -138,6 +138,9 @@ def _graph_manifest(input_shape, ops, n_buffers, input_name="x", output_name="y"
             k = op.get("kh", 1) * op.get("kw", 1) * op["c"]
             op["w_offset"] = take(k * op["cout"] * 4)
             op["b_offset"] = take(op["cout"] * 4)
+        elif op["op"] == "depthwise_conv":                  # kernel [kh, kw, c], bias [c]
+            op["w_offset"] = take(op["kh"] * op["kw"] * op["c"] * 4)
+            op["b_offset"] = take(op["c"] * 4)
         elif op["op"] in ("layernorm", "embed"):
             op["w_offset"] = take(op["c"] * 4)      # gamma
             op["b_offset"] = take(op["c"] * 4)      # beta
@@ -187,6 +190,90 @@ def resnet50_manifest(image=224, classes=1000, width=64, blocks=(3, 4, 6, 3), ou
     ops.append({"op": "avgpool", "src": cur, "dst": a, "h": h, "w": h, "c": cin})
     ops.append({"op": "dense", "src": a, "dst": -2, "h": 1, "w": 1, "c": cin, "cout": classes, "act": "none"})
     return _graph_manifest([image, image, 3], ops, 5, outputs=outputs)
+
+
+def _make_divisible(v: float, divisor: int = 8) -> int:
+    """torchvision's channel rounding: the nearest multiple of `divisor`, at least `divisor`, never 10 % below v."""
+    new_v = max(divisor, int(v + divisor / 2) // divisor * divisor)
+    return new_v + divisor if new_v < 0.9 * v else new_v
+
+
+def _conv(src, dst, h, c, cout, k=1, stride=1, act="none", res=None):
+    o = {"op": "conv", "src": src, "dst": dst, "h": h, "w": h, "c": c, "kh": k, "kw": k, "stride": stride, "pad": (k - 1) // 2,
+         "cout": cout, "act": act}
+    if res is not None:
+        o["res"] = res
+    return o
+
+
+def _depthwise(src, dst, h, c, k, stride, act):
+    return {"op": "depthwise_conv", "src": src, "dst": dst, "h": h, "w": h, "c": c, "kh": k, "kw": k, "stride": stride,
+            "pad": (k - 1) // 2, "act": act}
+
+
+def _classifier(ops, cur, h, cin, last, classes, act, n_buffers, image, outputs):
+    """the 1x1 conv to `last` channels, global average pool and the dense classifier that end both image nets"""
+    a, b = [x for x in range(n_buffers) if x != cur][:2]
+    ops.append(_conv(cur, a, h, cin, last, act=act))
+    ops.append({"op": "avgpool", "src": a, "dst": b, "h": h, "w": h, "c": last})
+    ops.append({"op": "dense", "src": b, "dst": -2, "h": 1, "w": 1, "c": last, "cout": classes, "act": "none"})
+    return _graph_manifest([image, image, 3], ops, n_buffers, outputs=outputs)
+
+
+def mobilenet_v2_manifest(image=224, classes=1000, width_mult=1.0, outputs=None):
+    """MobileNetV2 (Sandler et al. 2018; torchvision topology, symmetric padding) as a graph bundle, NHWC, BatchNorm folded
+    into kernel + bias, ReLU6 after every conv but the projections. An inverted-residual block is a 1x1 expansion (absent at
+    expansion 1), a 3x3 depthwise conv and a 1x1 projection with the block input as residual when the shape allows.
+    Dropout is identity at inference. Buffers: the block input and three others. outputs as for resnet50_manifest."""
+    setting = [(1, 16, 1, 1), (6, 24, 2, 2), (6, 32, 3, 2), (6, 64, 4, 2), (6, 96, 3, 1), (6, 160, 3, 2), (6, 320, 1, 1)]
+    cin = _make_divisible(32 * width_mult)
+    ops, h, cur = [_conv(-1, 0, image, 3, cin, k=3, stride=2, act="relu6")], (image - 1) // 2 + 1, 0
+    for t, c, n, s in setting:
+        cout = _make_divisible(c * width_mult)
+        for i in range(n):
+            stride, hidden = (s if i == 0 else 1), int(round(cin * t))
+            a, b, d = [x for x in range(4) if x != cur]
+            src = cur
+            if t != 1:
+                ops.append(_conv(cur, a, h, cin, hidden, act="relu6"))
+                src = a
+            ho = (h - 1) // stride + 1
+            ops.append(_depthwise(src, b, h, hidden, 3, stride, "relu6"))
+            ops.append(_conv(b, d, ho, hidden, cout, res=cur if stride == 1 and cin == cout else None))
+            cur, cin, h = d, cout, ho
+    return _classifier(ops, cur, h, cin, _make_divisible(1280 * max(1.0, width_mult)), classes, "relu6", 4, image, outputs)
+
+
+def efficientnet_manifest(image=224, classes=1000, width_mult=1.0, depth_mult=1.0, outputs=None):
+    """EfficientNet (Tan & Le 2019; torchvision topology, symmetric padding) as a graph bundle, NHWC, BatchNorm folded into
+    kernel + bias, SiLU activations. The default multipliers give B0; torchvision's (width_mult, depth_mult) of B1-B7 give
+    those topologies (image size is the caller's). An MBConv block is a 1x1 expansion (absent at expansion 1), a k x k
+    depthwise conv, squeeze-and-excitation (global average pool, a 1x1 conv to max(1, block input / 4) channels with SiLU, a
+    1x1 conv back with sigmoid, channel_scale by that gate) and a 1x1 projection with the block input as residual when the
+    shape allows. Stochastic depth and dropout are identity at inference. Buffers: the block input and three others, the SE
+    pool / gate in the one the projection writes. outputs as for resnet50_manifest."""
+    setting = [(1, 3, 1, 32, 16, 1), (6, 3, 2, 16, 24, 2), (6, 5, 2, 24, 40, 2), (6, 3, 2, 40, 80, 3), (6, 5, 1, 80, 112, 3),
+               (6, 5, 2, 112, 192, 4), (6, 3, 1, 192, 320, 1)]
+    cin = _make_divisible(32 * width_mult)
+    ops, h, cur = [_conv(-1, 0, image, 3, cin, k=3, stride=2, act="silu")], (image - 1) // 2 + 1, 0
+    for e, k, s, _ci, co, n in setting:
+        cout = _make_divisible(co * width_mult)
+        for i in range(int(math.ceil(n * depth_mult))):
+            stride, exp, sq = (s if i == 0 else 1), _make_divisible(cin * e), max(1, cin // 4)
+            a, b, d = [x for x in range(4) if x != cur]
+            src = cur
+            if exp != cin:
+                ops.append(_conv(cur, a, h, cin, exp, act="silu"))
+                src = a
+            ho = (h - 1) // stride + 1
+            ops.append(_depthwise(src, b, h, exp, k, stride, "silu"))
+            ops.append({"op": "avgpool", "src": b, "dst": d, "h": ho, "w": ho, "c": exp})
+            ops.append(_conv(d, a, 1, exp, sq, act="silu"))
+            ops.append(_conv(a, d, 1, sq, exp, act="sigmoid"))
+            ops.append({"op": "channel_scale", "src": b, "gate": d, "dst": a, "h": ho, "w": ho, "c": exp})
+            ops.append(_conv(a, d, ho, exp, cout, res=cur if stride == 1 and cin == cout else None))
+            cur, cin, h = d, cout, ho
+    return _classifier(ops, cur, h, cin, 4 * cin, classes, "silu", 4, image, outputs)
 
 
 def write_graph_bundle(version_dir: str, manifest: dict, blob: np.ndarray):
