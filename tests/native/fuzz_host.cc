@@ -70,6 +70,37 @@ int main(int argc, char** argv) {
     const float* d; int64_t n; std::vector<float> sc;
     if (!tensor_f32(v.inputs[0], &d, &n, &sc, &err) || n != 4) { fprintf(stderr, "good tensor failed\n"); return 1; }
   }
+  {  // a response frame around its float payload is byte for byte what the encoders write for the same DT_FLOAT tensor
+    const std::vector<std::vector<int64_t>> shapes = {{3}, {2, 4}, {0}, {}, {5, 40}};
+    for (auto& shape : shapes)
+      for (int64_t version : {(int64_t)0, (int64_t)123456789})
+        for (const char* sig : {"", "serving_default"})
+          for (const char* name : {"", "y:0"}) {
+            int64_t n = 1;
+            for (auto dim : shape) n *= dim;
+            std::vector<float> vals((size_t)n + 1);
+            for (int64_t k = 0; k < n; ++k) vals[k] = 0.25f * (float)k - 1.f;
+            const std::string payload(reinterpret_cast<const char*>(vals.data()), (size_t)n * 4);
+            OutTensor t;
+            t.name = name;
+            t.shape = shape;
+            t.data = vals.data();
+            t.n = n;
+            std::string prefix, suffix;
+            predict_response_frame("half_plus_two", version, sig, name, shape, &prefix, &suffix);
+            if (prefix + payload + suffix != encode_predict_response("half_plus_two", version, sig, {t})) {
+              fprintf(stderr, "predict_response_frame differs from encode_predict_response (rank %zu, version %lld, sig '%s', name '%s')\n",
+                      shape.size(), (long long)version, sig, name);
+              return 1;
+            }
+            session_run_response_frame("half_plus_two", version, sig, name, shape, &prefix, &suffix);
+            if (prefix + payload + suffix != encode_session_run_response("half_plus_two", version, sig, t)) {
+              fprintf(stderr, "session_run_response_frame differs from encode_session_run_response (rank %zu, version %lld, sig '%s', name '%s')\n",
+                      shape.size(), (long long)version, sig, name);
+              return 1;
+            }
+          }
+  }
   const std::string good_json = "{\"instances\": [[1.0, 2.5e3, -3], [4, 5, 6]], \"signature_name\": \"serving_default\", \"x\": {\"a\": [true, null, \"s\\u00e9\"]}}";
   const std::string good_manifest = "{\"format\":\"tfsc-b200-v1\",\"template\":\"mlp\",\"dtype\":\"float32\",\"weights_bytes\":1280,\"layers\":[{\"in\":8,\"out\":16,\"activation\":\"relu\",\"w_offset\":0,\"b_offset\":512},{\"in\":16,\"out\":4,\"activation\":\"linear\",\"w_offset\":768,\"b_offset\":1024}]}";
   long decoded = 0, jsons = 0, manifests = 0;

@@ -243,7 +243,7 @@ int tfsc_route(tfsc_server* s, const char* model_name, const char* version, int*
   return rc;
 }
 
-static int check_device_early() {
+static int check_device() {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
     cudaGetLastError();
@@ -374,57 +374,19 @@ static int abi_inputs(const tfsc_tensor* in, int n_in, bool need_data, std::vect
   return 0;
 }
 
-// Output shape of a request with input shape `in_shape` that the executor will run as `rows` rows. Returns false (with
-// a message) unless the shape accounts for exactly the rows * out_per_row elements the executor writes: the client's
-// tensor_shape must never be the only thing that sizes a response buffer (e.g. [1, 2*in_dim] is two rows, not one).
-static bool out_shape(const ModelDesc& d, int64_t rows, const std::vector<int64_t>& in_shape, std::vector<int64_t>* shape,
-                      std::string* why) {
-  shape->clear();
-  int64_t per_row = 1;
-  if (d.tmpl == Template::Affine) {
-    *shape = in_shape;
-  } else if (d.tmpl == Template::Graph) {
-    // [B, H, W, C] -> [B, classes]: batch dims are whatever precedes the per-image input shape
-    if (in_shape.size() > d.input_shape.size())
-      for (size_t i = 0; i + d.input_shape.size() < in_shape.size(); ++i) shape->push_back(in_shape[i]);
-    for (auto v : d.output_shape) shape->push_back(v);
-    per_row = d.out_dim;
-  } else {
-    // leading dims of the input are kept ([B, in] -> [B, out]; [in] -> [out])
-    if (in_shape.size() <= 1) {
-      if (rows != 1 || in_shape.empty()) shape->push_back(rows);
-    } else {
-      for (size_t i = 0; i + 1 < in_shape.size(); ++i) shape->push_back(in_shape[i]);
-    }
-    shape->push_back(d.out_dim);
-    per_row = d.out_dim;
-  }
-  int64_t on = 1;
-  for (auto v : *shape) {
-    if (v < 0 || (v != 0 && on > ((int64_t)1 << 40) / v)) {
-      on = -1;
-      break;
-    }
-    on *= v;
-  }
-  if (on != rows * per_row) {
-    std::string sh = "[";
-    for (size_t i = 0; i < in_shape.size(); ++i) sh += (i ? "," : "") + std::to_string(in_shape[i]);
-    *why = "input shape " + sh + "] does not match the model signature: the trailing dimensions must hold exactly " +
-           std::to_string(d.tmpl == Template::Affine ? 1 : d.in_dim) + " elements per row";
-    return false;
-  }
-  return true;
-}
+// ---- Predict responses: the executor writes packed rows (model.h; a single-output model's row is its one output), and
+// every front-end answers the outputs of one plan with the same rule, for local and forwarded requests alike.
 
-// ---- multi-output models (signature.outputs): the executor writes packed rows (model.h); every front-end cuts the
-// outputs it serves out of them with the same rule, for local and forwarded requests alike.
-
-// The selected outputs of one response, in the order they are answered, with their full shapes (batch dims + per row).
+// The selected outputs of one response, in the order they are answered, with their dtypes and full shapes (batch dims +
+// per row). A model without signature.outputs answers one float output, d.output_name.
 struct OutputPlan {
   std::vector<ModelOutput> sel;
+  std::vector<int> dtypes;
   std::vector<std::vector<int64_t>> shapes;
-  int64_t out_dim = 0, rows = 0;
+  int64_t out_dim = 0, rows = 0;  // out_dim: words per packed row
+  bool declared = false;          // the model declares signature.outputs
+  // the packed rows are exactly the one output's values, so the executor can write them into the final buffer
+  bool whole_row() const { return sel.size() == 1 && sel[0].offset == 0 && sel[0].width == out_dim; }
 };
 
 static int64_t product(const std::vector<int64_t>& v) {
@@ -433,12 +395,17 @@ static int64_t product(const std::vector<int64_t>& v) {
   return n;
 }
 
-// The batch dims of a request with input shape `in_shape` that runs as `rows` rows, by the rule out_shape applies to a
-// single output: a graph keeps what precedes the per-image input shape, an mlp the leading dims of the input.
+// The batch dims of a request with input shape `in_shape` that the executor will run as `rows` rows: an affine model
+// answers in the input's shape, a graph keeps what precedes the per-image input shape ([B, H, W, C] -> [B, ...]), an mlp
+// the leading dims of the input ([B, in] -> [B, out]; [in] -> [out]). Returns false (with a message) unless they account
+// for exactly `rows` rows: the client's tensor_shape must never be the only thing that sizes a response buffer (e.g.
+// [1, 2*in_dim] is two rows, not one).
 static bool batch_dims(const ModelDesc& d, int64_t rows, const std::vector<int64_t>& in_shape, std::vector<int64_t>* dims,
                        std::string* why) {
   dims->clear();
-  if (d.tmpl == Template::Graph) {
+  if (d.tmpl == Template::Affine) {
+    *dims = in_shape;
+  } else if (d.tmpl == Template::Graph) {
     if (in_shape.size() > d.input_shape.size())
       for (size_t i = 0; i + d.input_shape.size() < in_shape.size(); ++i) dims->push_back(in_shape[i]);
   } else if (in_shape.size() <= 1) {
@@ -448,28 +415,45 @@ static bool batch_dims(const ModelDesc& d, int64_t rows, const std::vector<int64
   }
   int64_t on = 1;
   for (auto v : *dims) {
-    if (v < 0 || (v != 0 && on > ((int64_t)1 << 40) / v)) return false;
+    if (v < 0 || (v != 0 && on > ((int64_t)1 << 40) / v)) {
+      on = -1;
+      break;
+    }
     on *= v;
   }
   if (on != rows) {
     std::string sh = "[";
     for (size_t i = 0; i < in_shape.size(); ++i) sh += (i ? "," : "") + std::to_string(in_shape[i]);
     *why = "input shape " + sh + "] does not match the model signature: the trailing dimensions must hold exactly " +
-           std::to_string(d.in_dim) + " elements per row";
+           std::to_string(d.tmpl == Template::Affine ? 1 : d.in_dim) + " elements per row";
     return false;
   }
   return true;
 }
 
-// `names` (empty = every output, in packed order) must name declared outputs, each once
+// `names` (empty = every output, in packed order) must name declared outputs, each once; a single-output model answers its
+// one output whatever they name. p->declared is set even when planning fails, for the front-ends' own name checks.
 static bool plan_outputs(const ModelDesc& d, int64_t rows, const std::vector<int64_t>& in_shape, const std::vector<std::string>& names,
                          OutputPlan* p, std::string* why) {
+  p->declared = !d.outputs.empty();
   std::vector<int64_t> dims;
   if (!batch_dims(d, rows, in_shape, &dims, why)) return false;
   p->sel.clear();
+  p->dtypes.clear();
   p->shapes.clear();
-  p->out_dim = d.out_dim;
+  p->out_dim = d.tmpl == Template::Affine ? 1 : d.out_dim;
   p->rows = rows;
+  if (!p->declared) {
+    ModelOutput o;
+    o.name = d.output_name;
+    o.width = p->out_dim;
+    p->sel.push_back(o);
+    p->dtypes.push_back(TFSC_DT_FLOAT);
+    if (d.tmpl == Template::Graph) dims.insert(dims.end(), d.output_shape.begin(), d.output_shape.end());
+    else if (d.tmpl == Template::Mlp) dims.push_back(d.out_dim);
+    p->shapes.push_back(dims);
+    return true;
+  }
   std::vector<std::string> want = names;
   if (want.empty())
     for (auto& o : d.outputs) want.push_back(o.name);
@@ -485,6 +469,7 @@ static bool plan_outputs(const ModelDesc& d, int64_t rows, const std::vector<int
       return false;
     }
     p->sel.push_back(*o);
+    p->dtypes.push_back(output_dtype(o->kind));
     std::vector<int64_t> sh = dims;
     const OutputForm f = output_form(o->kind, d.head_n, d.head_k);
     for (int r = 0; r < f.rank; ++r) sh.push_back(f.dims[r]);
@@ -504,35 +489,64 @@ static void split_output(const OutputPlan& p, size_t i, const void* packed, void
 
 static std::string dtype_name(int dt) { return dt == TFSC_DT_INT64 ? "DT_INT64" : dt == TFSC_DT_INT32 ? "DT_INT32" : "DT_FLOAT"; }
 
-// C ABI, multi-output model: out[i].name selects the outputs (any order, no repeats); checks that every caller buffer
-// holds its output and returns the packed staging rows for the executor (nullptr + *bad, or nullptr alone: buffer too small)
-static void* abi_outputs_alloc(const ModelDesc& d, int64_t rows, const std::vector<int64_t>& in_shape, const tfsc_tensor* out,
-                               int n_out, OutputPlan* plan, std::vector<float>* packed, std::string* bad) {
-  std::vector<std::string> names;
-  for (int i = 0; i < n_out; ++i) {
-    if (!out[i].name) {
-      *bad = "predict: the model has several outputs, every out[i].name must name one of " + expected_outputs(d);
-      return nullptr;
-    }
-    names.push_back(out[i].name);
-  }
-  if (!plan_outputs(d, rows, in_shape, names, plan, bad)) return nullptr;
-  for (size_t i = 0; i < plan->sel.size(); ++i)
-    if (!out[i].data || out[i].nbytes < (size_t)(rows * plan->sel[i].width) * 4 || plan->shapes[i].size() > 8) return nullptr;
-  packed->assign((size_t)(rows * d.out_dim), 0.f);
-  return packed->data();
+// A single-input model's signature check: the one input, when the request names it, must carry the model's input name.
+static bool input_matches(const ModelDesc& d, const std::string* name, std::string* bad) {
+  if (!d.inputs.empty() || !name || *name == d.input_name) return true;
+  *bad = "input '" + *name + "' does not match the model signature (expects '" + d.input_name + "')";
+  return false;
 }
 
-// fills out[i] (data, dtype, shape, nbytes) for every output of the plan; nothing for a single-output model (empty plan)
-static void abi_outputs_deliver(const OutputPlan& plan, const void* packed, tfsc_tensor* out) {
-  for (size_t i = 0; i < plan.sel.size(); ++i) {
-    split_output(plan, i, packed, out[i].data);
-    out[i].dtype = output_dtype(plan.sel[i].kind);
-    out[i].rank = (int32_t)plan.shapes[i].size();
-    for (size_t j = 0; j < plan.shapes[i].size(); ++j) out[i].shape[j] = plan.shapes[i][j];
-    out[i].nbytes = (size_t)(plan.rows * plan.sel[i].width) * 4;
+// The outputs of one C ABI request, synchronous, asynchronous or forwarded: out[i].name selects the outputs of a model
+// that declares them (any order, no repeats). A whole-row plan is written straight into out[0].data, any other into
+// `packed`, which deliver() cuts into out[i].
+struct AbiOutputs {
+  tfsc_tensor* out = nullptr;
+  int n_out = 0;
+  std::vector<int64_t> in_shape;  // of the first input in name order: the response's batch dims
+  bool in_named = false;          // the caller's in[0] has a name, in_name
+  std::string in_name;
+  OutputPlan plan;
+  std::vector<float> packed;
+  std::string bad;  // why the request does not fit the model
+
+  AbiOutputs() = default;
+  AbiOutputs(const tfsc_tensor& in0, const std::vector<int64_t>& shape, tfsc_tensor* o, int n)
+      : out(o), n_out(n), in_shape(shape), in_named(in0.name != nullptr), in_name(in0.name ? in0.name : "") {}
+
+  // the executor's destination for `rows` rows: nullptr with `bad` set when the request does not fit the model, nullptr
+  // alone when an output buffer is too small
+  void* alloc(const ModelDesc& d, int64_t rows) {
+    if (!input_matches(d, in_named ? &in_name : nullptr, &bad)) return nullptr;
+    std::vector<std::string> names;
+    bool all_named = true;
+    for (int i = 0; i < n_out; ++i) {
+      all_named = all_named && out[i].name;
+      names.push_back(out[i].name ? out[i].name : "");
+    }
+    const bool planned = plan_outputs(d, rows, in_shape, names, &plan, &bad);
+    if (plan.declared && !all_named) {  // reported ahead of the plan's own errors
+      bad = "predict: the model has several outputs, every out[i].name must name one of " + expected_outputs(d);
+      return nullptr;
+    }
+    if (!planned) return nullptr;
+    for (size_t i = 0; i < plan.sel.size(); ++i)
+      if (!out[i].data || out[i].nbytes < (size_t)(rows * plan.sel[i].width) * 4 || plan.shapes[i].size() > 8) return nullptr;
+    if (plan.whole_row()) return out[0].data;
+    packed.assign((size_t)(rows * plan.out_dim), 0.f);
+    return packed.data();
   }
-}
+
+  // fills out[i] (data, dtype, shape, nbytes) once the executor has written the rows
+  void deliver() {
+    for (size_t i = 0; i < plan.sel.size(); ++i) {
+      if (!plan.whole_row()) split_output(plan, i, packed.data(), out[i].data);
+      out[i].dtype = plan.dtypes[i];
+      out[i].rank = (int32_t)plan.shapes[i].size();
+      for (size_t j = 0; j < plan.shapes[i].size(); ++j) out[i].shape[j] = plan.shapes[i][j];
+      out[i].nbytes = (size_t)(plan.rows * plan.sel[i].width) * 4;
+    }
+  }
+};
 
 // owner = member `member` of the current member list (the cache tier of that member, cachemanager.ServeRest/ServeGrpc: no
 // ring lookup -- the caller already routed, e.g. with tfsc_route), local node or another rank
@@ -568,37 +582,64 @@ static int predict_impl(tfsc_server* s, const char* model_name, const char* vers
   std::vector<InTensor> ts;
   InputLayout layout;
   if ((rc = abi_inputs(in, n_in, false, &ts, &layout)) < 0) return rc;
-  const tfsc_tensor& x = in[0];
-  const std::vector<int64_t>& ishape = ts[0].shape;
-  std::string err, bad;
-  tfsc_tensor* o = &out[0];
-  OutputPlan plan;
-  std::vector<float> packed;
-  auto alloc = [&](const ModelDesc& d, int64_t rows) -> void* {
-    if (d.inputs.empty() && x.name && d.input_name != x.name) {  // signature check of a single-input model
-      bad = "input '" + std::string(x.name) + "' does not match the model signature (expects '" + d.input_name + "')";
-      return nullptr;
-    }
-    if (!d.outputs.empty()) return abi_outputs_alloc(d, rows, ishape, out, n_out, &plan, &packed, &bad);
-    std::vector<int64_t> sh;
-    if (!out_shape(d, rows, ishape, &sh, &bad)) return nullptr;
-    int64_t on = 1;
-    for (auto v : sh) on *= v;
-    if (!o->data || o->nbytes < (size_t)on * 4 || sh.size() > 8) return nullptr;
-    o->dtype = TFSC_DT_FLOAT;
-    o->rank = (int32_t)sh.size();
-    for (size_t i = 0; i < sh.size(); ++i) o->shape[i] = sh[i];
-    o->nbytes = (size_t)on * 4;
-    return o->data;
-  };
+  AbiOutputs outs(in[0], ts[0].shape, out, n_out);
+  std::string err;
+  auto alloc = [&](const ModelDesc& d, int64_t rows) { return outs.alloc(d, rows); };
   rc = run_predict(s, node, remote, id, ts, layout, alloc, &err, deadline_ns);
-  if (rc < 0 && !bad.empty()) return fail(TFSC_E_INVALID, "%s", bad.c_str());
+  if (rc < 0 && !outs.bad.empty()) return fail(TFSC_E_INVALID, "%s", outs.bad.c_str());
   if (rc < 0) return fail(rc, "%s", err.c_str());
-  abi_outputs_deliver(plan, packed.data(), out);
+  outs.deliver();
   return 0;
 }
 
-static void set_resp_bytes(const std::string& body, void** resp, size_t* resp_len);
+static void set_resp(const std::string& body, void** resp, size_t* resp_len) {
+  char* b = (char*)malloc(body.size() + 1);
+  memcpy(b, body.data(), body.size());
+  b[body.size()] = 0;
+  *resp = b;
+  *resp_len = body.size();
+}
+
+// A request tensor as an executor input: DT_INT32 (token ids) or else DT_FLOAT. tensor_content and packed float_val stay
+// zero-copy views into the request; values stored any other way are gathered in `fs` / `is`.
+static bool tensor_input(const TensorView& v, InTensor* t, std::vector<float>* fs, std::vector<int32_t>* is, std::string* err) {
+  t->shape = v.shape;
+  if (v.dtype == TFSC_DT_INT32) {
+    const int32_t* p = nullptr;
+    const bool ok = tensor_i32(v, &p, &t->n, is, err);
+    t->data = p;
+    t->dtype = TFSC_DT_INT32;
+    return ok;
+  }
+  const float* p = nullptr;
+  const bool ok = tensor_f32(v, &p, &t->n, fs, err);
+  t->data = p;
+  t->dtype = TFSC_DT_FLOAT;
+  return ok;
+}
+
+// A gRPC response with a hole of `payload` bytes between prefix and suffix, for the executor to write the values into
+static void* frame_hole(const std::string& prefix, size_t payload, const std::string& suffix, char** buf, size_t* len) {
+  *len = prefix.size() + payload + suffix.size();
+  *buf = (char*)malloc(*len ? *len : 1);
+  if (!*buf) return nullptr;
+  memcpy(*buf, prefix.data(), prefix.size());
+  memcpy(*buf + prefix.size() + payload, suffix.data(), suffix.size());
+  return *buf + prefix.size();
+}
+
+// output i of the plan as a response tensor, its values cut out of the packed rows into `vals`
+static OutTensor out_tensor(const OutputPlan& p, size_t i, const void* packed, std::vector<char>* vals) {
+  vals->resize((size_t)(p.rows * p.sel[i].width) * 4);
+  split_output(p, i, packed, vals->data());
+  OutTensor t;
+  t.name = p.sel[i].name;
+  t.dtype = p.dtypes[i];
+  t.shape = p.shapes[i];
+  t.data = vals->data();
+  t.n = product(p.shapes[i]);
+  return t;
+}
 
 static int grpc_predict_impl(tfsc_server* s, const void* req, size_t req_len, void** resp, size_t* resp_len) {
   if (!s || !req || !resp || !resp_len) return fail(TFSC_E_INVALID, "grpc_predict: bad arguments");
@@ -633,23 +674,12 @@ static int grpc_predict_impl(tfsc_server* s, const void* req, size_t req_len, vo
   std::vector<std::vector<int32_t>> iscratch(n_in);
   bool input_ok = true;
   for (size_t i = 0; i < n_in && input_ok; ++i) {
-    const TensorView& v = view.inputs[i];
-    ts[i].name = v.name;
-    ts[i].shape = v.shape;
-    if (v.dtype == TFSC_DT_INT32) {  // token-id inputs (BERT bundles)
-      const int32_t* ip = nullptr;
-      input_ok = tensor_i32(v, &ip, &ts[i].n, &iscratch[i], &err);
-      ts[i].data = ip;
-      ts[i].dtype = TFSC_DT_INT32;
-    } else {
-      const float* fp = nullptr;
-      input_ok = tensor_f32(v, &fp, &ts[i].n, &scratch[i], &err);
-      ts[i].data = fp;
-      ts[i].dtype = TFSC_DT_FLOAT;
-    }
+    ts[i].name = view.inputs[i].name;
+    input_ok = tensor_input(view.inputs[i], &ts[i], &scratch[i], &iscratch[i], &err);
   }
   const InputLayout layout = layout_inputs(&ts);
   const TensorView& tv = view.inputs[0];
+  const std::string sig = view.signature_name.empty() ? "serving_default" : view.signature_name;
   char* buf = nullptr;
   size_t total = 0;
   std::string bad_sig;
@@ -660,39 +690,36 @@ static int grpc_predict_impl(tfsc_server* s, const void* req, size_t req_len, vo
       bad_sig = "input keys do not match the model signature (expects '" + d.input_name + "')";
       return nullptr;
     }
-    if (!d.outputs.empty()) {
-      // output_filter selects outputs (empty: all); the response map lists them in sorted name order. The two messages follow
-      // TF-Serving's predict_util.cc as far as they are known (wording unverified against its source).
-      std::set<std::string> sel;
-      for (auto& a : view.output_filter) {
-        if (!d.output(a)) {
-          std::string set;
-          for (auto& o : d.outputs) set += (set.empty() ? "" : ",") + o.name;
-          bad_sig = "output tensor alias not found in signature: " + a + " Outputs expected to be in the set {" + set + "}.";
-          return nullptr;
-        }
-        if (!sel.insert(a).second) {
-          bad_sig = "duplicate output tensor alias: " + a;
-          return nullptr;
-        }
+    // output_filter selects declared outputs (empty: all); the response map lists them in sorted name order. The two
+    // messages follow TF-Serving's predict_util.cc as far as they are known (wording unverified against its source), and
+    // are reported ahead of the plan's own errors.
+    std::set<std::string> sel;
+    std::string bad_filter;
+    for (auto& a : view.output_filter) {
+      if (!d.output(a)) {
+        std::string set;
+        for (auto& o : d.outputs) set += (set.empty() ? "" : ",") + o.name;
+        bad_filter = "output tensor alias not found in signature: " + a + " Outputs expected to be in the set {" + set + "}.";
+        break;
       }
-      if (!plan_outputs(d, rows, ts[0].shape, std::vector<std::string>(sel.begin(), sel.end()), &plan, &bad_sig)) return nullptr;
-      packed.assign((size_t)(rows * d.out_dim), 0.f);
-      return packed.data();
+      if (!sel.insert(a).second) {
+        bad_filter = "duplicate output tensor alias: " + a;
+        break;
+      }
     }
-    std::vector<int64_t> sh;
-    if (!out_shape(d, rows, ts[0].shape, &sh, &bad_sig)) return nullptr;
-    std::string prefix, suffix;
-    predict_response_frame(view.model_name, id.version, view.signature_name.empty() ? "serving_default" : view.signature_name,
-                           d.output_name, sh, &prefix, &suffix);
-    int64_t on = 1;
-    for (auto v : sh) on *= v;
-    total = prefix.size() + (size_t)on * 4 + suffix.size();
-    buf = (char*)malloc(total ? total : 1);
-    if (!buf) return nullptr;
-    memcpy(buf, prefix.data(), prefix.size());
-    memcpy(buf + prefix.size() + (size_t)on * 4, suffix.data(), suffix.size());
-    return buf + prefix.size();  // the executor's D2H result is scattered straight into the response
+    const bool planned = plan_outputs(d, rows, ts[0].shape, std::vector<std::string>(sel.begin(), sel.end()), &plan, &bad_sig);
+    if (plan.declared && !bad_filter.empty()) {
+      bad_sig = bad_filter;
+      return nullptr;
+    }
+    if (!planned) return nullptr;
+    if (plan.whole_row() && plan.dtypes[0] == TFSC_DT_FLOAT) {  // the executor's result goes straight into the response
+      std::string prefix, suffix;
+      predict_response_frame(view.model_name, id.version, sig, plan.sel[0].name, plan.shapes[0], &prefix, &suffix);
+      return frame_hole(prefix, (size_t)(rows * plan.out_dim) * 4, suffix, &buf, &total);
+    }
+    packed.assign((size_t)(rows * plan.out_dim), 0.f);
+    return packed.data();
   };
   if (!input_ok) {
     std::string e2;
@@ -708,40 +735,22 @@ static int grpc_predict_impl(tfsc_server* s, const void* req, size_t req_len, vo
     if (!bad_sig.empty()) return fail(TFSC_E_INVALID, "%s", bad_sig.c_str());
     return fail(rc, "%s", err.c_str());
   }
-  if (!plan.sel.empty()) {
-    std::vector<std::vector<char>> vals(plan.sel.size());
-    std::vector<OutTensor> outs(plan.sel.size());
-    for (size_t i = 0; i < plan.sel.size(); ++i) {
-      vals[i].resize((size_t)(plan.rows * plan.sel[i].width) * 4);
-      split_output(plan, i, packed.data(), vals[i].data());
-      outs[i].name = plan.sel[i].name;
-      outs[i].dtype = output_dtype(plan.sel[i].kind);
-      outs[i].shape = plan.shapes[i];
-      outs[i].data = vals[i].data();
-      outs[i].n = product(plan.shapes[i]);
-    }
-    set_resp_bytes(encode_predict_response(view.model_name, id.version,
-                                           view.signature_name.empty() ? "serving_default" : view.signature_name, outs),
-                   resp, resp_len);
+  if (buf) {
+    *resp = buf;
+    *resp_len = total;
     return 0;
   }
-  *resp = buf;
-  *resp_len = total;
+  std::vector<std::vector<char>> vals(plan.sel.size());
+  std::vector<OutTensor> outs;
+  for (size_t i = 0; i < plan.sel.size(); ++i) outs.push_back(out_tensor(plan, i, packed.data(), &vals[i]));
+  set_resp(encode_predict_response(view.model_name, id.version, sig, outs), resp, resp_len);
   return 0;
-}
-
-static void set_resp_bytes(const std::string& body, void** resp, size_t* resp_len) {
-  char* b = (char*)malloc(body.size() + 1);
-  memcpy(b, body.data(), body.size());
-  b[body.size()] = 0;
-  *resp = b;
-  *resp_len = body.size();
 }
 
 // ---- Classify / Regress (tfservingproxy.go:173-198): tf.Example inputs -> one row per example -> the predict path.
 // method: 1 = classify, 2 = regress. Fills scores [n, per] (classify: per = outputs per example; regress: per == 1).
 static int run_examples(tfsc_server* s, const ExampleRequestView& view, int method, std::vector<float>* scores, int64_t* n_out,
-                        int64_t* per_out, ModelId* id_out, std::string* sig_out, std::string* err, int* code) {
+                        int64_t* per_out, ModelId* id_out, std::string* sig_out, std::string* err) {
   const std::string version = std::to_string(view.version);  // clientForSpec: "0" when absent
   Node* node;
   ModelId id;
@@ -822,7 +831,6 @@ static int run_examples(tfsc_server* s, const ExampleRequestView& view, int meth
   *per_out = per;
   *id_out = id;
   *sig_out = want;
-  (void)code;
   return 0;
 }
 
@@ -839,14 +847,14 @@ static int grpc_examples_impl(tfsc_server* s, int method, const void* req, size_
   int64_t n = 0, per = 0;
   ModelId id;
   std::string sig;
-  int rc = run_examples(s, view, method, &scores, &n, &per, &id, &sig, &err, nullptr);
+  int rc = run_examples(s, view, method, &scores, &n, &per, &id, &sig, &err);
   if (rc < 0) {
     s->fail_grpc++;
     return fail(rc, "%s", err.c_str());
   }
   const std::string out = method == 1 ? encode_classification_response(view.model_name, id.version, sig, scores.data(), n, per)
                                       : encode_regression_response(view.model_name, id.version, sig, scores.data(), n);
-  set_resp_bytes(out, resp, resp_len);
+  set_resp(out, resp, resp_len);
   return 0;
 }
 
@@ -878,77 +886,54 @@ static int grpc_session_run_impl(tfsc_server* s, const void* req, size_t req_len
     return fail(TFSC_E_INVALID, "SessionRun on a model template takes exactly one feed (the signature input) and one fetch (its output)");
   }
   const TensorView& tv = view.feeds[0];
-  const void* xdata = nullptr;
-  int64_t n = 0;
+  std::vector<InTensor> ts(1);  // unnamed: the feed's name is checked against the signature below
   std::vector<float> scratch;
   std::vector<int32_t> iscratch;
-  bool ok;
-  if (tv.dtype == TFSC_DT_INT32) {
-    const int32_t* ip = nullptr;
-    ok = tensor_i32(tv, &ip, &n, &iscratch, &err);
-    xdata = ip;
-  } else {
-    const float* fp = nullptr;
-    ok = tensor_f32(tv, &fp, &n, &scratch, &err);
-    xdata = fp;
-  }
-  if (!ok) {
+  if (!tensor_input(tv, &ts[0], &scratch, &iscratch, &err)) {
     s->fail_grpc++;
     return fail(TFSC_E_INVALID, "%s", err.c_str());
   }
+  const InputLayout layout = layout_inputs(&ts);
   char* buf = nullptr;
   size_t total = 0;
   std::string bad;
   OutputPlan plan;
   std::vector<float> packed;
   auto alloc = [&](const ModelDesc& d, int64_t rows) -> void* {
-    if (!d.outputs.empty()) {  // a multi-output model: the fetch names any one of its outputs
-      if (strip(tv.name) != d.input_name || !d.output(strip(view.fetch[0]))) {
-        bad = "feed / fetch do not name the model's tensors (feed '" + d.input_name + ":0', fetch one of " + expected_outputs(d) + ")";
-        return nullptr;
-      }
-      if (!plan_outputs(d, rows, tv.shape, {strip(view.fetch[0])}, &plan, &bad)) return nullptr;
-      packed.assign((size_t)(rows * d.out_dim), 0.f);
-      return packed.data();
-    }
-    if (strip(tv.name) != d.input_name || strip(view.fetch[0]) != d.output_name) {
-      bad = "feed / fetch do not name the model's tensors (feed '" + d.input_name + ":0', fetch '" + d.output_name + ":0')";
+    const std::string fetch = strip(view.fetch[0]);
+    const bool planned = plan_outputs(d, rows, tv.shape, {fetch}, &plan, &bad);
+    // the feed names the model's input and the fetch its output, or any one of its declared outputs (reported ahead of the
+    // plan's own errors)
+    if (strip(tv.name) != d.input_name || (plan.declared ? !d.output(fetch) : fetch != d.output_name)) {
+      bad = "feed / fetch do not name the model's tensors (feed '" + d.input_name + ":0', fetch " +
+            (plan.declared ? "one of " + expected_outputs(d) : "'" + d.output_name + ":0'") + ")";
       return nullptr;
     }
-    std::vector<int64_t> sh;
-    if (!out_shape(d, rows, tv.shape, &sh, &bad)) return nullptr;
-    std::string prefix, suffix;
-    session_run_response_frame(view.model_name, id.version, view.signature_name, view.fetch[0], sh, &prefix, &suffix);
-    int64_t on = 1;
-    for (auto v : sh) on *= v;
-    total = prefix.size() + (size_t)on * 4 + suffix.size();
-    buf = (char*)malloc(total ? total : 1);
-    if (!buf) return nullptr;
-    memcpy(buf, prefix.data(), prefix.size());
-    memcpy(buf + prefix.size() + (size_t)on * 4, suffix.data(), suffix.size());
-    return buf + prefix.size();
+    if (!planned) return nullptr;
+    if (plan.whole_row() && plan.dtypes[0] == TFSC_DT_FLOAT) {  // the executor's result goes straight into the response
+      std::string prefix, suffix;
+      session_run_response_frame(view.model_name, id.version, view.signature_name, view.fetch[0], plan.shapes[0], &prefix, &suffix);
+      return frame_hole(prefix, (size_t)(rows * plan.out_dim) * 4, suffix, &buf, &total);
+    }
+    packed.assign((size_t)(rows * plan.out_dim), 0.f);
+    return packed.data();
   };
-  rc = run_predict_one(s, node, remote, id, xdata, n, tv.dtype == TFSC_DT_INT32 ? TFSC_DT_INT32 : TFSC_DT_FLOAT, alloc, &err);
+  rc = run_predict(s, node, remote, id, ts, layout, alloc, &err);
   if (rc < 0) {
     free(buf);
     s->fail_grpc++;
     if (!bad.empty()) return fail(TFSC_E_INVALID, "%s", bad.c_str());
     return fail(rc, "%s", err.c_str());
   }
-  if (!plan.sel.empty()) {
-    std::vector<char> vals((size_t)(plan.rows * plan.sel[0].width) * 4);
-    split_output(plan, 0, packed.data(), vals.data());
-    OutTensor t;
-    t.name = view.fetch[0];
-    t.dtype = output_dtype(plan.sel[0].kind);
-    t.shape = plan.shapes[0];
-    t.data = vals.data();
-    t.n = product(plan.shapes[0]);
-    set_resp_bytes(encode_session_run_response(view.model_name, id.version, view.signature_name, t), resp, resp_len);
+  if (buf) {
+    *resp = buf;
+    *resp_len = total;
     return 0;
   }
-  *resp = buf;
-  *resp_len = total;
+  std::vector<char> vals;
+  OutTensor t = out_tensor(plan, 0, packed.data(), &vals);
+  t.name = view.fetch[0];
+  set_resp(encode_session_run_response(view.model_name, id.version, view.signature_name, t), resp, resp_len);
   return 0;
 }
 
@@ -973,14 +958,6 @@ static int http_for(int rc) {
     case TFSC_E_EMPTY_RING: return 503;
     default: return 500;
   }
-}
-
-static void set_resp(const std::string& body, void** resp, size_t* resp_len) {
-  char* b = (char*)malloc(body.size() + 1);
-  memcpy(b, body.data(), body.size());
-  b[body.size()] = 0;
-  *resp = b;
-  *resp_len = body.size();
 }
 
 static std::string error_json(const std::string& msg) {
@@ -1236,7 +1213,6 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
       return fail_http(400, err.empty() ? "empty request" : err);
     }
     std::vector<float> y;
-    std::vector<int64_t> oshape;
     std::string bad_sig;
     OutputPlan plan;
     std::vector<InTensor> ts(columns.size());
@@ -1250,19 +1226,10 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
     const InputLayout layout = layout_inputs(&ts);
     if (!ts.empty()) shape = ts[0].shape;  // the batch dimension of the response
     auto alloc = [&](const ModelDesc& d, int64_t rows) -> void* {
-      if (d.inputs.empty() && !input_key.empty() && input_key != d.input_name) {
-        bad_sig = "input '" + input_key + "' does not match the model signature (expects '" + d.input_name + "')";
-        return nullptr;
-      }
-      if (!d.outputs.empty()) {  // every output (REST has no output filter), answered in packed order below
-        if (!plan_outputs(d, rows, shape, {}, &plan, &bad_sig)) return nullptr;
-        y.assign((size_t)(rows * d.out_dim), 0.f);
-        return y.data();
-      }
-      if (!out_shape(d, rows, shape, &oshape, &bad_sig)) return nullptr;
-      int64_t on = 1;
-      for (auto v : oshape) on *= v;
-      y.resize((size_t)on);
+      if (!input_matches(d, input_key.empty() ? nullptr : &input_key, &bad_sig)) return nullptr;
+      // every output (REST has no output filter), answered in packed order below
+      if (!plan_outputs(d, rows, shape, {}, &plan, &bad_sig)) return nullptr;
+      y.assign((size_t)(rows * plan.out_dim), 0.f);
       return y.data();
     };
     if (!ts.empty()) rc = run_predict(s, node, remote, id, ts, layout, alloc, &err);
@@ -1275,12 +1242,13 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
       rc = run_predict_one(s, node, remote, id, ints.data(), (int64_t)ints.size(), TFSC_DT_INT32, alloc, &err);
     }
     if (rc < 0) return fail_http(bad_sig.empty() ? http_for(rc) : 400, bad_sig.empty() ? err : bad_sig);
-    if (!plan.sel.empty()) {
+    if (plan.declared) {
       *http_status = 200;
       set_resp(rest_multi_output_json(plan, y.data(), instances != nullptr), resp, resp_len);
       return 0;
     }
     // TF-Serving's writer: 4-space indent, arrays on one line, closing bracket on its own line
+    const std::vector<int64_t>& oshape = plan.shapes[0];
     std::string b = std::string("{\n    \"") + (instances ? "predictions" : "outputs") + "\": ";
     size_t idx = 0;
     if (oshape.empty()) {
@@ -1379,7 +1347,7 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
     int64_t n = 0, per = 0;
     ModelId rid;
     std::string sig;
-    rc = run_examples(s, view, method, &scores, &n, &per, &rid, &sig, &err, nullptr);
+    rc = run_examples(s, view, method, &scores, &n, &per, &rid, &sig, &err);
     if (rc < 0) return fail_http(rc == TFSC_E_INVALID ? 400 : http_for(rc), err);
     std::string b = "{\n    \"results\": [";
     for (int64_t i = 0; i < n; ++i) {
@@ -1452,11 +1420,8 @@ struct tfsc_ticket {
   PredictRequest req;
   char* staging = nullptr;
   size_t staging_bytes = 0, in_al = 0, out_bytes = 0;
-  tfsc_tensor* out = nullptr;
-  int n_out = 0;
-  std::vector<int64_t> oshape;
-  OutputPlan plan;            // multi-output model: the outputs out[i] asked for, split from `packed` by wait()
-  std::vector<float> packed;
+  AbiOutputs outs;
+  void* y = nullptr;  // where wait() copies the staged result: outs' destination
   // requests owned by another rank take the (synchronous) forward hop on a helper thread
   std::thread remote_thread;
   std::mutex mu;
@@ -1482,13 +1447,10 @@ static int submit_impl(tfsc_server* s, const char* model_name, const char* versi
   std::vector<InTensor> ts;
   InputLayout layout;
   if ((rc = abi_inputs(in, n_in, true, &ts, &layout)) < 0) return rc;
-  const tfsc_tensor& x = in[0];
-  const std::vector<int64_t> ishape = ts[0].shape;
   auto t = std::make_unique<tfsc_ticket>();
   t->srv = s;
   t->node = node;
-  t->out = &out[0];
-  t->n_out = n_out;
+  t->outs = AbiOutputs(in[0], ts[0].shape, out, n_out);
   std::string err;
   if (!node) {
     // another rank owns the model: the forward hop is synchronous, run it beside the caller
@@ -1500,28 +1462,11 @@ static int submit_impl(tfsc_server* s, const char* model_name, const char* versi
     t->remote_ts = ts;
     t->remote_l = layout;
     tfsc_ticket* tp = t.get();
-    const std::string xname = x.name ? x.name : "";
-    const bool has_name = x.name != nullptr;
-    t->remote_thread = std::thread([tp, s, remote, id, ishape, xname, has_name, deadline_ns] {
-      std::string e2, bad;
-      auto alloc = [&](const ModelDesc& d, int64_t rows) -> void* {
-        if (d.inputs.empty() && has_name && d.input_name != xname) {
-          bad = "input '" + xname + "' does not match the model signature (expects '" + d.input_name + "')";
-          return nullptr;
-        }
-        if (!d.outputs.empty()) {
-          void* y = abi_outputs_alloc(d, rows, ishape, tp->out, tp->n_out, &tp->plan, &tp->packed, &bad);
-          tp->out_bytes = tp->packed.size() * 4;
-          return y;
-        }
-        if (!out_shape(d, rows, ishape, &tp->oshape, &bad)) return nullptr;
-        int64_t on = 1;
-        for (auto v : tp->oshape) on *= v;
-        if (!tp->out->data || tp->out->nbytes < (size_t)on * 4 || tp->oshape.size() > 8) return nullptr;
-        tp->out_bytes = (size_t)on * 4;
-        return tp->out->data;
-      };
+    t->remote_thread = std::thread([tp, s, remote, id, deadline_ns] {
+      std::string e2;
+      auto alloc = [tp](const ModelDesc& d, int64_t rows) { return tp->outs.alloc(d, rows); };
       int r = s->fwd->forward(remote, id.name, id.version, tp->remote_ts, tp->remote_l, alloc, nullptr, deadline_ns, &e2);
+      const std::string& bad = tp->outs.bad;
       std::lock_guard<std::mutex> lk(tp->mu);
       tp->remote_rc = r < 0 && !bad.empty() ? TFSC_E_INVALID : r;
       tp->remote_err = !bad.empty() ? bad : e2;
@@ -1532,27 +1477,13 @@ static int submit_impl(tfsc_server* s, const char* model_name, const char* versi
   }
   rc = node->prepare(id, layout, &t->req, nullptr, &err);
   if (rc < 0) return fail(rc, "%s", err.c_str());
-  const ModelDesc& d = t->req.dm->desc;
-  std::string bad;
-  if (d.inputs.empty() && x.name && d.input_name != x.name)
-    bad = "input '" + std::string(x.name) + "' does not match the model signature (expects '" + d.input_name + "')";
-  bool buffers_ok = true;
-  if (bad.empty() && !d.outputs.empty()) {
-    buffers_ok = abi_outputs_alloc(d, t->req.rows, ishape, out, n_out, &t->plan, &t->packed, &bad) != nullptr;
-  } else if (bad.empty()) {
-    out_shape(d, t->req.rows, ishape, &t->oshape, &bad);
-  }
-  if (!bad.empty()) {
+  t->y = t->outs.alloc(t->req.dm->desc, t->req.rows);
+  if (!t->y) {
     node->abandon(&t->req);
-    return fail(TFSC_E_INVALID, "%s", bad.c_str());
-  }
-  int64_t on = 1;
-  for (auto v : t->oshape) on *= v;
-  t->out_bytes = d.outputs.empty() ? (size_t)on * 4 : t->packed.size() * 4;
-  if (d.outputs.empty() ? (!out[0].data || out[0].nbytes < t->out_bytes || t->oshape.size() > 8) : !buffers_ok) {
-    node->abandon(&t->req);
+    if (!t->outs.bad.empty()) return fail(TFSC_E_INVALID, "%s", t->outs.bad.c_str());
     return fail(TFSC_E_BUFFER, "output buffer too small");
   }
+  t->out_bytes = (size_t)(t->req.rows * t->outs.plan.out_dim) * 4;
   t->in_al = ((size_t)layout.n_elems * 4 + 255) & ~(size_t)255;
   t->staging_bytes = t->in_al + t->out_bytes;
   t->staging = static_cast<char*>(node->staging_alloc(t->staging_bytes));
@@ -1590,19 +1521,11 @@ static int wait_impl(tfsc_ticket* t, int64_t timeout_ns) {
       return fail(TFSC_E_TIMEOUT, "predict_wait: request still in flight");
     rc = t->req.rc;
     err = t->req.err;
-    if (rc == 0 && !t->delivered)
-      memcpy(t->plan.sel.empty() ? t->out->data : (void*)t->packed.data(), t->staging + t->in_al, t->out_bytes);
   }
   if (rc < 0) return fail(rc, "%s", err.c_str());
-  if (!t->delivered && !t->plan.sel.empty()) {
-    abi_outputs_deliver(t->plan, t->packed.data(), t->out);
-    t->delivered = true;
-  }
   if (!t->delivered) {
-    t->out->dtype = TFSC_DT_FLOAT;
-    t->out->rank = (int32_t)t->oshape.size();
-    for (size_t i = 0; i < t->oshape.size(); ++i) t->out->shape[i] = t->oshape[i];
-    t->out->nbytes = t->out_bytes;
+    if (t->node) memcpy(t->y, t->staging + t->in_al, t->out_bytes);  // a forwarded result is already in place
+    t->outs.deliver();
     t->delivered = true;
   }
   return 0;
@@ -1675,7 +1598,7 @@ int tfsc_node_set_max_resident(tfsc_server* s, int node, int max_concurrent_mode
 }
 
 int tfsc_k_copy_segments(const tfsc_copy_seg* segs, int n, void* stream) {
-  if (int rc = check_device_early()) return rc;
+  if (int rc = check_device()) return rc;
   if (!segs || n < 0) return fail(TFSC_E_INVALID, "copy_segments: bad arguments");
   static_assert(sizeof(tfsc_copy_seg) == sizeof(CopySeg), "ABI struct mirrors the kernel's segment");
   cudaError_t e = launch_copy_segments(reinterpret_cast<const CopySeg*>(segs), n, (cudaStream_t)stream);
@@ -1716,15 +1639,6 @@ int tfsc_get_stats(tfsc_server* s, int node, tfsc_stats* out) {
 }
 
 // ------------------------------------------------------------------ raw kernel entries ------
-static int check_device() {
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-    cudaGetLastError();
-    return fail(TFSC_E_NO_DEVICE, "no CUDA device available: this library has no CPU fallback");
-  }
-  return 0;
-}
-
 int tfsc_k_affine(const float* x, float* y, int64_t n, const float* a, const float* b, void* stream) {
   if (int rc = check_device()) return rc;
   cudaError_t e = launch_affine(x, y, n, a, b, (cudaStream_t)stream);

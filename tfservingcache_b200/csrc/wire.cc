@@ -261,56 +261,6 @@ bool tensor_i32(const TensorView& t, const int32_t** data, int64_t* n, std::vect
   return true;
 }
 
-void predict_response_frame(const std::string& model_name, int64_t version, const std::string& signature_name,
-                            const std::string& output_name, const std::vector<int64_t>& shape, std::string* prefix,
-                            std::string* suffix) {
-  int64_t n = 1;
-  for (auto d : shape) n *= d;
-  const size_t payload = (size_t)n * 4;
-  // TensorProto head: dtype, tensor_shape, then the float_val length header
-  std::string thead;
-  put_tag(&thead, 1, 0);
-  put_varint(&thead, TFSC_DT_FLOAT);
-  std::string sh;
-  for (auto d : shape) {
-    std::string dim;
-    if (d != 0) {
-      put_tag(&dim, 1, 0);
-      put_varint(&dim, (uint64_t)d);
-    }
-    put_ld(&sh, 2, dim);
-  }
-  put_ld(&thead, 2, sh);
-  if (payload) {
-    put_tag(&thead, 5, 2);
-    put_varint(&thead, payload);
-  }
-  const size_t tensor_len = thead.size() + payload;
-  std::string ehead;  // map entry: key, then value header
-  put_ld(&ehead, 1, output_name);
-  put_tag(&ehead, 2, 2);
-  put_varint(&ehead, tensor_len);
-  const size_t entry_len = ehead.size() + tensor_len;
-  prefix->clear();
-  put_tag(prefix, 1, 2);
-  put_varint(prefix, entry_len);
-  prefix->append(ehead);
-  prefix->append(thead);
-  // model_spec
-  std::string spec;
-  if (!model_name.empty()) put_ld(&spec, 1, model_name);
-  std::string ver;
-  if (version != 0) {
-    put_tag(&ver, 1, 0);
-    put_varint(&ver, (uint64_t)version);
-  }
-  put_ld(&spec, 2, ver);
-  if (!signature_name.empty()) put_ld(&spec, 3, signature_name);
-  suffix->clear();
-  put_ld(suffix, 2, spec);
-}
-
-
 // ------------------------------------------------------------------ Classify / Regress / SessionRun ----
 static bool decode_model_spec_field(const uint8_t* p, size_t l, std::string* name, bool* has_version, int64_t* version,
                                     std::string* signature) {
@@ -570,15 +520,12 @@ bool decode_session_run_request(const void* data, size_t len, SessionRunView* ou
   return true;
 }
 
-void session_run_response_frame(const std::string& model_name, int64_t version, const std::string& signature_name,
-                                const std::string& tensor_name, const std::vector<int64_t>& shape, std::string* prefix,
-                                std::string* suffix) {
-  int64_t n = 1;
-  for (auto d : shape) n *= d;
-  const size_t payload = (size_t)n * 4;
-  std::string thead;
-  put_tag(&thead, 1, 0);
-  put_varint(&thead, TFSC_DT_FLOAT);
+// ------------------------------------------------------------------ Predict / SessionRun responses ----
+// TensorProto up to its values: dtype, tensor_shape
+static std::string tensor_header(int dtype, const std::vector<int64_t>& shape) {
+  std::string s;
+  put_tag(&s, 1, 0);
+  put_varint(&s, (uint64_t)dtype);
   std::string sh;
   for (auto d : shape) {
     std::string dim;
@@ -588,40 +535,12 @@ void session_run_response_frame(const std::string& model_name, int64_t version, 
     }
     put_ld(&sh, 2, dim);
   }
-  put_ld(&thead, 2, sh);
-  if (payload) {
-    put_tag(&thead, 5, 2);
-    put_varint(&thead, payload);
-  }
-  const size_t tensor_len = thead.size() + payload;
-  std::string nhead;  // NamedTensorProto: name, then the tensor header
-  if (!tensor_name.empty()) put_ld(&nhead, 1, tensor_name);
-  put_tag(&nhead, 2, 2);
-  put_varint(&nhead, tensor_len);
-  prefix->clear();
-  put_tag(prefix, 1, 2);
-  put_varint(prefix, nhead.size() + tensor_len);
-  prefix->append(nhead);
-  prefix->append(thead);
-  suffix->clear();
-  put_ld(suffix, 3, spec_bytes(model_name, version, signature_name));
+  put_ld(&s, 2, sh);
+  return s;
 }
 
-// ------------------------------------------------------------------ multi-output responses ----
 static std::string tensor_proto(const OutTensor& t) {
-  std::string s;
-  put_tag(&s, 1, 0);
-  put_varint(&s, (uint64_t)t.dtype);
-  std::string sh;
-  for (auto d : t.shape) {
-    std::string dim;
-    if (d != 0) {
-      put_tag(&dim, 1, 0);
-      put_varint(&dim, (uint64_t)d);
-    }
-    put_ld(&sh, 2, dim);
-  }
-  put_ld(&s, 2, sh);
+  std::string s = tensor_header(t.dtype, t.shape);
   if (t.n > 0) {
     std::string vals;
     if (t.dtype == TFSC_DT_FLOAT) {
@@ -661,6 +580,46 @@ std::string encode_session_run_response(const std::string& model_name, int64_t v
   put_ld(&s, 1, named);
   put_ld(&s, 3, spec_bytes(model_name, version, signature_name));
   return s;
+}
+
+// The bytes of a response whose field 1 is one {name_field, tensor = 2} entry holding a DT_FLOAT tensor of `shape`, and
+// whose field `spec_field` is the model spec, split around the packed float_val payload: the encoders' bytes, with the
+// values left for the executor to write in between.
+static void float_frame(const std::string& name_field, const std::vector<int64_t>& shape, uint32_t spec_field,
+                        const std::string& spec, std::string* prefix, std::string* suffix) {
+  int64_t n = 1;
+  for (auto d : shape) n *= d;
+  const size_t payload = (size_t)n * 4;
+  std::string thead = tensor_header(TFSC_DT_FLOAT, shape);
+  if (payload) {
+    put_tag(&thead, 5, 2);
+    put_varint(&thead, payload);
+  }
+  std::string entry = name_field;
+  put_tag(&entry, 2, 2);
+  put_varint(&entry, thead.size() + payload);
+  prefix->clear();
+  put_tag(prefix, 1, 2);
+  put_varint(prefix, entry.size() + thead.size() + payload);
+  *prefix += entry + thead;
+  suffix->clear();
+  put_ld(suffix, spec_field, spec);
+}
+
+void predict_response_frame(const std::string& model_name, int64_t version, const std::string& signature_name,
+                            const std::string& output_name, const std::vector<int64_t>& shape, std::string* prefix,
+                            std::string* suffix) {
+  std::string key;  // a map entry always carries its key
+  put_ld(&key, 1, output_name);
+  float_frame(key, shape, 2, spec_bytes(model_name, version, signature_name), prefix, suffix);
+}
+
+void session_run_response_frame(const std::string& model_name, int64_t version, const std::string& signature_name,
+                                const std::string& tensor_name, const std::vector<int64_t>& shape, std::string* prefix,
+                                std::string* suffix) {
+  std::string name;
+  if (!tensor_name.empty()) put_ld(&name, 1, tensor_name);
+  float_frame(name, shape, 3, spec_bytes(model_name, version, signature_name), prefix, suffix);
 }
 
 }  // namespace tfsc

@@ -75,15 +75,22 @@ class Server:
         segment_ids, int32 [batch, seq] each). outputs: names of outputs of a multi-output model (signature.outputs,
         e.g. ("classes", "probabilities")): the result is then {name: ndarray} (classes int64, top-k classes int32);
         without it the result is the one ndarray of a single-output model."""
+        _x, tin, tout, n_out, result = self._request(x, dict(out_capacity_elems=out_capacity_elems, input_name=input_name,
+                                                             outputs=outputs))
+        check(lib.tfsc_predict(self._h, model_name.encode(), version.encode(), tin, len(tin), tout, n_out), "predict")
+        return result()
+
+    @staticmethod
+    def _request(x, kw):
+        """(the input arrays kept alive, the input tensors, the output tensor(s), their count, result) of one Predict;
+        result() reads what the call wrote: {name: ndarray} when kw["outputs"] names outputs, else one ndarray."""
+        outputs = kw.get("outputs")
         if outputs is not None:
-            _x, tin, ys, touts = self._tensors_multi(x, out_capacity_elems, input_name, outputs)
-            check(lib.tfsc_predict(self._h, model_name.encode(), version.encode(), tin, len(tin), touts, len(outputs)),
-                  "predict")
-            return self._results(ys, touts, outputs)
-        _x, tin, y, tout = self._tensors(x, out_capacity_elems, input_name)
-        check(lib.tfsc_predict(self._h, model_name.encode(), version.encode(), tin, len(tin), C.byref(tout), 1),
-              "predict")
-        return self._result(y, tout)
+            outputs = list(outputs)
+            arrays, tin, ys, touts = Server._tensors_multi(x, kw.get("out_capacity_elems"), kw.get("input_name"), outputs)
+            return arrays, tin, touts, len(outputs), lambda: Server._results(ys, touts, outputs)
+        arrays, tin, y, tout = Server._tensors(x, kw.get("out_capacity_elems"), kw.get("input_name"))
+        return arrays, tin, C.byref(tout), 1, lambda: Server._result(y, tout)
 
     @staticmethod
     def _tensors_multi(x, out_capacity_elems, input_name, outputs):
@@ -146,30 +153,18 @@ class Server:
 
     def predict_deadline(self, model_name: str, version: str, x: np.ndarray, deadline_ns: int, **kw) -> np.ndarray:
         """tfsc_predict_deadline: deadline is absolute on the clock of now_ns() (0 = none). outputs= as for predict()."""
-        if kw.get("outputs") is not None:
-            outs = kw["outputs"]
-            _x, tin, ys, touts = self._tensors_multi(x, kw.get("out_capacity_elems"), kw.get("input_name"), outs)
-            check(lib.tfsc_predict_deadline(self._h, model_name.encode(), version.encode(), tin, len(tin), touts, len(outs),
-                                            int(deadline_ns)), "predict")
-            return self._results(ys, touts, outs)
-        _x, tin, y, tout = self._tensors(x, kw.get("out_capacity_elems"), kw.get("input_name"))
-        check(lib.tfsc_predict_deadline(self._h, model_name.encode(), version.encode(), tin, len(tin), C.byref(tout), 1,
+        _x, tin, tout, n_out, result = self._request(x, kw)
+        check(lib.tfsc_predict_deadline(self._h, model_name.encode(), version.encode(), tin, len(tin), tout, n_out,
                                         int(deadline_ns)), "predict")
-        return self._result(y, tout)
+        return result()
 
     def predict_member(self, member: int, model_name: str, version: str, x: np.ndarray, deadline_ns: int = 0, **kw) -> np.ndarray:
         """tfsc_predict_member: the cache tier of member `member` (index into gpu.members), no ring lookup. outputs= as for
         predict()."""
-        if kw.get("outputs") is not None:
-            outs = kw["outputs"]
-            _x, tin, ys, touts = self._tensors_multi(x, kw.get("out_capacity_elems"), kw.get("input_name"), outs)
-            check(lib.tfsc_predict_member(self._h, member, model_name.encode(), version.encode(), tin, len(tin), touts,
-                                          len(outs), int(deadline_ns)), "predict_member")
-            return self._results(ys, touts, outs)
-        _x, tin, y, tout = self._tensors(x, kw.get("out_capacity_elems"), kw.get("input_name"))
-        check(lib.tfsc_predict_member(self._h, member, model_name.encode(), version.encode(), tin, len(tin), C.byref(tout), 1,
+        _x, tin, tout, n_out, result = self._request(x, kw)
+        check(lib.tfsc_predict_member(self._h, member, model_name.encode(), version.encode(), tin, len(tin), tout, n_out,
                                       int(deadline_ns)), "predict_member")
-        return self._result(y, tout)
+        return result()
 
     @staticmethod
     def now_ns() -> int:
@@ -179,16 +174,10 @@ class Server:
         """Asynchronous Predict (tfsc_predict_submit): returns a Ticket; .wait() yields the result. outputs= as for
         predict()."""
         t = C.c_void_p()
-        if kw.get("outputs") is not None:
-            outs = list(kw["outputs"])
-            xk, tin, ys, touts = self._tensors_multi(x, kw.get("out_capacity_elems"), kw.get("input_name"), outs)
-            check(lib.tfsc_predict_submit(self._h, model_name.encode(), version.encode(), tin, len(tin), touts, len(outs),
-                                          int(deadline_ns), C.byref(t)), "predict_submit")
-            return Ticket(t, ys, touts, outs, keep=xk)
-        xk, tin, y, tout = self._tensors(x, kw.get("out_capacity_elems"), kw.get("input_name"))
-        check(lib.tfsc_predict_submit(self._h, model_name.encode(), version.encode(), tin, len(tin), C.byref(tout), 1,
+        xk, tin, tout, n_out, result = self._request(x, kw)
+        check(lib.tfsc_predict_submit(self._h, model_name.encode(), version.encode(), tin, len(tin), tout, n_out,
                                       int(deadline_ns), C.byref(t)), "predict_submit")
-        return Ticket(t, y, tout)
+        return Ticket(t, result, keep=(xk, tout))
 
     def fwd_window(self):
         """(rank, device pointer, bytes, slot bytes) of this rank's forward window (needs cluster.endpoints)."""
@@ -202,15 +191,6 @@ class Server:
         check(lib.tfsc_fwd_peer_window(self._h, peer_rank, C.byref(p), C.byref(n)), "fwd_peer_window")
         return p.value, n.value
 
-    def grpc_predict(self, request_bytes: bytes) -> bytes:
-        resp = C.c_void_p()
-        n = C.c_size_t()
-        check(lib.tfsc_grpc_predict(self._h, request_bytes, len(request_bytes), C.byref(resp), C.byref(n)), "grpc_predict")
-        try:
-            return C.string_at(resp, n.value)
-        finally:
-            lib.tfsc_free(resp)
-
     def _wire_call(self, fn, request_bytes: bytes, where: str) -> bytes:
         resp = C.c_void_p()
         n = C.c_size_t()
@@ -219,6 +199,9 @@ class Server:
             return C.string_at(resp, n.value)
         finally:
             lib.tfsc_free(resp)
+
+    def grpc_predict(self, request_bytes: bytes) -> bytes:
+        return self._wire_call(lib.tfsc_grpc_predict, request_bytes, "grpc_predict")
 
     def grpc_classify(self, request_bytes: bytes) -> bytes:
         return self._wire_call(lib.tfsc_grpc_classify, request_bytes, "grpc_classify")
@@ -259,14 +242,12 @@ class Server:
 class Ticket:
     """An in-flight asynchronous Predict (tfsc_ticket). Keeps the output buffer alive until released."""
 
-    def __init__(self, handle, y, tout, outputs=None, keep=None):
-        self._t, self._y, self._tout, self._outputs, self._keep = handle, y, tout, outputs, keep
+    def __init__(self, handle, result, keep=None):
+        self._t, self._result, self._keep = handle, result, keep
 
     def wait(self, timeout_s: float | None = None):
         check(lib.tfsc_predict_wait(self._t, -1 if timeout_s is None else int(timeout_s * 1e9)), "predict_wait")
-        if self._outputs is not None:
-            return Server._results(self._y, self._tout, self._outputs)
-        return Server._result(self._y, self._tout)
+        return self._result()
 
     def release(self):
         if self._t:
