@@ -360,6 +360,19 @@ int tfsc_k_depthwise_conv(const float* x, const float* w, const float* bias, flo
 /* Squeeze-and-excitation gate: y[b, p, ch] = x[b, p, ch] * gate[b, ch] over hw positions p. TFSC_E_INVALID unless
  * hw * c < 2^31. */
 int tfsc_k_channel_scale(const float* x, const float* gate, float* y, int batch, int hw, int c, void* stream);
+/* Swin Transformer building blocks (fp32, device, NHWC). Shifted-window multi-head attention: qkv[batch, h, w, 3c] (q | k | v
+ * of every token), ctx[batch, h, w, c], head width d = c / heads. The map is rolled by -shift on both axes and cut into
+ * window x window windows of N = window^2 tokens; within a window, score(i, j) = q_i . k_j / sqrt(d) + bias[head, i, j]
+ * (bias fp32 [heads, N, N], torchvision's relative_position_bias_table[relative_position_index]), plus -100 when shift > 0
+ * and i, j lie in different regions of torchvision's shift mask; ctx_i = softmax_j(score) . v. A window's bits depend
+ * neither on the batch nor on the alignment. TFSC_E_INVALID unless h and w are multiples of window, 1 <= window <= 16,
+ * 0 <= shift < window, d <= 64, K and V of a window fit in 48 KB ((2d + 1) N floats plus 4 (N + d)), h * w * 3c < 2^31 and
+ * every pointer is given. */
+int tfsc_k_window_attention(const float* qkv, const float* bias, float* ctx, int batch, int h, int w, int c, int heads, int window,
+                            int shift, void* stream);
+/* Patch merging: y[b, oy, ox, q*c + ch] = x[b, 2 oy + (q & 1), 2 ox + (q >> 1), ch], [h, w, c] -> [h/2, w/2, 4c] (torchvision's
+ * x0 | x1 | x2 | x3). TFSC_E_INVALID unless h and w are even, h * w * c < 2^31 and both pointers are given. */
+int tfsc_k_patch_merge(const float* x, float* y, int batch, int h, int w, int c, void* stream);
 /* X5 building blocks of the transformer graphs. Multi-head self-attention: qkv[batch, seq, 3*hidden] (q | k | v of every
  * token), ctx[batch, seq, hidden]; head width d = hidden / heads, scores scaled by 1/sqrt(d). ids[batch, seq] may be NULL;
  * a key whose id is 0 ([PAD]) gets the additive mask -10000 unless every key of its sequence is [PAD]. Every seq runs for

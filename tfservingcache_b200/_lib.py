@@ -137,6 +137,8 @@ _sig("tfsc_k_maxpool", C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_
 _sig("tfsc_k_avgpool", C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, vp)
 _sig("tfsc_k_depthwise_conv", C.c_int, vp, vp, vp, vp, *([C.c_int] * 9), vp)
 _sig("tfsc_k_channel_scale", C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp)
+_sig("tfsc_k_window_attention", C.c_int, vp, vp, vp, *([C.c_int] * 7), vp)
+_sig("tfsc_k_patch_merge", C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp)
 _sig("tfsc_k_attention", C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp)
 _sig("tfsc_k_attention_mask", C.c_int, vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp)
 _sig("tfsc_k_embed", C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp)

@@ -53,6 +53,14 @@ cudaError_t launch_depthwise_conv(const float* x, const float* w, const float* b
                                   int KW, int stride, int pad, int act, cudaStream_t s);
 // y[b, p, ch] = x[b, p, ch] * gate[b, ch] over HW positions p (the squeeze-and-excitation gate)
 cudaError_t launch_channel_scale(const float* x, const float* gate, float* y, int Bn, int HW, int C, cudaStream_t s);
+// Swin blocks (swin.cu). Shifted-window attention over the packed q | k | v [H, W, 3C] of each image, writing ctx [H, W, C]:
+// heads of d = C / heads columns, ws x ws windows of the map rolled by -shift, bias [heads, ws^2, ws^2] added to the
+// scores, -100 between tokens of different shift regions (shift > 0). cudaErrorInvalidValue outside
+// window_attention_supported (nn_limits.h) or for a null pointer.
+cudaError_t launch_window_attention(const float* qkv, const float* bias, float* ctx, int Bn, int H, int W, int C, int heads, int ws,
+                                    int shift, cudaStream_t s);
+// y[b, oy, ox, q*C + c] = x[b, 2oy + (q & 1), 2ox + (q >> 1), c] (patch merging), [H, W, C] -> [H/2, W/2, 4C]
+cudaError_t launch_patch_merge(const float* x, float* y, int Bn, int H, int W, int C, cudaStream_t s);
 // y = LayerNorm(x (+res)) or, with ids != nullptr, LayerNorm(word[id] + pos[s] + type[t]) (BERT embeddings): token
 // b*S + s reads ids[b*stride + s] and, unless types is nullptr (segment 0), t = clamp(types[b*stride + s], 0, 1)
 cudaError_t launch_layernorm(const float* x, const float* res, const int* ids, const int* types, int stride, const float* word,

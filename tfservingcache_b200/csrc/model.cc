@@ -630,6 +630,8 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       else if (kind == "mask_gather") o.kind = OpKind::MaskGather;
       else if (kind == "depthwise_conv") o.kind = OpKind::DepthwiseConv;
       else if (kind == "channel_scale") o.kind = OpKind::ChannelScale;
+      else if (kind == "window_attention") o.kind = OpKind::WindowAttention;
+      else if (kind == "patch_merge") o.kind = OpKind::PatchMerge;
       else {
         *err = "graph manifest: unknown op '" + kind + "'";
         return false;
@@ -652,8 +654,8 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         *err = "graph manifest: depthwise_conv act '" + act + "' is not none, relu, relu6, silu or sigmoid";
         return false;
       }
-      if (o.kind == OpKind::ChannelScale && act != "none") {
-        *err = "graph manifest: channel_scale takes no activation (act '" + act + "')";
+      if ((o.kind == OpKind::ChannelScale || o.kind == OpKind::WindowAttention || o.kind == OpKind::PatchMerge) && act != "none") {
+        *err = "graph manifest: " + kind + " takes no activation (act '" + act + "')";
         return false;
       }
       o.heads = (int)oj.get_int("heads", 1);
@@ -736,6 +738,69 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         }
         o.oh = (o.h + 2 * o.pad - o.kh) / o.stride + 1;
         o.ow = (o.w + 2 * o.pad - o.kw) / o.stride + 1;
+      } else if (o.kind == OpKind::WindowAttention) {
+        o.oh = o.h;
+        o.ow = o.w;
+        o.cout = o.c / 3;
+        o.window = (int)oj.get_int("window", 0);
+        o.shift = (int)oj.get_int("shift", 0);
+        o.b_off = (size_t)oj.get_int("bias_offset", 0);
+        const std::string at = " (h x w = " + std::to_string(o.h) + " x " + std::to_string(o.w) + ", window " + std::to_string(o.window);
+        if (o.c % 3) {
+          *err = "graph manifest: window_attention expects a packed [h, w, 3C] qkv source (c = " + std::to_string(o.c) + ")";
+          return false;
+        }
+        if (o.heads < 1 || o.cout % o.heads) {
+          *err = "graph manifest: window_attention needs heads that divide C = " + std::to_string(o.cout) + " (heads " +
+                 std::to_string(o.heads) + ")";
+          return false;
+        }
+        // torchvision zero-pads a map that is not a multiple of the window before the qkv projection, so its padded
+        // tokens are keys with k = the qkv bias: not served
+        if (o.window >= 1 && (o.h % o.window || o.w % o.window)) {
+          *err = "graph manifest: window_attention needs a feature map that is a multiple of the window" + at + ")";
+          return false;
+        }
+        if (o.window >= 1 && (o.shift < 0 || o.shift >= o.window)) {
+          *err = "graph manifest: window_attention shift " + std::to_string(o.shift) + " is outside [0, window)" + at + ")";
+          return false;
+        }
+        if (!window_attention_supported(o.h, o.w, o.cout, o.heads, o.window, o.shift)) {
+          *err = "graph manifest: no window_attention kernel for C = " + std::to_string(o.cout) + ", " + std::to_string(o.heads) +
+                 " heads" + at + ", shift " + std::to_string(o.shift) + ") (window <= " + std::to_string(kWindowMaxWs) +
+                 ", head width <= " + std::to_string(kWindowMaxD) + ", K and V of a window within 48 KB, h * w * 3C < 2^31)";
+          return false;
+        }
+        if (o.res != -100) {
+          *err = "graph manifest: window_attention takes no residual input";
+          return false;
+        }
+        const size_t n = (size_t)o.window * o.window;
+        if ((o.b_off & 255) || o.b_off + (size_t)o.heads * n * n * 4 > d->weights_bytes) {
+          *err = "graph manifest: window_attention bias table out of range or not 256-byte aligned";
+          return false;
+        }
+      } else if (o.kind == OpKind::PatchMerge) {
+        o.oh = o.h / 2;
+        o.ow = o.w / 2;
+        if (o.h % 2 || o.w % 2) {
+          *err = "graph manifest: patch_merge needs an even h and w (h x w = " + std::to_string(o.h) + " x " + std::to_string(o.w) + ")";
+          return false;
+        }
+        if (oj.get("cout") && o.cout != 4 * o.c) {
+          *err = "graph manifest: patch_merge writes 4c = " + std::to_string(4 * o.c) + " channels (cout " + std::to_string(o.cout) + ")";
+          return false;
+        }
+        o.cout = 4 * o.c;
+        if (o.res != -100) {
+          *err = "graph manifest: patch_merge takes no residual input";
+          return false;
+        }
+        if (!patch_merge_supported(o.h, o.w, o.c)) {
+          *err = "graph manifest: no patch_merge kernel for " + std::to_string(o.h) + " x " + std::to_string(o.w) + " x " +
+                 std::to_string(o.c) + " (h * w * c < 2^31)";
+          return false;
+        }
       } else if (o.kind == OpKind::Dense) {
         o.oh = o.ow = 1;
         o.kh = o.kw = 1;

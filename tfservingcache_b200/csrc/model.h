@@ -23,11 +23,16 @@ enum class Template { Affine, Mlp, Graph };
 // DepthwiseConv (MobileNet / EfficientNet): one kh x kw filter per channel, kernel [kh, kw, c] (TF's [kh, kw, c, 1]) at
 // w_off, bias [c] at b_off, cout = c. ChannelScale (squeeze-and-excitation): dst[b, p, ch] = src[b, p, ch] * gate[b, ch],
 // where `gate` is a scratch buffer an earlier op wrote with c values per image.
-enum class OpKind { Conv, MaxPool, AvgPool, Dense, Embed, LayerNorm, Attention, MaskGather, DepthwiseConv, ChannelScale };
+// WindowAttention (Swin): shifted-window multi-head attention from the packed q | k | v [h, w, c = 3C] to [h, w, C] in
+// window x window windows of the map rolled by -shift, with the relative-position bias expanded to fp32 [heads, N, N]
+// (N = window^2) at b_off. PatchMerge (Swin): [h, w, c] -> [h/2, w/2, 4c] in torchvision's x0 | x1 | x2 | x3 order.
+enum class OpKind { Conv, MaxPool, AvgPool, Dense, Embed, LayerNorm, Attention, MaskGather, DepthwiseConv, ChannelScale,
+                    WindowAttention, PatchMerge };
 struct GraphOp {
   OpKind kind = OpKind::Conv;
   int src = -1, dst = 0, res = -100;  // res = -100: no residual input
   int gate = -100;                    // ChannelScale: the buffer holding the [c] gate of each image
+  int window = 0, shift = 0;          // WindowAttention
   int h = 1, w = 1, c = 1;            // input H, W, C per image
   int kh = 1, kw = 1, stride = 1, pad = 0, cout = 1, oh = 1, ow = 1;
   int act = 0;                        // 0 none, 1 relu, 2 gelu(erf), 3 tanh, 4 relu6, 5 silu, 6 sigmoid

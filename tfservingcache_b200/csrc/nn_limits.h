@@ -65,4 +65,27 @@ inline bool depthwise_supported(int H, int W, int C, int KH, int KW, int stride,
          (long long)H * W * C <= 0x7fffffffLL;
 }
 
+// Shifted-window attention (swin.cu): one CTA per (image, window, head) stages K [N][d+1] and V [N][d] of its window
+// (N = ws^2 tokens) and a query row and a probability row per warp in shared memory, within the 48 KB a kernel gets without
+// opting in; a lane holds ceil(N / 32) <= 8 scores. ws = 7 and 12 at d = 32 (every torchvision Swin V1) fit, ws = 12 up to
+// d = 39, ws = 7 up to d = 64. C is the context width (the source holds 3C values per token); offsets within an image are
+// 32-bit (H * W * 3C < 2^31).
+constexpr int kWindowMaxWs = 16, kWindowMaxD = 64, kWindowWarps = 4;
+inline size_t window_attention_smem_bytes(int ws, int d) {
+  const size_t N = (size_t)ws * ws;
+  return (N * (2 * d + 1) + (size_t)kWindowWarps * (N + d)) * sizeof(float);
+}
+inline bool window_attention_supported(int H, int W, int C, int heads, int ws, int shift) {
+  if (H < 1 || W < 1 || C < 1 || heads < 1 || C % heads || ws < 1 || ws > kWindowMaxWs || H % ws || W % ws || shift < 0 ||
+      shift >= ws)
+    return false;
+  const int d = C / heads;
+  return d <= kWindowMaxD && window_attention_smem_bytes(ws, d) <= 48 * 1024 && (long long)H * W * 3 * C <= 0x7fffffffLL;
+}
+
+// Patch merging (swin.cu): a 2 x 2 space-to-depth gather, [h, w, c] -> [h/2, w/2, 4c]; offsets within an image are 32-bit.
+inline bool patch_merge_supported(int h, int w, int c) {
+  return h >= 2 && w >= 2 && h % 2 == 0 && w % 2 == 0 && c >= 1 && (long long)h * w * c <= 0x7fffffffLL;
+}
+
 }  // namespace tfsc

@@ -770,6 +770,10 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
                                   o.kh, o.kw, o.stride, o.pad, o.act, st);
       } else if (o.kind == OpKind::ChannelScale) {
         e = launch_channel_scale(src, (const float*)buf(o.gate), dst, B, o.h * o.w, o.c, st);
+      } else if (o.kind == OpKind::WindowAttention) {
+        e = launch_window_attention(src, (const float*)(dm.dptr + o.b_off), dst, B, o.h, o.w, o.cout, o.heads, o.window, o.shift, st);
+      } else if (o.kind == OpKind::PatchMerge) {
+        e = launch_patch_merge(src, dst, B, o.h, o.w, o.c, st);
       } else {
         e = launch_avgpool(src, dst, B, o.h * o.w, o.c, st);
       }

@@ -1738,6 +1738,23 @@ int tfsc_k_channel_scale(const float* x, const float* gate, float* y, int batch,
   cudaError_t e = launch_channel_scale(x, gate, y, batch, hw, c, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "channel_scale: %s", cudaGetErrorString(e));
 }
+int tfsc_k_window_attention(const float* qkv, const float* bias, float* ctx, int batch, int h, int w, int c, int heads, int window,
+                            int shift, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (!qkv || !bias || !ctx || batch < 0 || !window_attention_supported(h, w, c, heads, window, shift))
+    return fail(TFSC_E_INVALID, "window_attention: no kernel for batch %d, %d x %d, c %d, %d heads, window %d, shift %d (h, w multiples "
+                "of window <= %d, 0 <= shift < window, head width <= %d, K and V of a window within 48 KB, h * w * 3c < 2^31)",
+                batch, h, w, c, heads, window, shift, kWindowMaxWs, kWindowMaxD);
+  cudaError_t e = launch_window_attention(qkv, bias, ctx, batch, h, w, c, heads, window, shift, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "window_attention: %s", cudaGetErrorString(e));
+}
+int tfsc_k_patch_merge(const float* x, float* y, int batch, int h, int w, int c, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (!x || !y || batch < 0 || !patch_merge_supported(h, w, c))
+    return fail(TFSC_E_INVALID, "patch_merge: no kernel for batch %d, %d x %d x %d (even h and w, h * w * c < 2^31)", batch, h, w, c);
+  cudaError_t e = launch_patch_merge(x, y, batch, h, w, c, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "patch_merge: %s", cudaGetErrorString(e));
+}
 int tfsc_k_attention(const float* qkv, const int* ids, float* ctx, int batch, int seq, int hidden, int heads, void* stream) {
   if (int rc = check_device()) return rc;
   const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;

@@ -141,6 +141,8 @@ def _graph_manifest(input_shape, ops, n_buffers, input_name="x", output_name="y"
         elif op["op"] == "depthwise_conv":                  # kernel [kh, kw, c], bias [c]
             op["w_offset"] = take(op["kh"] * op["kw"] * op["c"] * 4)
             op["b_offset"] = take(op["c"] * 4)
+        elif op["op"] == "window_attention":                # relative-position bias expanded to [heads, N, N]
+            op["bias_offset"] = take(op["heads"] * op["window"] ** 4 * 4)
         elif op["op"] in ("layernorm", "embed"):
             op["w_offset"] = take(op["c"] * 4)      # gamma
             op["b_offset"] = take(op["c"] * 4)      # beta
@@ -274,6 +276,50 @@ def efficientnet_manifest(image=224, classes=1000, width_mult=1.0, depth_mult=1.
             ops.append(_conv(a, d, ho, exp, cout, res=cur if stride == 1 and cin == cout else None))
             cur, cin, h = d, cout, ho
     return _classifier(ops, cur, h, cin, 4 * cin, classes, "silu", 4, image, outputs)
+
+
+def swin_manifest(image=224, classes=1000, embed_dim=96, depths=(2, 2, 6, 2), heads=(3, 6, 12, 24), window=7, outputs=None):
+    """Swin Transformer V1 (Liu et al. 2021; torchvision's SwinTransformer topology) as a graph bundle, NHWC. The defaults
+    give swin_t; depths (2, 2, 18, 2) give swin_s, embed_dim 128 with heads (4, 8, 16, 32) swin_b. The stem is a 4x4 /
+    stride-4 conv and a LayerNorm. A block is LayerNorm, the qkv projection, window_attention (shifted by window // 2 in
+    every second block, unshifted where the window covers the whole map, as torchvision does), the output projection with
+    the block input as residual, LayerNorm, the MLP (4x, GELU) with the attention output as residual. Between stages,
+    patch_merge, LayerNorm(4C) and the bias-free reduction 4C -> 2C (a zero bias). The end is LayerNorm, the global average
+    pool and the dense classifier. Every Linear is a 1x1 conv over the h * w tokens ([h * w, 1, c]). Token maps must be
+    multiples of the window at every stage (no padding). Buffers: the block input and three others. outputs as for
+    resnet50_manifest."""
+    def ln(src, dst, n, c):
+        return {"op": "layernorm", "src": src, "dst": dst, "h": n, "w": 1, "c": c, "eps": 1e-5}
+
+    def linear(src, dst, n, c, cout, act="none", res=None):
+        o = {"op": "conv", "src": src, "dst": dst, "h": n, "w": 1, "c": c, "kh": 1, "kw": 1, "stride": 1, "pad": 0, "cout": cout,
+             "act": act}
+        if res is not None:
+            o["res"] = res
+        return o
+
+    h, c = image // 4, embed_dim
+    ops = [{"op": "conv", "src": -1, "dst": 0, "h": image, "w": image, "c": 3, "kh": 4, "kw": 4, "stride": 4, "pad": 0,
+            "cout": c, "act": "none"}, ln(0, 1, h * h, c)]
+    cur = 1
+    for stage, (depth, nh) in enumerate(zip(depths, heads)):
+        n = h * h
+        a, b, d = [x for x in range(4) if x != cur]
+        for i in range(depth):
+            shift = window // 2 if i % 2 == 1 and window < h else 0
+            ops += [ln(cur, a, n, c), linear(a, b, n, c, 3 * c),
+                    {"op": "window_attention", "src": b, "dst": a, "h": h, "w": h, "c": 3 * c, "heads": nh, "window": window,
+                     "shift": shift},
+                    linear(a, d, n, c, c, res=cur), ln(d, a, n, c), linear(a, b, n, c, 4 * c, act="gelu"),
+                    linear(b, cur, n, 4 * c, c, res=d)]
+        if stage + 1 < len(depths):
+            ops += [{"op": "patch_merge", "src": cur, "dst": a, "h": h, "w": h, "c": c}, ln(a, b, n // 4, 4 * c),
+                    linear(b, cur, n // 4, 4 * c, 2 * c)]
+            h, c = h // 2, 2 * c
+    a, b = [x for x in range(4) if x != cur][:2]
+    ops += [ln(cur, a, h * h, c), {"op": "avgpool", "src": a, "dst": b, "h": h, "w": h, "c": c},
+            {"op": "dense", "src": b, "dst": -2, "h": 1, "w": 1, "c": c, "cout": classes, "act": "none"}]
+    return _graph_manifest([image, image, 3], ops, 4, outputs=outputs)
 
 
 def write_graph_bundle(version_dir: str, manifest: dict, blob: np.ndarray):
