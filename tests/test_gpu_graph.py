@@ -22,8 +22,10 @@ def _err(got, ref):
 
 
 @pytest.mark.parametrize("m,n,k,lda", [(1, 8, 4, 4), (49, 64, 147, 148), (200, 100, 37, 37), (128, 64, 16, 16), (300, 1000, 2048, 2048),
-                                        (3136, 256, 64, 64), (130, 66, 18, 20)])
-@pytest.mark.parametrize("act", [0, 1, 2])
+                                        (3136, 256, 64, 64), (130, 66, 18, 20),
+                                        # BERT's pooler: token 0 of every sequence, lda = S*H
+                                        (64, 768, 768, 128 * 768), (65, 768, 768, 128 * 768), (130, 1024, 1024, 384 * 1024)])
+@pytest.mark.parametrize("act", [0, 1, 2, 3])
 def test_k_gemm(m, n, k, lda, act):
     torch = _torch()
     rng = np.random.default_rng(m * 7 + n + k + act)
@@ -40,11 +42,15 @@ def test_k_gemm(m, n, k, lda, act):
         ref = np.maximum(ref, 0)
     elif act == 2:
         ref = torch.nn.functional.gelu(torch.from_numpy(ref)).numpy()
+    elif act == 3:
+        ref = np.tanh(ref)
     assert _err(cd.cpu().numpy(), ref) <= TOL
 
 
 @pytest.mark.parametrize("m,n,k,lda", [(128, 128, 32, 32), (64, 64, 64, 64), (300, 256, 96, 96), (3136, 64, 147, 148), (1024, 768, 768, 768),
-                                        (1000, 3072, 768, 768), (512, 768, 3072, 3072), (6272, 128, 1152, 1152), (130, 96, 40, 44)])
+                                        (1000, 3072, 768, 768), (512, 768, 3072, 3072), (6272, 128, 1152, 1152), (130, 96, 40, 44),
+                                        # BERT's pooler: token 0 of every sequence, lda = S*H (a TMA row stride of S*H*4 bytes)
+                                        (64, 768, 768, 128 * 768), (65, 768, 768, 128 * 768), (130, 1024, 1024, 384 * 1024)])
 @pytest.mark.parametrize("act", [0, 1, 2, 3])
 def test_k_gemm_tc_matches_oracle(m, n, k, lda, act):
     """wgmma 3xTF32 GEMM (gemm_tc.cu) vs fp64; bias + residual + activation fused in the epilogue."""

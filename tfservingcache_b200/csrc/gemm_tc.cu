@@ -391,21 +391,32 @@ cudaError_t launch_gemm_tc(const float* A, const float* B, const float* bias, co
   EncodeTiledFn enc = tc_encode_fn();
   if (!enc) return cudaErrorNotSupported;
   const int BN = pick_bn(M, N);
-  CUtensorMap am, bm;
-  if (!cached_map({A, M, K, lda}, [&](CUtensorMap* m) {
-        const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)M};
-        const cuuint64_t gstride[1] = {(cuuint64_t)lda * 4};
-        const cuuint32_t box[2] = {(cuuint32_t)gt::BK, (cuuint32_t)gt::BM};
-        const cuuint32_t estr[2] = {1, 1};
-        return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(A), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-      }, &am))
-    return cudaErrorInvalidValue;
-  if (!weight_map(B, K, N, BN, &bm)) return cudaErrorInvalidValue;
-  const ConvGeom none{};
-  return BN == 128 ? launch_gt<128, false>(am, bm, bias, R, C, M, N, K, act, none, s)
-                   : launch_gt<64, false>(am, bm, bias, R, C, M, N, K, act, none, s);
+  // gridDim.y (one CTA row per 128 rows) is capped at 65,535: a taller A runs as consecutive launches over row chunks,
+  // each with its own A map (the map cache is keyed by base pointer); one launch below the cap, as before
+  constexpr int chunk_rows = kMaxGridY * gt::BM;
+  for (int r0 = 0; r0 < M; r0 += chunk_rows) {
+    const int rows = M - r0 < chunk_rows ? M - r0 : chunk_rows;
+    const float* a = A + (size_t)r0 * lda;
+    CUtensorMap am, bm;
+    if (!cached_map({a, rows, K, lda}, [&](CUtensorMap* m) {
+          const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
+          const cuuint64_t gstride[1] = {(cuuint64_t)lda * 4};
+          const cuuint32_t box[2] = {(cuuint32_t)gt::BK, (cuuint32_t)gt::BM};
+          const cuuint32_t estr[2] = {1, 1};
+          return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(a), gdim, gstride, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+        }, &am))
+      return cudaErrorInvalidValue;
+    if (!weight_map(B, K, N, BN, &bm)) return cudaErrorInvalidValue;
+    const ConvGeom none{};
+    const float* r = R ? R + (size_t)r0 * N : nullptr;
+    float* c = C + (size_t)r0 * N;
+    const cudaError_t e = BN == 128 ? launch_gt<128, false>(am, bm, bias, r, c, rows, N, K, act, none, s)
+                                    : launch_gt<64, false>(am, bm, bias, r, c, rows, N, K, act, none, s);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 // ---- implicit-GEMM convolution: NHWC activations x HWIO kernel, A tiles gathered by TMA im2col (no col buffer) ----
@@ -437,25 +448,37 @@ cudaError_t launch_conv_tc(const float* x, const float* w, const float* bias, co
   if (!enc) return cudaErrorNotSupported;
   const int M = Bn * OH * OW, K = KH * KW * C;
   const int BN = pick_bn(M, N);
-  CUtensorMap am, bm;
-  if (!cached_map({x, ((int64_t)Bn << 40) | ((int64_t)H << 20) | W, ((int64_t)C << 32) | (KH << 16) | KW, ((int64_t)stride << 8) | pad},
-                  [&](CUtensorMap* m) {
-        const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)Bn};
-        const cuuint64_t gstride[3] = {(cuuint64_t)C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4};
-        // base pixels (top-left corner of the filter window, input space) range over [-pad, dim + pad - K] per axis,
-        // visited with the conv stride; tap offsets {kw, kh} are added per load
-        const int lower[2] = {-pad, -pad};
-        const int upper[2] = {pad - (KW - 1), pad - (KH - 1)};
-        const cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
-        return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(x), gdim, gstride, lower, upper, (cuuint32_t)gt::BK,
-                   (cuuint32_t)gt::BM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-      }, &am))
-    return cudaErrorInvalidValue;
-  if (!weight_map(w, K, N, BN, &bm)) return cudaErrorInvalidValue;
-  const ConvGeom cg{C, KW, OH, OW, stride, pad};
-  return BN == 128 ? launch_gt<128, true>(am, bm, bias, R, y, M, N, K, act, cg, s)
-                   : launch_gt<64, true>(am, bm, bias, R, y, M, N, K, act, cg, s);
+  // gridDim.y (one CTA row per 128 output pixels) is capped at 65,535: a larger batch runs as consecutive launches over
+  // whole images, each with an im2col map over its own images; one launch below the cap, as before
+  const int per_img = OH * OW;
+  const int chunk = kMaxGridY * gt::BM / per_img > 0 ? kMaxGridY * gt::BM / per_img : 1;
+  for (int b0 = 0; b0 < Bn; b0 += chunk) {
+    const int nb = Bn - b0 < chunk ? Bn - b0 : chunk;
+    const float* xc = x + (size_t)b0 * H * W * C;
+    CUtensorMap am, bm;
+    if (!cached_map({xc, ((int64_t)nb << 40) | ((int64_t)H << 20) | W, ((int64_t)C << 32) | (KH << 16) | KW, ((int64_t)stride << 8) | pad},
+                    [&](CUtensorMap* m) {
+          const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)nb};
+          const cuuint64_t gstride[3] = {(cuuint64_t)C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4};
+          // base pixels (top-left corner of the filter window, input space) range over [-pad, dim + pad - K] per axis,
+          // visited with the conv stride; tap offsets {kw, kh} are added per load
+          const int lower[2] = {-pad, -pad};
+          const int upper[2] = {pad - (KW - 1), pad - (KH - 1)};
+          const cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
+          return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(xc), gdim, gstride, lower, upper, (cuuint32_t)gt::BK,
+                     (cuuint32_t)gt::BM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+        }, &am))
+      return cudaErrorInvalidValue;
+    if (!weight_map(w, K, N, BN, &bm)) return cudaErrorInvalidValue;
+    const ConvGeom cg{C, KW, OH, OW, stride, pad};
+    const size_t out0 = (size_t)b0 * per_img * N;
+    const float* r = R ? R + out0 : nullptr;
+    const cudaError_t e = BN == 128 ? launch_gt<128, true>(am, bm, bias, r, y + out0, nb * per_img, N, K, act, cg, s)
+                                    : launch_gt<64, true>(am, bm, bias, r, y + out0, nb * per_img, N, K, act, cg, s);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
 }
 
 }  // namespace tfsc

@@ -145,18 +145,18 @@ static bool gemm_tc_enabled() {  // TFSC_GEMM_TC=0 forces the CUDA-core GEMM
   return v != 0;
 }
 
+// The SIMT kernel's launcher is defined at the end of this file, after every kernel: with -lineinfo a kernel's source
+// lines reach ptxas, and host code above the kernels that changes their line numbers can change their register
+// allocation (attention_tile_kernel<8>) without changing what they compute.
+static cudaError_t launch_gemm_f32(const float* A, const float* B, const float* bias, const float* R, float* C, int M, int N,
+                                   int K, int lda, int act, cudaStream_t s);
+
 cudaError_t launch_gemm(const float* A, const float* B, const float* bias, const float* R, float* C, int M, int N, int K,
                         int lda, int act, cudaStream_t s) {
   if (M <= 0 || N <= 0) return cudaSuccess;
   if (gemm_tc_enabled() && gemm_tc_supported(A, B, bias, R, C, M, N, K, lda))
     return launch_gemm_tc(A, B, bias, R, C, M, N, K, lda, act, s);
-  dim3 grid((N + GBN - 1) / GBN, (M + GBM - 1) / GBM);
-  const bool vec = (lda % 4 == 0) && (N % 4 == 0) && ((reinterpret_cast<uintptr_t>(A) & 15) == 0) &&
-                   ((reinterpret_cast<uintptr_t>(B) & 15) == 0);
-  if (vec) gemm_f32_kernel<true><<<grid, GTHREADS, 0, s>>>(A, B, bias, R, C, M, N, K, lda, act);
-  else gemm_f32_kernel<false><<<grid, GTHREADS, 0, s>>>(A, B, bias, R, C, M, N, K, lda, act);
-  g_launches_nn++;
-  return cudaGetLastError();
+  return launch_gemm_f32(A, B, bias, R, C, M, N, K, lda, act, s);
 }
 
 // ----------------------------------------------------------------------------------- im2col ----
@@ -719,11 +719,22 @@ cudaError_t launch_attention(const float* qkv, const int* mask, int mask_stride,
   const int d = H / heads;
   if (d % 4 == 0 && H % 4 == 0 && al && d <= 128) {
     const int kpl = (S + 31) / 32;
-    if (kpl <= 1 && attention_tile_smem(S, d, 1) <= kAttnSmemCap) return launch_attention_tile<1>(qkv, mask, mask_stride, ctx, Bn, S, H, heads, s);
-    if (kpl <= 2 && attention_tile_smem(S, d, 2) <= kAttnSmemCap) return launch_attention_tile<2>(qkv, mask, mask_stride, ctx, Bn, S, H, heads, s);
-    if (kpl <= 4 && attention_tile_smem(S, d, 4) <= kAttnSmemCap) return launch_attention_tile<4>(qkv, mask, mask_stride, ctx, Bn, S, H, heads, s);
-    if (kpl <= 8 && attention_tile_smem(S, d, 8) <= kAttnSmemCap) return launch_attention_tile<8>(qkv, mask, mask_stride, ctx, Bn, S, H, heads, s);
-    return launch_attention_keyblock(qkv, mask, mask_stride, ctx, Bn, S, H, heads, s);
+    // gridDim.y = sequences x heads is capped at 65,535: more sequences run as consecutive launches; one launch below the cap
+    const int chunk = heads < kMaxGridY ? kMaxGridY / heads : 1;
+    for (int b0 = 0; b0 < Bn; b0 += chunk) {
+      const int nb = Bn - b0 < chunk ? Bn - b0 : chunk;
+      const float* q = qkv + (size_t)b0 * S * 3 * H;
+      const int* m = mask ? mask + (size_t)b0 * mask_stride : nullptr;
+      float* c = ctx + (size_t)b0 * S * H;
+      cudaError_t e;
+      if (kpl <= 1 && attention_tile_smem(S, d, 1) <= kAttnSmemCap) e = launch_attention_tile<1>(q, m, mask_stride, c, nb, S, H, heads, s);
+      else if (kpl <= 2 && attention_tile_smem(S, d, 2) <= kAttnSmemCap) e = launch_attention_tile<2>(q, m, mask_stride, c, nb, S, H, heads, s);
+      else if (kpl <= 4 && attention_tile_smem(S, d, 4) <= kAttnSmemCap) e = launch_attention_tile<4>(q, m, mask_stride, c, nb, S, H, heads, s);
+      else if (kpl <= 8 && attention_tile_smem(S, d, 8) <= kAttnSmemCap) e = launch_attention_tile<8>(q, m, mask_stride, c, nb, S, H, heads, s);
+      else e = launch_attention_keyblock(q, m, mask_stride, c, nb, S, H, heads, s);
+      if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
   }
   const size_t smem = attention_smem_bytes(S, H, heads);
   static bool attr[64] = {};
@@ -792,6 +803,28 @@ cudaError_t launch_copy_segments(const CopySeg* segs, int n, cudaStream_t s) {
     copy_segments_kernel<<<dim3((unsigned)chunks, (unsigned)m), 256, 0, s>>>(tab);
     g_launches_nn++;
     cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
+}
+
+// gridDim.y (one CTA row per 128 rows) is capped at 65,535: a taller A runs as consecutive launches over row chunks; one
+// launch below the cap
+static cudaError_t launch_gemm_f32(const float* A, const float* B, const float* bias, const float* R, float* C, int M, int N,
+                                   int K, int lda, int act, cudaStream_t s) {
+  const bool vec = (lda % 4 == 0) && (N % 4 == 0) && ((reinterpret_cast<uintptr_t>(A) & 15) == 0) &&
+                   ((reinterpret_cast<uintptr_t>(B) & 15) == 0);
+  constexpr int chunk_rows = kMaxGridY * GBM;
+  for (int r0 = 0; r0 < M; r0 += chunk_rows) {
+    const int rows = M - r0 < chunk_rows ? M - r0 : chunk_rows;
+    const float* a = A + (size_t)r0 * lda;
+    const float* r = R ? R + (size_t)r0 * N : nullptr;
+    float* c = C + (size_t)r0 * N;
+    dim3 grid((N + GBN - 1) / GBN, (rows + GBM - 1) / GBM);
+    if (vec) gemm_f32_kernel<true><<<grid, GTHREADS, 0, s>>>(a, B, bias, r, c, rows, N, K, lda, act);
+    else gemm_f32_kernel<false><<<grid, GTHREADS, 0, s>>>(a, B, bias, r, c, rows, N, K, lda, act);
+    g_launches_nn++;
+    const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
   }
   return cudaSuccess;

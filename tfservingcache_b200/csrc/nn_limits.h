@@ -7,6 +7,9 @@ namespace tfsc {
 
 constexpr size_t kAttnSmemCap = 200 * 1024;  // dynamic shared memory the attention kernels opt in to
 
+// CUDA's cap on gridDim.y (and z). Launchers whose y extent grows with the batch split the batch on the host above it.
+constexpr int kMaxGridY = 65535;
+
 // row-at-a-time attention kernel: K [S][d+1], V [S][d], P [8][S], Q [8][d] and the mask [S] of one head
 inline size_t attention_smem_bytes(int S, int H, int heads) {
   const int d = H / heads;

@@ -1758,7 +1758,7 @@ int tfsc_k_patch_merge(const float* x, float* y, int batch, int h, int w, int c,
 int tfsc_k_attention(const float* qkv, const int* ids, float* ctx, int batch, int seq, int hidden, int heads, void* stream) {
   if (int rc = check_device()) return rc;
   const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;
-  if (!qkv || !ctx || batch < 1 || (int64_t)batch * heads > 65535 || !attention_supported(seq, hidden, heads, al))
+  if (!qkv || !ctx || batch < 1 || (int64_t)batch * heads > 0x7fffffff || !attention_supported(seq, hidden, heads, al))
     return fail(TFSC_E_INVALID, "attention: no kernel for batch %d, seq %d, hidden %d, heads %d", batch, seq, hidden, heads);
   cudaError_t e = launch_attention(qkv, ids, seq, ctx, batch, seq, hidden, heads, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "attention: %s", cudaGetErrorString(e));
@@ -1767,7 +1767,7 @@ int tfsc_k_attention_mask(const float* qkv, const int* mask, int mask_stride, fl
                           void* stream) {
   if (int rc = check_device()) return rc;
   const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;
-  if (!qkv || !ctx || batch < 1 || (int64_t)batch * heads > 65535 || !attention_supported(seq, hidden, heads, al))
+  if (!qkv || !ctx || batch < 1 || (int64_t)batch * heads > 0x7fffffff || !attention_supported(seq, hidden, heads, al))
     return fail(TFSC_E_INVALID, "attention_mask: no kernel for batch %d, seq %d, hidden %d, heads %d", batch, seq, hidden, heads);
   if (mask && mask_stride < seq) return fail(TFSC_E_INVALID, "attention_mask: mask_stride %d is below seq %d", mask_stride, seq);
   cudaError_t e = launch_attention(qkv, mask, mask_stride, ctx, batch, seq, hidden, heads, (cudaStream_t)stream);
