@@ -328,8 +328,8 @@ typedef struct tfsc_copy_seg {
 int tfsc_k_copy_segments(const tfsc_copy_seg* segs, int n, void* stream);
 
 /* X4/X5 building blocks of the graph executor (conv nets), fp32, row-major / NHWC. act: 0 none, 1 relu, 2 gelu, 3 tanh,
- * 4 relu6 (min(max(x, 0), 6)), 5 silu (x / (1 + exp(-x))), 6 sigmoid (1 / (1 + exp(-x))); the same on tfsc_k_gemm_tc and
- * tfsc_k_conv_tc.
+ * 4 relu6 (min(max(x, 0), 6)), 5 silu (x / (1 + exp(-x))), 6 sigmoid (1 / (1 + exp(-x))), 7 gelu_tanh (0.5 x (1 + tanh(
+ * sqrt(2 / pi) (x + 0.044715 x^3))), GPT-2's GELU); the same on tfsc_k_gemm_tc and tfsc_k_conv_tc.
  * C[M,N] = act(A[M,K] (row stride lda) * B[K,N] + bias[N] (+ R[M,N])); bias / R may be NULL. */
 int tfsc_k_gemm(const float* a, const float* b, const float* bias, const float* r, float* c, int m, int n, int k, int lda,
                 int act, void* stream);
@@ -441,6 +441,28 @@ int tfsc_k_mask_gather(const float* hidden, const int32_t* ids, const int32_t* m
  * given. */
 int tfsc_k_fill_mask_head(const float* logits, int64_t ld, const int32_t* positions, int rows, int slots, int vocab, int k,
                           int32_t* top_ids, float* top_probs, float* top_logits, void* stream);
+/* GPT-2 building blocks (fp32, device). Causal multi-head self-attention: as tfsc_k_attention_mask, but query i of a sequence
+ * sees keys j <= i only; a key it cannot see gets exactly zero weight. mask may be NULL (no key masked by it); a key whose
+ * mask is 0 is masked by the same rule as tfsc_k_attention_mask. TFSC_E_INVALID unless d = hidden / heads has d % 4 == 0
+ * and d <= 128, qkv and ctx are 16-byte aligned, and mask_stride >= seq for a mask. */
+int tfsc_k_attention_causal(const float* qkv, const int* mask, int mask_stride, float* ctx, int batch, int seq, int hidden, int heads,
+                            void* stream);
+/* Embedding without LayerNorm: y[b*seq + s] = word[id] + pos[s] (one fp32 add) with id = ids[b*stride + s] clamped to
+ * 0..vocab-1; word[vocab, hidden], pos[>= seq, hidden]. TFSC_E_INVALID for stride < seq or a null pointer. */
+int tfsc_k_embed_positions(const int32_t* ids, int stride, const float* word, const float* pos, float* y, int batch, int seq,
+                           int hidden, int vocab, void* stream);
+/* Last attended token of rows of hidden states hidden[rows, S, H]: p = the highest position with mask[r * stride + p] != 0
+ * (mask NULL: S - 1; no such position: -1). positions[r] = p (int32) and gathered[r, :] = hidden[r, p, :] (a bit-exact
+ * copy; zeros for p = -1). Either output may be NULL. TFSC_E_INVALID for stride < S with a mask, or gathered without
+ * hidden. */
+int tfsc_k_last_token(const float* hidden, const int32_t* mask, int stride, int rows, int S, int H, int32_t* positions,
+                      float* gathered, void* stream);
+/* Next-token head: tfsc_k_fill_mask_head with one slot per row (row r reads logits + r * ld and positions[r]) and a vocabulary
+ * of up to 57344. Outputs are [rows, k]; at vocab <= 32768 they carry the bits tfsc_k_fill_mask_head gives on the same logits.
+ * TFSC_E_INVALID unless 1 <= vocab <= 57344 and 1 <= k <= min(vocab, 32), and positions, and logits for a top-k output, are
+ * given. */
+int tfsc_k_next_token_head(const float* logits, int64_t ld, const int32_t* positions, int rows, int vocab, int k, int32_t* top_ids,
+                           float* top_probs, float* top_logits, void* stream);
 
 #ifdef __cplusplus
 }

@@ -148,6 +148,10 @@ _sig("tfsc_k_span_head", C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c
 _sig("tfsc_k_encoder_head", C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp)
 _sig("tfsc_k_mask_gather", C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp)
 _sig("tfsc_k_fill_mask_head", C.c_int, vp, C.c_int64, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp)
+_sig("tfsc_k_attention_causal", C.c_int, vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp)
+_sig("tfsc_k_embed_positions", C.c_int, vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp)
+_sig("tfsc_k_last_token", C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp)
+_sig("tfsc_k_next_token_head", C.c_int, vp, C.c_int64, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp)
 
 
 class TfscError(RuntimeError):

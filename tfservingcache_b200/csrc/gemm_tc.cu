@@ -86,6 +86,7 @@ __device__ __noinline__ float4 act_call4(float4 v, int act) {
   if (act == 4) return make_float4(relu6f(v.x), relu6f(v.y), relu6f(v.z), relu6f(v.w));
   if (act == 5) return make_float4(siluf(v.x), siluf(v.y), siluf(v.z), siluf(v.w));
   if (act == 6) return make_float4(sigmoidf(v.x), sigmoidf(v.y), sigmoidf(v.z), sigmoidf(v.w));
+  if (act == 7) return make_float4(gelu_tanhf(v.x), gelu_tanhf(v.y), gelu_tanhf(v.z), gelu_tanhf(v.w));
   return v;
 }
 __device__ __forceinline__ float4 apply_act_rt(float4 v, int act) {

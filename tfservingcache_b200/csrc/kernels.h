@@ -38,7 +38,8 @@ cudaError_t launch_dense_cluster(const float* x, const float* w, const float* bi
 // grid of the cluster kernel on the current device: co-resident 2-CTA clusters and the strip width chosen for n columns
 cudaError_t dense_cluster_grid(int rows, int n, int* active_clusters, int* strip_cols);
 
-// X4/X5 building blocks (nn_kernels.cu): act 0 none / 1 relu / 2 gelu(erf) / 3 tanh / 4 relu6 / 5 silu / 6 sigmoid
+// X4/X5 building blocks (nn_kernels.cu): act 0 none / 1 relu / 2 gelu(erf) / 3 tanh / 4 relu6 / 5 silu / 6 sigmoid /
+// 7 gelu_tanh
 cudaError_t launch_gemm(const float* A, const float* B, const float* bias, const float* R, float* C, int M, int N, int K,
                         int lda, int act, cudaStream_t s);
 cudaError_t launch_im2col(const float* x, float* col, int Bn, int H, int W, int C, int KH, int KW, int stride, int pad,
@@ -71,6 +72,10 @@ cudaError_t launch_layernorm(const float* x, const float* res, const int* ids, c
 // Both launchers return cudaErrorInvalidValue for shapes outside attention_supported / layernorm_supported (nn_limits.h).
 cudaError_t launch_attention(const float* qkv, const int* mask, int mask_stride, float* ctx, int Bn, int S, int H, int heads,
                              cudaStream_t s);
+// The same under the causal rule: query i sees keys j <= i, a hidden key gets exactly zero weight, and the mask (may be
+// nullptr) hides keys as above. cudaErrorInvalidValue outside attention_causal_supported (nn_limits.h).
+cudaError_t launch_attention_causal(const float* qkv, const int* mask, int mask_stride, float* ctx, int Bn, int S, int H, int heads,
+                                    cudaStream_t s);
 
 // Classification head (head.cu): from logits[rows, n] writes, for each non-null pointer, row r of that output at
 // ptr + r * ld (ld in 32-bit words): a copy of the logits [n], softmax probabilities [n], the argmax class as a
@@ -167,8 +172,18 @@ struct FillMaskOutputs {
   float* logits = nullptr;
   int64_t logits_ld = 0;
 };
+// max_vocab is the cap to check: kHeadMaxN (fill_mask_supported), or kNextTokenMaxVocab with M = 1 (next_token_supported).
 cudaError_t launch_fill_mask_head(const float* logits, int64_t ld, const int* positions, int rows, int M, int vocab, int k,
-                                  const FillMaskOutputs& o, cudaStream_t s);
+                                  int max_vocab, const FillMaskOutputs& o, cudaStream_t s);
+
+// GPT-2 (gpt2.cu). Embedding without LayerNorm: y[b*S + s, :] = word[id, :] + pos[s, :], id = ids[b*stride + s] clamped to
+// 0..vocab-1, one fp32 add. cudaErrorInvalidValue for stride < S or a null pointer.
+cudaError_t launch_embed_positions(const int* ids, int64_t stride, const float* word, const float* pos, float* y, int rows, int S,
+                                   int H, int vocab, cudaStream_t s);
+// Last attended token: p = the largest position with mask[r*stride + p] != 0 (mask nullptr: S - 1; none: -1);
+// positions[r] = p and gathered[r, :] = hidden[r, p, :] (a bit-exact copy; zeros for p = -1). Either output may be nullptr.
+cudaError_t launch_last_token(const float* hidden, const int* mask, int64_t stride, int rows, int S, int H, int* positions,
+                              float* gathered, cudaStream_t s);
 
 // wgmma 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
 bool gemm_tc_supported(const float* A, const float* B, const float* bias, const float* R, const float* C, int M, int N, int K,

@@ -159,16 +159,20 @@ __global__ void __launch_bounds__(kHeadThreadsMax) fill_mask_head_kernel(const f
 }
 
 cudaError_t launch_fill_mask_head(const float* logits, int64_t ld, const int* positions, int rows, int M, int vocab, int k,
-                                  const FillMaskOutputs& o, cudaStream_t s) {
+                                  int max_vocab, const FillMaskOutputs& o, cudaStream_t s) {
   const bool topk = o.ids || o.probs || o.logits;
-  if (!fill_mask_supported(M, vocab, topk ? k : 1) || rows < 0 || !positions || (topk && (!logits || ld < vocab)))
-    return cudaErrorInvalidValue;
+  // max_vocab: kHeadMaxN for fill-mask bundles (fill_mask_supported), kNextTokenMaxVocab for the next-token head's one slot
+  const bool shape_ok = max_vocab == kNextTokenMaxVocab ? M == 1 && next_token_supported(vocab, topk ? k : 1)
+                                                         : max_vocab == kHeadMaxN && fill_mask_supported(M, vocab, topk ? k : 1);
+  if (!shape_ok || rows < 0 || !positions || (topk && (!logits || ld < vocab))) return cudaErrorInvalidValue;
   if (rows == 0) return cudaSuccess;
   static bool attr[64] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   if (!attr[dev & 63]) {
-    cudaError_t e = cudaFuncSetAttribute(fill_mask_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kHeadMaxN * (int)sizeof(float));
+    // the largest row either head stages; the opt-in permits more shared memory and changes no launch's code
+    cudaError_t e = cudaFuncSetAttribute(fill_mask_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         kNextTokenMaxVocab * (int)sizeof(float));
     if (e != cudaSuccess) return e;
     attr[dev & 63] = true;
   }

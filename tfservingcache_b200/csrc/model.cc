@@ -16,9 +16,10 @@ size_t ModelDesc::scratch_bytes(int64_t rows) const {
   if (tmpl == Template::Graph) {
     size_t last = 1;
     for (auto v : output_shape) last *= (size_t)v;
-    // a fill-mask bundle's int32 [rows, M] positions follow the head's logits
+    // a fill-mask bundle's int32 [rows, M] positions follow the head's logits, a next-token bundle's [rows]
     return head_scratch_offset(rows) + (outputs.empty() ? 0 : align256((size_t)rows * last * 4)) +
-           (head == HeadKind::FillMask ? align256((size_t)rows * (size_t)head_n * 4) : 0);
+           (head == HeadKind::FillMask ? align256((size_t)rows * (size_t)head_n * 4) : 0) +
+           (head == HeadKind::NextToken ? align256((size_t)rows * 4) : 0);
   }
   return 256;
 }
@@ -36,9 +37,9 @@ size_t ModelDesc::mlm_positions_offset(int64_t rows) const {
 }
 
 // ------------------------------------------------------------------------------------------------ output kinds ----
-// A row of an output kind in the bundle's head_n / head_k (ModelDesc): one int64 scalar (2 words), a vector of head_n or
-// head_k values, or a head_k x head_n / head_n x head_k matrix
-enum class Rows { Int64, N, K, KxN, NxK };
+// A row of an output kind in the bundle's head_n / head_k (ModelDesc): one int64 scalar (2 words), one 32-bit scalar, a
+// vector of head_n or head_k values, or a head_k x head_n / head_n x head_k matrix
+enum class Rows { Int64, One, N, K, KxN, NxK };
 // The entry fields a kind takes besides name and kind: "k"; "k", "max_answer_length" and "sep_id"; or "normalize"
 enum class Fields { None, K, Span, Normalize };
 struct OutputKindInfo {
@@ -68,6 +69,10 @@ static constexpr OutputKindInfo kOutputKinds[] = {
     {"masked_top_k_ids", HeadKind::FillMask, TFSC_DT_INT32, Rows::NxK, Fields::K},
     {"masked_top_k_probabilities", HeadKind::FillMask, TFSC_DT_FLOAT, Rows::NxK, Fields::K},
     {"masked_top_k_logits", HeadKind::FillMask, TFSC_DT_FLOAT, Rows::NxK, Fields::K},
+    {"next_token_position", HeadKind::NextToken, TFSC_DT_INT32, Rows::One, Fields::None},
+    {"next_token_top_k_ids", HeadKind::NextToken, TFSC_DT_INT32, Rows::K, Fields::K},
+    {"next_token_top_k_probabilities", HeadKind::NextToken, TFSC_DT_FLOAT, Rows::K, Fields::K},
+    {"next_token_top_k_logits", HeadKind::NextToken, TFSC_DT_FLOAT, Rows::K, Fields::K},
 };
 static_assert(sizeof(kOutputKinds) / sizeof(kOutputKinds[0]) == (size_t)kLastOutputKind + 1, "one row per OutputKind");
 
@@ -82,6 +87,7 @@ OutputForm output_form(OutputKind k, int head_n, int head_k) {
   f.dtype = kind_info(k).dtype;
   switch (kind_info(k).rows) {
     case Rows::Int64: f.width = 2, f.rank = 0, f.dims[0] = 1; break;
+    case Rows::One: f.width = 1, f.rank = 0, f.dims[0] = 1; break;
     case Rows::N: f.width = f.dims[0] = head_n; break;
     case Rows::K: f.width = f.dims[0] = head_k; break;
     case Rows::KxN: f.rank = 2, f.dims[0] = head_k, f.dims[1] = head_n, f.width = (int64_t)head_k * head_n; break;
@@ -104,6 +110,10 @@ static bool declares_k(const ModelDesc& d) {
 static bool classify_fits(int n, int k, bool with_k) { return head_supported(n, with_k ? k : 1) && (with_k || k == 0); }
 static bool span_fits(int S, int L, int k, bool with_k) { return span_supported(S, with_k ? L : 1, with_k ? k : 1) && (with_k || k == 0); }
 static bool fill_mask_fits(int M, int V, int k, bool with_k) { return fill_mask_supported(M, V, with_k ? k : 1) && (with_k || k == 0); }
+static bool next_token_fits(int V, int k, bool with_k) { return next_token_supported(V, with_k ? k : 1) && (with_k || k == 0); }
+static std::string next_token_limits() {
+  return "1 <= vocab <= " + std::to_string(kNextTokenMaxVocab) + ", 1 <= k <= min(vocab, " + std::to_string(kHeadMaxK) + ")";
+}
 static bool encoder_fits(int S, int H, std::string* err) {
   if (encoder_head_supported(S, H)) return true;
   *err = "signature.outputs: no encoder head kernel for S = " + std::to_string(S) + " and H = " + std::to_string(H) +
@@ -115,6 +125,13 @@ bool layout_outputs(ModelDesc* d, std::string* err) {
   set_head(d);
   const bool with_k = declares_k(*d);
   switch (d->head) {
+    case HeadKind::NextToken:
+      if (!next_token_fits(d->head_n, d->head_k, with_k)) {
+        *err = "signature.outputs: no next-token head for vocab = " + std::to_string(d->head_n) + " and k = " +
+               std::to_string(d->head_k) + " (" + next_token_limits() + ")";
+        return false;
+      }
+      break;
     case HeadKind::FillMask:  // vocab is the owner's business, so only M and k decide whether a row can be laid out
       if (!fill_mask_fits(d->head_n, kHeadMaxN, d->head_k, with_k)) {
         *err = "signature.outputs: no fill-mask head for M = " + std::to_string(d->head_n) + " slots and k = " +
@@ -236,9 +253,12 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
     const OutputKindInfo* ki = nullptr;
     for (auto& i : kOutputKinds)
       if (kind == i.name) ki = &i;
-    if (!ki) {
-      *err = "signature.outputs: unknown kind '" + kind + "' (";
-      for (auto& i : kOutputKinds) *err += std::string(&i == kOutputKinds ? "" : ", ") + i.name;
+    if (!ki) {  // a name that starts with next_token is told the next-token kinds, any other the kinds of the other heads
+      const bool next = kind.rfind("next_token", 0) == 0;
+      *err = "signature.outputs: unknown " + std::string(next ? "next-token " : "") + "kind '" + kind + "' (";
+      bool any = false;
+      for (auto& i : kOutputKinds)
+        if ((i.head == HeadKind::NextToken) == next) *err += std::string(any ? ", " : "") + i.name, any = true;
       *err += ")";
       return false;
     }
@@ -254,12 +274,17 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
       }
     const HeadKind h = ki->head, first = d->outputs.empty() ? h : kind_info(d->outputs.front().kind).head;
     const std::string is = " ('" + mo.name + "' is " + kind + ")";
+    if ((h == HeadKind::NextToken) != (first == HeadKind::NextToken)) {
+      *err = "signature.outputs: next-token outputs (next_token_position, next_token_top_k_ids, next_token_top_k_probabilities,"
+             " next_token_top_k_logits) cannot be mixed with classification, span, encoder or fill-mask outputs" + is;
+      return false;
+    }
     if ((h == HeadKind::FillMask) != (first == HeadKind::FillMask)) {
       *err = "signature.outputs: fill-mask outputs (masked_positions, masked_top_k_ids, masked_top_k_probabilities,"
              " masked_top_k_logits) cannot be mixed with classification, span or encoder outputs" + is;
       return false;
     }
-    if (h != HeadKind::FillMask) {
+    if (h != HeadKind::FillMask && h != HeadKind::NextToken) {
       if ((h == HeadKind::Encoder) != (first == HeadKind::Encoder)) {
         *err = "signature.outputs: encoder outputs (sequence_output, pooled_output, cls_embedding, mean_embedding) cannot be mixed"
                " with classification or span outputs" + is;
@@ -296,6 +321,22 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
         }
         if (takes_k(mo.kind) && (int_field(oj, "k", &v) != 1 || v < 1 || (k >= 0 && v != k))) {
           *err = "signature.outputs: '" + mo.name + "' needs an integer 'k' >= 1, the same for every fill-mask top-k output";
+          return false;
+        }
+        if (takes_k(mo.kind)) k = v;
+        break;
+      case HeadKind::NextToken:
+        if (oj.get("normalize") || span_fields) {
+          *err = "signature.outputs: 'normalize', 'max_answer_length' and 'sep_id' do not apply to next-token outputs" + is;
+          return false;
+        }
+        if (!takes_k(mo.kind) && oj.get("k")) {
+          *err = "signature.outputs: 'k' belongs to next_token_top_k_ids, next_token_top_k_probabilities and"
+                 " next_token_top_k_logits" + is;
+          return false;
+        }
+        if (takes_k(mo.kind) && (int_field(oj, "k", &v) != 1 || v < 1 || (k >= 0 && v != k))) {
+          *err = "signature.outputs: '" + mo.name + "' needs an integer 'k' >= 1, the same for every next-token top-k output";
           return false;
         }
         if (takes_k(mo.kind)) k = v;
@@ -480,6 +521,40 @@ static bool check_fill_mask_bundle(ModelDesc* d, int gathers, std::string* err) 
   return true;
 }
 
+// the next-token head: one last_token op reads the decoder's [S, 1, H] hidden states, the ops after it run on that one
+// token and the last one writes [1, 1, Vp] vocabulary logits: head_n = vocab
+static bool check_next_token_bundle(ModelDesc* d, int last_tokens, std::string* err) {
+  if (!embed_graph(*d, "next-token", "a GPT-2 decoder, a last_token op and the vocabulary projection", err)) return false;
+  if (last_tokens != 1) {
+    *err = "signature.outputs: next-token outputs need exactly one last_token op (the bundle has " + std::to_string(last_tokens) + ")";
+    return false;
+  }
+  const GraphOp& emb = d->ops.front();
+  const int S = emb.h, H = emb.c, V = emb.vocab;
+  const GraphOp* g = nullptr;
+  for (auto& o : d->ops)
+    if (o.kind == OpKind::LastToken) g = &o;
+  if (g->src < 0 || g->h != S || g->w != 1 || g->c != H) {
+    *err = "signature.outputs: the last_token op needs the [" + std::to_string(S) + ", 1, " + std::to_string(H) +
+           "] hidden states of a scratch buffer (it reads [" + std::to_string(g->h) + ", " + std::to_string(g->w) + ", " +
+           std::to_string(g->c) + "] of buffer " + std::to_string(g->src) + ")";
+    return false;
+  }
+  const GraphOp& last = d->ops.back();
+  if (last.oh != 1 || last.ow != 1 || last.cout < V) {
+    *err = "signature.outputs: next-token outputs need a last op that writes [1, 1, Vp] logits, Vp >= " + std::to_string(V) +
+           " (it writes [" + std::to_string(last.oh) + ", " + std::to_string(last.ow) + ", " + std::to_string(last.cout) + "])";
+    return false;
+  }
+  if (!next_token_fits(V, d->head_k, declares_k(*d))) {
+    *err = "signature.outputs: no next-token head for vocab = " + std::to_string(V) + " and k = " + std::to_string(d->head_k) +
+           " (" + next_token_limits() + ")";
+    return false;
+  }
+  d->head_n = V;
+  return true;
+}
+
 // ---------------------------------------------------------------------------------------------------- op kinds ----
 // How an op's [oh, ow, cout] follow from its fields: the kh x kw window at stride and pad, cout from the manifest (Pool:
 // cout = c); [h, w, c]; [h, w, c / 3] from the packed q | k | v; [1, 1, c]; [1, 1, cout] with kh = kw = 1; [slots, 1, c];
@@ -504,9 +579,11 @@ static constexpr OpKindInfo kOpKinds[] = {
     // lda > c (a [S, H] source) reads token 0 of every sequence: BERT's pooler
     {"dense", Geometry::Dense, Acts::Lenient, Residual::Fused, Weights::Kernel},
     // token ids (and segment ids) [S] -> [S, 1, c]: word + position + type embeddings, then LayerNorm
+    // with "norm": false (GPT-2) word + position embeddings only, one fp32 add, no type table and no LayerNorm
     {"embed", Geometry::Same, Acts::Lenient, Residual::Ignored, Weights::Embed},
     {"layernorm", Geometry::Same, Acts::Lenient, Residual::Fused, Weights::Gamma},  // of src + res
-    // multi-head self-attention [S, 1, 3H] -> [S, 1, H] under the request's attention mask
+    // multi-head self-attention [S, 1, 3H] -> [S, 1, H] under the request's attention mask; with "causal": true (GPT-2)
+    // query i sees keys j <= i only, and a bundle without a mask input masks no key
     {"attention", Geometry::Qkv, Acts::Lenient, Residual::Ignored, Weights::None},
     // fill-mask bundles: from the [S, 1, H] hidden states in src, copies those of the first `slots` = M tokens whose id is
     // mask_token_id (and whose mask is set, with a mask input) to dst [M, 1, H], ascending position, zeros for empty
@@ -522,6 +599,10 @@ static constexpr OpKindInfo kOpKinds[] = {
     {"window_attention", Geometry::Qkv, Acts::Refused, Residual::Refused, Weights::WindowBias},
     // Swin: [h, w, c] -> [h/2, w/2, 4c] in torchvision's x0 | x1 | x2 | x3 order
     {"patch_merge", Geometry::Merge, Acts::Refused, Residual::Refused, Weights::None},
+    // next-token bundles: from the [S, 1, H] hidden states in src, copies those of each row's last attended token (the
+    // highest position whose mask is set with a mask input, else S - 1; none: zeros) to dst [1, 1, H], and writes that
+    // position (int32, -1 none) to the executor's positions scratch for the head
+    {"last_token", Geometry::Point, Acts::Refused, Residual::Refused, Weights::None},
 };
 static_assert(sizeof(kOpKinds) / sizeof(kOpKinds[0]) == (size_t)kLastOpKind + 1, "one row per OpKind");
 
@@ -548,10 +629,17 @@ static std::string kind_error(const Json& oj, GraphOp& o) {
   auto hwc = [&] { return std::to_string(o.h) + " x " + std::to_string(o.w) + " x " + std::to_string(o.c); };
   switch (o.kind) {
     case OpKind::Embed:
+      if (!o.norm) return "";
+      [[fallthrough]];
     case OpKind::LayerNorm:
       return layernorm_supported(o.c) ? "" : "no LayerNorm kernel for hidden " + std::to_string(o.c) + " (at most 12272)";
     case OpKind::Attention:
       if (o.c % 3 || o.heads < 1 || o.cout % o.heads || o.w != 1) return "attention expects a packed [S,1,3H] qkv source";
+      if (o.causal) {
+        if (attention_causal_supported(o.h, o.cout, o.heads, o.src >= 0 && o.dst >= 0)) return "";
+        return "no causal attention kernel for S = " + std::to_string(o.h) + ", hidden " + std::to_string(o.cout) + ", " +
+               std::to_string(o.heads) + " heads (head width d % 4 == 0 and d <= 128, on scratch buffers)";
+      }
       // the executor's scratch buffers are 256-byte aligned (graph_buf_bytes); the request input (src -1) and the response
       // (dst -2) may be any caller pointer, so an op that reads or writes those must run without the aligned kernels
       if (attention_supported(o.h, o.cout, o.heads, o.src >= 0 && o.dst >= 0)) return "";
@@ -612,8 +700,9 @@ static const char* weights_error(const GraphOp& o, Weights w, size_t bytes) {
         return nullptr;
       return "weights out of range or misaligned";
     case Weights::Embed:
-      if (!fits(o.word_off, (size_t)o.vocab * c) || !fits(o.pos_off, (size_t)o.max_pos * c) || !fits(o.type_off, 2 * c))
+      if (!fits(o.word_off, (size_t)o.vocab * c) || !fits(o.pos_off, (size_t)o.max_pos * c) || (o.norm && !fits(o.type_off, 2 * c)))
         return "bad embed op";
+      if (!o.norm) return nullptr;
       [[fallthrough]];
     case Weights::Gamma: return fits(o.w_off, c) && fits(o.b_off, c) ? nullptr : "LayerNorm gamma/beta out of range";
     case Weights::WindowBias:
@@ -783,13 +872,29 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       o.cout = (int)oj.get_int("cout", o.c);
       const std::string act = oj.get_str("act", "none");
       o.act = act == "relu" ? 1 : act == "gelu" ? 2 : act == "tanh" ? 3 : act == "relu6" ? 4 : act == "silu" ? 5 : act == "sigmoid" ? 6 : 0;
-      if (k->acts == Acts::Depthwise && !(act == "none" || o.act == 1 || o.act >= 4)) {
+      // gelu_tanh runs on the GEMM epilogues only; every other lenient op reads it as none, as any unknown name
+      if (act == "gelu_tanh" && (o.kind == OpKind::Conv || o.kind == OpKind::Dense)) o.act = 7;
+      if (k->acts == Acts::Depthwise && !(act == "none" || o.act == 1 || (o.act >= 4 && o.act <= 6))) {
         *err = "graph manifest: " + kind + " act '" + act + "' is not none, relu, relu6, silu or sigmoid";
         return false;
       }
       if (k->acts == Acts::Refused && act != "none") {
         *err = "graph manifest: " + kind + " takes no activation (act '" + act + "')";
         return false;
+      }
+      // the flags of one kind: "causal" (attention), "norm" (embed)
+      for (const char* flag : {"causal", "norm"}) {
+        const Json* f = oj.get(flag);
+        if (!f) continue;
+        if (o.kind != (flag[0] == 'c' ? OpKind::Attention : OpKind::Embed)) {
+          *err = "graph manifest: " + kind + " takes no '" + flag + "' (" + (flag[0] == 'c' ? "attention" : "embed") + " only)";
+          return false;
+        }
+        if (f->type != Json::Bool) {
+          *err = "graph manifest: " + kind + " has a '" + flag + "' that is not true or false";
+          return false;
+        }
+        (flag[0] == 'c' ? o.causal : o.norm) = f->b;
       }
       o.heads = (int)oj.get_int("heads", 1);
       o.vocab = (int)oj.get_int("vocab", 0);
@@ -891,20 +996,30 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       *err = "signature.inputs needs input_dtype int32";
       return false;
     }
+    if (!d->ops.front().norm && d->input(InputRole::TypeIds)) {
+      *err = "signature.inputs: an embed op with norm false reads no type_ids input";
+      return false;
+    }
     const int64_t S = d->ops.front().h;
     for (size_t i = 0; i < d->inputs.size(); ++i) d->inputs[i].offset = (int64_t)i * S;
   }
   finish(d);
-  int gathers = 0;
-  for (auto& o : d->ops) gathers += o.kind == OpKind::MaskGather;
+  int gathers = 0, last_tokens = 0;
+  for (auto& o : d->ops) gathers += o.kind == OpKind::MaskGather, last_tokens += o.kind == OpKind::LastToken;
   if (gathers && d->head != HeadKind::FillMask) {
     *err = "graph manifest: a mask_gather op needs fill-mask outputs (masked_positions, masked_top_k_ids, "
            "masked_top_k_probabilities, masked_top_k_logits)";
     return false;
   }
+  if (last_tokens && d->head != HeadKind::NextToken) {
+    *err = "graph manifest: a last_token op needs next-token outputs (next_token_position, next_token_top_k_ids, "
+           "next_token_top_k_probabilities, next_token_top_k_logits)";
+    return false;
+  }
   if (d->outputs.empty()) return true;
   bool ok = false;
   switch (d->head) {
+    case HeadKind::NextToken: ok = check_next_token_bundle(d, last_tokens, err); break;
     case HeadKind::FillMask: ok = check_fill_mask_bundle(d, gathers, err); break;
     case HeadKind::Encoder: ok = check_encoder_bundle(d, err); break;
     case HeadKind::Span: ok = check_span_bundle(d, err); break;

@@ -18,8 +18,8 @@ enum class Template { Affine, Mlp, Graph };
 // request tensor, -2 = the response tensor). What each kind computes, its manifest name, shape rule, activations,
 // residual and weights are in the op kind table (model.cc).
 enum class OpKind { Conv, MaxPool, AvgPool, Dense, Embed, LayerNorm, Attention, MaskGather, DepthwiseConv, ChannelScale,
-                    WindowAttention, PatchMerge };
-constexpr OpKind kLastOpKind = OpKind::PatchMerge;
+                    WindowAttention, PatchMerge, LastToken };
+constexpr OpKind kLastOpKind = OpKind::LastToken;
 struct GraphOp {
   OpKind kind = OpKind::Conv;
   int src = -1, dst = 0, res = -100;  // res = -100: no residual input
@@ -27,7 +27,7 @@ struct GraphOp {
   int window = 0, shift = 0;          // WindowAttention
   int h = 1, w = 1, c = 1;            // input H, W, C per image
   int kh = 1, kw = 1, stride = 1, pad = 0, cout = 1, oh = 1, ow = 1;
-  int act = 0;                        // 0 none, 1 relu, 2 gelu(erf), 3 tanh, 4 relu6, 5 silu, 6 sigmoid
+  int act = 0;                        // 0 none, 1 relu, 2 gelu(erf), 3 tanh, 4 relu6, 5 silu, 6 sigmoid, 7 gelu_tanh
   size_t w_off = 0, b_off = 0;        // kernel / bias; LayerNorm + Embed: gamma / beta
   // transformer ops (a "image" is a sequence: h = S tokens, w = 1, c = hidden width)
   int heads = 1, vocab = 0, max_pos = 0;
@@ -35,6 +35,8 @@ struct GraphOp {
   float eps = 1e-12f;
   int64_t lda = 0;                    // Dense: elements per image of the source (> c selects the first token)
   int mask_token_id = 0;              // MaskGather (slots = oh)
+  bool causal = false;                // Attention: query i sees keys j <= i
+  bool norm = true;                   // Embed: LayerNorm after the sum (false: word + position only)
 };
 
 struct DenseLayer {
@@ -63,8 +65,9 @@ struct ModelInput {
 // Classify: the last op's N logits (head.cu). Span (question answering): the last op's [S, 1, 2] per-token start / end
 // logits (span.cu). Encoder (embeddings): the last hidden states [S, 1, H] and the pooler's [H] (encoder_head.cu).
 // FillMask (masked-language-model prediction): the [M, 1, Vp] vocabulary logits of the M [MASK] slots a mask_gather op
-// selected (mlm.cu).
-enum class HeadKind { None, Classify, Span, Encoder, FillMask };
+// selected (mlm.cu). NextToken (causal language-model prediction): the [1, 1, Vp] vocabulary logits of the one token a
+// last_token op selected per row (the fill-mask head's kernel with one slot).
+enum class HeadKind { None, Classify, Span, Encoder, FillMask, NextToken };
 
 // One declared output of a multi-output bundle (signature.outputs). Its name, head, dtype and per-row shape are in the
 // kind table (model.cc). New kinds go at the end: the forward hop sends the enum's numbers.
@@ -72,9 +75,10 @@ enum class OutputKind {
   Logits, Probabilities, Classes, TopKClasses, TopKProbabilities,
   StartLogits, EndLogits, SpanStarts, SpanEnds, SpanScores,
   SequenceOutput, PooledOutput, ClsEmbedding, MeanEmbedding,
-  MaskedPositions, MaskedTopKIds, MaskedTopKProbabilities, MaskedTopKLogits
+  MaskedPositions, MaskedTopKIds, MaskedTopKProbabilities, MaskedTopKLogits,
+  NextTokenPosition, NextTokenTopKIds, NextTokenTopKProbabilities, NextTokenTopKLogits
 };
-constexpr OutputKind kLastOutputKind = OutputKind::MaskedTopKLogits;
+constexpr OutputKind kLastOutputKind = OutputKind::NextTokenTopKLogits;
 struct ModelOutput {
   std::string name;
   OutputKind kind = OutputKind::Logits;
@@ -127,6 +131,7 @@ struct ModelDesc {
   //   Span:     head_n = S, head_k = the number of spans (0: logits only).
   //   Encoder:  head_n = H, head_k = S.
   //   FillMask: head_n = M (the mask_gather op's slots), head_k = k (0: masked_positions only).
+  //   NextToken: head_n = vocab (the embed op's), head_k = k (0: next_token_position only).
   // The rest is known to the owner only, the kernels' business: a span head's span_max_len = max_answer_length and
   // span_sep_id = sep_id (-1: none); an encoder head's encoder_pooler (the last op is the pooler: it writes pooled_output,
   // and the hidden states are its source buffer) and normalize_cls / normalize_mean; a fill-mask head's mlm_vocab (the
@@ -154,7 +159,8 @@ struct ModelDesc {
   size_t graph_buf_bytes(int64_t rows) const;
   // offset of the head's logits in that scratch (graph bundles with outputs: after the buffers and the im2col matrix)
   size_t head_scratch_offset(int64_t rows) const;
-  // fill-mask bundles: offset of the mask_gather op's int32 positions [rows, M] in that scratch, after the head's logits
+  // fill-mask and next-token bundles: offset of the mask_gather op's int32 positions [rows, M] (the last_token op's
+  // [rows]) in that scratch, after the head's logits
   size_t mlm_positions_offset(int64_t rows) const;
 };
 

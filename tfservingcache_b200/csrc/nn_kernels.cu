@@ -132,6 +132,7 @@ gemm_f32_kernel(const float* __restrict__ A, const float* __restrict__ B, const 
       else if (act == 4) v = relu6f(v);
       else if (act == 5) v = siluf(v);
       else if (act == 6) v = sigmoidf(v);
+      else if (act == 7) v = gelu_tanhf(v);
       C[(size_t)gm * N + gn] = v;
     }
   }
@@ -431,7 +432,8 @@ attention_kernel(const float* __restrict__ qkv, const int* __restrict__ mask, in
 // d+4 floats: conflict-free LDS.128; q rows are broadcasts). Softmax in registers + warp shuffles; the unnormalised
 // probabilities go through shared memory once for the P.V product (lane = two output dims). ~10x fewer shared-memory
 // instructions per FMA than the row-at-a-time kernel above, and 4x the CTAs (BERT-base, 8 x 128: 384 CTAs, 2 per SM).
-template <int KPL>
+// kCausal: query i sees keys j <= i only (GPT-2); a hidden key gets exactly zero weight, and key 0 is visible to every row.
+template <int KPL, bool kCausal>
 __global__ void __launch_bounds__(128)
 attention_tile_kernel(const float* __restrict__ qkv, const int* __restrict__ mask, int mask_stride, float* __restrict__ ctx, int S,
                       int H, int heads) {
@@ -494,7 +496,8 @@ attention_tile_kernel(const float* __restrict__ qkv, const int* __restrict__ mas
 #pragma unroll
     for (int t = 0; t < KPL; ++t) {
       const float m = Ms[lane + 32 * t];
-      sc[r][t] = m == -FLT_MAX ? -FLT_MAX : sc[r][t] * scale + m;
+      const bool hidden = m == -FLT_MAX || (kCausal && lane + 32 * t > q0 + r0 + r);
+      sc[r][t] = hidden ? -FLT_MAX : sc[r][t] * scale + m;
       mx = fmaxf(mx, sc[r][t]);
     }
 #pragma unroll
@@ -511,7 +514,8 @@ attention_tile_kernel(const float* __restrict__ qkv, const int* __restrict__ mas
     inv[r] = 1.f / sum;
   }
   __syncwarp();  // a warp only reads the 8 rows of P it wrote
-  const int S4 = (S + 3) & ~3;   // V rows and P columns in [S, S4) are zeros
+  // V rows and P columns in [S, S4) are zeros; under kCausal so are the P columns past the tile's last query
+  const int S4 = kCausal ? min((S + 3) & ~3, q0 + 32) : (S + 3) & ~3;
   for (int dd = lane * 2; dd < d; dd += 64) {
     float2 acc[8];
 #pragma unroll
@@ -538,7 +542,9 @@ attention_tile_kernel(const float* __restrict__ qkv, const int* __restrict__ mas
 // through shared memory 64 keys at a time, so shared memory does not grow with S. Online softmax (Milakov & Gimelshein
 // 2018): each row keeps a running max m and its lanes partial sums l; when a block raises m, l and the P.V accumulators
 // are rescaled by exp(m_old - m_new). A lane owns output dims lane*2 and 64 + lane*2 (d <= 128, d % 4 == 0).
+// kCausal: as attention_tile_kernel's; a query tile stops at the last key block it can see.
 constexpr int kAttnKeyBlock = 64;
+template <bool kCausal>
 __global__ void __launch_bounds__(128)
 attention_keyblock_kernel(const float* __restrict__ qkv, const int* __restrict__ mask, int mask_stride, float* __restrict__ ctx,
                           int S, int H, int heads) {
@@ -573,7 +579,10 @@ attention_keyblock_kernel(const float* __restrict__ qkv, const int* __restrict__
     lsum[r] = 0.f;
     acc[0][r] = acc[1][r] = make_float2(0.f, 0.f);
   }
-  for (int j0 = 0; j0 < S; j0 += KB) {
+  // causal: the blocks up to the tile's last query q0 + 31. Blocks start at multiples of 64 and tiles at multiples of 32, so
+  // the first key j0 of every block visited is <= q0: visible to every row of the tile
+  const int jend = kCausal ? min(S, q0 + 32) : S;
+  for (int j0 = 0; j0 < jend; j0 += KB) {
     __syncthreads();  // the previous block's K / V / mask are no longer read
     for (int idx = threadIdx.x; idx < KB * d4; idx += 128) {
       const int j = idx / d4, c = (idx - j * d4) << 2;
@@ -609,12 +618,14 @@ attention_keyblock_kernel(const float* __restrict__ qkv, const int* __restrict__
 #pragma unroll
       for (int t = 0; t < 2; ++t) {
         const float m = Ms[lane + 32 * t];
-        sc[r][t] = m == -FLT_MAX ? -FLT_MAX : sc[r][t] * scale + m;
+        const bool hidden = m == -FLT_MAX || (kCausal && j0 + lane + 32 * t > q0 + r0 + r);
+        sc[r][t] = hidden ? -FLT_MAX : sc[r][t] * scale + m;
         mx = fmaxf(mx, sc[r][t]);
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-      // every block holds at least one key < S, so mx is finite from the first block on
+      // every block holds at least one key < S (under kCausal key j0, visible to every row), so mx is finite from the
+      // first block on
       const float alpha = mrow[r] == -FLT_MAX ? 0.f : expf(mrow[r] - mx);
       mrow[r] = mx;
       float part = 0.f;
@@ -677,7 +688,7 @@ static size_t attention_keyblock_smem(int d) {
 }
 
 
-template <int KPL>
+template <int KPL, bool kCausal>
 static cudaError_t launch_attention_tile(const float* qkv, const int* mask, int mask_stride, float* ctx, int Bn, int S, int H, int heads,
                                          cudaStream_t s) {
   const size_t smem = attention_tile_smem(S, H / heads, KPL);
@@ -685,15 +696,16 @@ static cudaError_t launch_attention_tile(const float* qkv, const int* mask, int 
   int dev = 0;
   cudaGetDevice(&dev);
   if (!attr[dev & 63]) {
-    cudaError_t e = cudaFuncSetAttribute(attention_tile_kernel<KPL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttnSmemCap);
+    cudaError_t e = cudaFuncSetAttribute(attention_tile_kernel<KPL, kCausal>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAttnSmemCap);
     if (e != cudaSuccess) return e;
     attr[dev & 63] = true;
   }
-  attention_tile_kernel<KPL><<<dim3((S + 31) / 32, Bn * heads), 128, smem, s>>>(qkv, mask, mask_stride, ctx, S, H, heads);
+  attention_tile_kernel<KPL, kCausal><<<dim3((S + 31) / 32, Bn * heads), 128, smem, s>>>(qkv, mask, mask_stride, ctx, S, H, heads);
   g_launches_nn++;
   return cudaGetLastError();
 }
 
+template <bool kCausal>
 static cudaError_t launch_attention_keyblock(const float* qkv, const int* mask, int mask_stride, float* ctx, int Bn, int S, int H,
                                              int heads, cudaStream_t s) {
   const size_t smem = attention_keyblock_smem(H / heads);
@@ -701,14 +713,46 @@ static cudaError_t launch_attention_keyblock(const float* qkv, const int* mask, 
   int dev = 0;
   cudaGetDevice(&dev);
   if (!attr[dev & 63]) {
-    cudaError_t e = cudaFuncSetAttribute(attention_keyblock_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(attention_keyblock_kernel<kCausal>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)attention_keyblock_smem(128));
     if (e != cudaSuccess) return e;
     attr[dev & 63] = true;
   }
-  attention_keyblock_kernel<<<dim3((S + 31) / 32, Bn * heads), 128, smem, s>>>(qkv, mask, mask_stride, ctx, S, H, heads);
+  attention_keyblock_kernel<kCausal><<<dim3((S + 31) / 32, Bn * heads), 128, smem, s>>>(qkv, mask, mask_stride, ctx, S, H, heads);
   g_launches_nn++;
   return cudaGetLastError();
+}
+
+// The tiled kernels up to S = 256 and the key-block kernel above, for d % 4 == 0, d <= 128 on 16-byte aligned qkv / ctx.
+// gridDim.y = sequences x heads is capped at 65,535: more sequences run as consecutive launches; one launch below the cap
+template <bool kCausal>
+static cudaError_t launch_attention_tiled(const float* qkv, const int* mask, int mask_stride, float* ctx, int Bn, int S, int H,
+                                          int heads, cudaStream_t s) {
+  const int d = H / heads;
+  const int kpl = (S + 31) / 32;
+  const int chunk = heads < kMaxGridY ? kMaxGridY / heads : 1;
+  for (int b0 = 0; b0 < Bn; b0 += chunk) {
+    const int nb = Bn - b0 < chunk ? Bn - b0 : chunk;
+    const float* q = qkv + (size_t)b0 * S * 3 * H;
+    const int* m = mask ? mask + (size_t)b0 * mask_stride : nullptr;
+    float* c = ctx + (size_t)b0 * S * H;
+    cudaError_t e;
+    if (kpl <= 1 && attention_tile_smem(S, d, 1) <= kAttnSmemCap) e = launch_attention_tile<1, kCausal>(q, m, mask_stride, c, nb, S, H, heads, s);
+    else if (kpl <= 2 && attention_tile_smem(S, d, 2) <= kAttnSmemCap) e = launch_attention_tile<2, kCausal>(q, m, mask_stride, c, nb, S, H, heads, s);
+    else if (kpl <= 4 && attention_tile_smem(S, d, 4) <= kAttnSmemCap) e = launch_attention_tile<4, kCausal>(q, m, mask_stride, c, nb, S, H, heads, s);
+    else if (kpl <= 8 && attention_tile_smem(S, d, 8) <= kAttnSmemCap) e = launch_attention_tile<8, kCausal>(q, m, mask_stride, c, nb, S, H, heads, s);
+    else e = launch_attention_keyblock<kCausal>(q, m, mask_stride, c, nb, S, H, heads, s);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
+}
+
+cudaError_t launch_attention_causal(const float* qkv, const int* mask, int mask_stride, float* ctx, int Bn, int S, int H, int heads,
+                                    cudaStream_t s) {
+  if (Bn <= 0) return cudaSuccess;
+  const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;
+  if (!attention_causal_supported(S, H, heads, al)) return cudaErrorInvalidValue;
+  return launch_attention_tiled<true>(qkv, mask, mask_stride, ctx, Bn, S, H, heads, s);
 }
 
 cudaError_t launch_attention(const float* qkv, const int* mask, int mask_stride, float* ctx, int Bn, int S, int H, int heads,
@@ -717,25 +761,7 @@ cudaError_t launch_attention(const float* qkv, const int* mask, int mask_stride,
   const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;
   if (!attention_supported(S, H, heads, al)) return cudaErrorInvalidValue;
   const int d = H / heads;
-  if (d % 4 == 0 && H % 4 == 0 && al && d <= 128) {
-    const int kpl = (S + 31) / 32;
-    // gridDim.y = sequences x heads is capped at 65,535: more sequences run as consecutive launches; one launch below the cap
-    const int chunk = heads < kMaxGridY ? kMaxGridY / heads : 1;
-    for (int b0 = 0; b0 < Bn; b0 += chunk) {
-      const int nb = Bn - b0 < chunk ? Bn - b0 : chunk;
-      const float* q = qkv + (size_t)b0 * S * 3 * H;
-      const int* m = mask ? mask + (size_t)b0 * mask_stride : nullptr;
-      float* c = ctx + (size_t)b0 * S * H;
-      cudaError_t e;
-      if (kpl <= 1 && attention_tile_smem(S, d, 1) <= kAttnSmemCap) e = launch_attention_tile<1>(q, m, mask_stride, c, nb, S, H, heads, s);
-      else if (kpl <= 2 && attention_tile_smem(S, d, 2) <= kAttnSmemCap) e = launch_attention_tile<2>(q, m, mask_stride, c, nb, S, H, heads, s);
-      else if (kpl <= 4 && attention_tile_smem(S, d, 4) <= kAttnSmemCap) e = launch_attention_tile<4>(q, m, mask_stride, c, nb, S, H, heads, s);
-      else if (kpl <= 8 && attention_tile_smem(S, d, 8) <= kAttnSmemCap) e = launch_attention_tile<8>(q, m, mask_stride, c, nb, S, H, heads, s);
-      else e = launch_attention_keyblock(q, m, mask_stride, c, nb, S, H, heads, s);
-      if (e != cudaSuccess) return e;
-    }
-    return cudaSuccess;
-  }
+  if (d % 4 == 0 && H % 4 == 0 && al && d <= 128) return launch_attention_tiled<false>(qkv, mask, mask_stride, ctx, Bn, S, H, heads, s);
   const size_t smem = attention_smem_bytes(S, H, heads);
   static bool attr[64] = {};
   int dev = 0;

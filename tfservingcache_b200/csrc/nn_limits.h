@@ -25,6 +25,14 @@ inline bool attention_supported(int S, int H, int heads, bool aligned16) {
   return attention_smem_bytes(S, H, heads) <= kAttnSmemCap;
 }
 
+// Causal attention (query i sees keys j <= i) runs on the tiled and key-block kernels only: d % 4 == 0, d <= 128, 16-byte
+// aligned qkv / ctx, every S.
+inline bool attention_causal_supported(int S, int H, int heads, bool aligned16) {
+  if (S < 1 || heads < 1 || H < heads || H % heads) return false;
+  const int d = H / heads;
+  return d % 4 == 0 && H % 4 == 0 && d <= 128 && aligned16;
+}
+
 // LayerNorm stages one row of H floats in dynamic shared memory next to its 64-byte reduction scratch, within the 48 KB a
 // kernel gets without opting in: H <= 12272
 inline bool layernorm_supported(int H) { return H >= 1 && (size_t)H * sizeof(float) + 64 <= 48 * 1024; }
@@ -56,6 +64,14 @@ inline bool mask_gather_supported(int S, int H, int M) {
 }
 inline bool fill_mask_supported(int M, int vocab, int k) {
   return M >= 1 && M <= kMaskGatherMaxS && vocab >= 1 && vocab <= kHeadMaxN && k >= 1 && k <= kHeadMaxK && k <= vocab;
+}
+
+// Next-token head (mlm.cu): the fill-mask head's kernel with one slot per row. Its CTA stages a row of `vocab` fp32 logits
+// in dynamic shared memory beside about 0.4 KB of static shared memory, within the 227 KB a CTA may opt in to on an H100:
+// vocab <= 57344 (224 KB), which holds GPT-2's 50257. A head with next_token_position only runs as k = 1.
+constexpr int kNextTokenMaxVocab = 57344;
+inline bool next_token_supported(int vocab, int k) {
+  return vocab >= 1 && vocab <= kNextTokenMaxVocab && k >= 1 && k <= kHeadMaxK && k <= vocab;
 }
 
 // Depthwise convolution (depthwise.cu): a thread runs the kh x kw taps of one output pixel for 4 channels (1 on the scalar

@@ -583,7 +583,7 @@ size_t Node::model_ws_bytes(const ModelDesc& d) {
       size_t w = dense_workspace_bytes(kMaxRowsPerLaunch, o.c, o.cout);
       if (w > m) m = w;
     }
-    after_gather = after_gather || o.kind == OpKind::MaskGather;
+    after_gather = after_gather || o.kind == OpKind::MaskGather || o.kind == OpKind::LastToken;
   }
   return m;
 }
@@ -599,8 +599,9 @@ static bool conv_tc_enabled() {  // TFSC_CONV_TC=0: explicit im2col + GEMM (the 
 // multi-output bundles: one launch of the bundle's head writes every declared output of a row at its offset in the packed
 // row (out_dim words). `out` is what the last op (or the mlp's last layer) wrote: N logits (classify), [S, 2] start / end
 // logits (span), the [S, H] hidden states or, under a pooler, its [H] output (encoder), [M, Vp] vocabulary logits
-// (fill-mask). The graph heads read the request's ids / mask / segment ids where the embedding reads them (`in`), an
-// encoder under a pooler its source buffer (`hidden`), a fill-mask head the mask_gather op's [rows, M] `positions`.
+// (fill-mask), [1, Vp] vocabulary logits (next-token). The graph heads read the request's ids / mask / segment ids where the embedding reads them (`in`), an
+// encoder under a pooler its source buffer (`hidden`), a fill-mask head the mask_gather op's [rows, M] `positions`, a
+// next-token head the last_token op's [rows] `positions`.
 static cudaError_t run_head(const ModelDesc& d, const float* out, const SpanInputs& in, const float* hidden, const int* positions,
                             int64_t rows, char* y, cudaStream_t st) {
   float* yf = reinterpret_cast<float*>(y);
@@ -654,7 +655,21 @@ static cudaError_t run_head(const ModelDesc& d, const float* out, const SpanInpu
           default: break;
         }
       }
-      return launch_fill_mask_head(out, d.ops.back().cout, positions, (int)rows, d.head_n, d.mlm_vocab, d.head_k, o, st);
+      return launch_fill_mask_head(out, d.ops.back().cout, positions, (int)rows, d.head_n, d.mlm_vocab, d.head_k, kHeadMaxN, o, st);
+    }
+    case HeadKind::NextToken: {  // the fill-mask head with one slot per row, up to the next-token vocabulary cap
+      FillMaskOutputs o;
+      for (const ModelOutput& m : d.outputs) {
+        float* p = yf + m.offset;
+        switch (m.kind) {
+          case OutputKind::NextTokenPosition: o.positions = reinterpret_cast<int*>(p), o.positions_ld = ld; break;
+          case OutputKind::NextTokenTopKIds: o.ids = reinterpret_cast<int*>(p), o.ids_ld = ld; break;
+          case OutputKind::NextTokenTopKProbabilities: o.probs = p, o.probs_ld = ld; break;
+          case OutputKind::NextTokenTopKLogits: o.logits = p, o.logits_ld = ld; break;
+          default: break;
+        }
+      }
+      return launch_fill_mask_head(out, d.ops.back().cout, positions, (int)rows, 1, d.head_n, d.head_k, kNextTokenMaxVocab, o, st);
     }
     case HeadKind::Classify: {
       HeadOutputs o;
@@ -705,8 +720,14 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
       types = ti ? (const int*)x + ti->offset : nullptr;
       stride = (int)d.in_dim;
     }
-    // fill-mask bundles: the mask_gather op writes the [MASK] positions here, and the head reads them
-    int* positions = d.head == HeadKind::FillMask ? reinterpret_cast<int*>(scratch + d.mlm_positions_offset(rows)) : nullptr;
+    // fill-mask bundles: the mask_gather op writes the [MASK] positions here, next-token bundles the last_token op its
+    // positions, and the head reads them
+    int* positions = d.head == HeadKind::FillMask || d.head == HeadKind::NextToken
+                         ? reinterpret_cast<int*>(scratch + d.mlm_positions_offset(rows))
+                         : nullptr;
+    // the request's attention-mask input, or nullptr: what the causal attention and last_token ops read (GPT-2's id 0 is a
+    // token, not [PAD], so they never derive a mask from the ids)
+    const int* mask_input = d.input(InputRole::Mask) ? mask : nullptr;
     bool after_gather = false;
     for (const GraphOp& o : d.ops) {
       const float* src = (const float*)buf(o.src);
@@ -756,6 +777,11 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
         case OpKind::MaxPool: e = launch_maxpool(src, dst, B, o.h, o.w, o.c, o.kh, o.kw, o.stride, o.pad, o.oh, o.ow, st); break;
         case OpKind::AvgPool: e = launch_avgpool(src, dst, B, o.h * o.w, o.c, st); break;
         case OpKind::Embed:
+          if (!o.norm) {
+            e = launch_embed_positions(ids, stride ? stride : o.h, (const float*)(dm.dptr + o.word_off), (const float*)(dm.dptr + o.pos_off),
+                                       dst, B, o.h, o.c, o.vocab, st);
+            break;
+          }
           e = launch_layernorm(nullptr, nullptr, ids, types, stride ? stride : o.h, (const float*)(dm.dptr + o.word_off),
                                (const float*)(dm.dptr + o.pos_off), (const float*)(dm.dptr + o.type_off),
                                (const float*)(dm.dptr + o.w_off), (const float*)(dm.dptr + o.b_off), dst, B * o.h, o.h, o.c, o.vocab,
@@ -765,7 +791,10 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
           e = launch_layernorm(src, o.res == -100 ? nullptr : (const float*)buf(o.res), nullptr, nullptr, 0, nullptr, nullptr, nullptr,
                                (const float*)(dm.dptr + o.w_off), (const float*)(dm.dptr + o.b_off), dst, B * o.h, o.h, o.c, 0, o.eps, st);
           break;
-        case OpKind::Attention: e = launch_attention(src, mask, stride ? stride : o.h, dst, B, o.h, o.cout, o.heads, st); break;
+        case OpKind::Attention:
+          if (o.causal) e = launch_attention_causal(src, mask_input, stride ? stride : o.h, dst, B, o.h, o.cout, o.heads, st);
+          else e = launch_attention(src, mask, stride ? stride : o.h, dst, B, o.h, o.cout, o.heads, st);
+          break;
         case OpKind::MaskGather:
           e = launch_mask_gather(src, ids, d.input(InputRole::Mask) ? mask : nullptr, stride ? stride : o.h, B, o.h, o.c, o.oh,
                                  o.mask_token_id, positions, dst, st);
@@ -780,6 +809,10 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
           e = launch_window_attention(src, (const float*)(dm.dptr + o.b_off), dst, B, o.h, o.w, o.cout, o.heads, o.window, o.shift, st);
           break;
         case OpKind::PatchMerge: e = launch_patch_merge(src, dst, B, o.h, o.w, o.c, st); break;
+        case OpKind::LastToken:
+          e = launch_last_token(src, mask_input, stride ? stride : o.h, B, o.h, o.c, positions, dst, st);
+          after_gather = true;  // the vocabulary projection below 64 rows streams its weights, as fill-mask's
+          break;
       }
       if (e != cudaSuccess) return e;
     }

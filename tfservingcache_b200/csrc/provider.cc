@@ -289,6 +289,11 @@ std::shared_ptr<HostModel> SyntheticModelProvider::load_model(const std::string&
         }
         case OpKind::LayerNorm:
         case OpKind::Embed: {
+          if (!o.norm) {  // word and position tables only
+            fill(base + o.word_off / 4, seed, t0 + 2, (uint64_t)o.vocab * o.c, 0.05f, threads_);
+            fill(base + o.pos_off / 4, seed, t0 + 3, (uint64_t)o.max_pos * o.c, 0.05f, 1);
+            break;
+          }
           float* g = base + o.w_off / 4;
           fill(g, seed, t0, (uint64_t)o.c, 0.1f, 1);
           for (int c = 0; c < o.c; ++c) g[c] += 1.0f;  // gamma = 1 + 0.1 u
@@ -302,7 +307,7 @@ std::shared_ptr<HostModel> SyntheticModelProvider::load_model(const std::string&
         }
         case OpKind::WindowAttention:  // the relative-position bias stays zero
         case OpKind::MaxPool: case OpKind::AvgPool: case OpKind::Attention: case OpKind::MaskGather:
-        case OpKind::ChannelScale: case OpKind::PatchMerge:
+        case OpKind::ChannelScale: case OpKind::PatchMerge: case OpKind::LastToken:
           break;
       }
     }

@@ -1899,8 +1899,56 @@ int tfsc_k_fill_mask_head(const float* logits, int64_t ld, const int32_t* positi
   o.probs_ld = (int64_t)slots * k;
   o.logits = top_logits;
   o.logits_ld = (int64_t)slots * k;
-  cudaError_t e = launch_fill_mask_head(logits, ld, positions, rows, slots, vocab, k, o, (cudaStream_t)stream);
+  cudaError_t e = launch_fill_mask_head(logits, ld, positions, rows, slots, vocab, k, kHeadMaxN, o, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "fill_mask_head: %s", cudaGetErrorString(e));
+}
+int tfsc_k_attention_causal(const float* qkv, const int* mask, int mask_stride, float* ctx, int batch, int seq, int hidden, int heads,
+                            void* stream) {
+  if (int rc = check_device()) return rc;
+  const bool al = ((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(ctx)) & 15) == 0;
+  if (!qkv || !ctx || batch < 1 || (int64_t)batch * heads > 0x7fffffff || !attention_causal_supported(seq, hidden, heads, al))
+    return fail(TFSC_E_INVALID, "attention_causal: no kernel for batch %d, seq %d, hidden %d, heads %d (d %% 4 == 0, d <= 128, "
+                "16-byte aligned qkv / ctx)", batch, seq, hidden, heads);
+  if (mask && mask_stride < seq) return fail(TFSC_E_INVALID, "attention_causal: mask_stride %d is below seq %d", mask_stride, seq);
+  cudaError_t e = launch_attention_causal(qkv, mask, mask_stride, ctx, batch, seq, hidden, heads, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "attention_causal: %s", cudaGetErrorString(e));
+}
+int tfsc_k_embed_positions(const int32_t* ids, int stride, const float* word, const float* pos, float* y, int batch, int seq, int hidden,
+                           int vocab, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (!ids || !word || !pos || !y || batch < 0 || seq < 1 || hidden < 1 || vocab < 1)
+    return fail(TFSC_E_INVALID, "embed_positions: no kernel for batch %d, seq %d, hidden %d, vocab %d", batch, seq, hidden, vocab);
+  if (stride < seq) return fail(TFSC_E_INVALID, "embed_positions: stride %d is below seq %d", stride, seq);
+  cudaError_t e = launch_embed_positions(ids, stride, word, pos, y, batch, seq, hidden, vocab, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "embed_positions: %s", cudaGetErrorString(e));
+}
+int tfsc_k_last_token(const float* hidden, const int32_t* mask, int stride, int rows, int S, int H, int32_t* positions, float* gathered,
+                      void* stream) {
+  if (int rc = check_device()) return rc;
+  if (rows < 0 || S < 1 || H < 1 || (gathered && !hidden))
+    return fail(TFSC_E_INVALID, "last_token: no kernel for %d rows of S = %d, H = %d (the gathered rows need the hidden states)",
+                rows, S, H);
+  if (mask && stride < S) return fail(TFSC_E_INVALID, "last_token: stride %d is below S %d", stride, S);
+  cudaError_t e = launch_last_token(hidden, mask, stride, rows, S, H, positions, gathered, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "last_token: %s", cudaGetErrorString(e));
+}
+int tfsc_k_next_token_head(const float* logits, int64_t ld, const int32_t* positions, int rows, int vocab, int k, int32_t* top_ids,
+                           float* top_probs, float* top_logits, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (rows < 0 || !next_token_supported(vocab, k))
+    return fail(TFSC_E_INVALID, "next_token_head: no kernel for %d rows of vocab = %d, k = %d (1 <= vocab <= %d, 1 <= k <= min(vocab, %d))",
+                rows, vocab, k, kNextTokenMaxVocab, kHeadMaxK);
+  if (!positions || ((top_ids || top_probs || top_logits) && (!logits || ld < vocab)))
+    return fail(TFSC_E_INVALID, "next_token_head: needs the positions and the logits, ld >= vocab (%lld < %d)", (long long)ld, vocab);
+  FillMaskOutputs o;
+  o.ids = top_ids;
+  o.ids_ld = k;
+  o.probs = top_probs;
+  o.probs_ld = k;
+  o.logits = top_logits;
+  o.logits_ld = k;
+  cudaError_t e = launch_fill_mask_head(logits, ld, positions, rows, 1, vocab, k, kNextTokenMaxVocab, o, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "next_token_head: %s", cudaGetErrorString(e));
 }
 int tfsc_debug_gemm_trace(long long*) {
   return fail(TFSC_E_UNIMPLEMENTED, "no GEMM clock trace: the persistent GEMM kernel it timed is not part of the sm_90a build");

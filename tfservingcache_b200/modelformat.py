@@ -16,10 +16,11 @@ def _align256(x: int) -> int:
 
 
 # signature.outputs kinds as the loader's kind table (csrc/model.cc) has them: kind -> (head, dtype, per-row dims in n and
-# k). n is the last op's per-row width (classify), S (span), H (encoder) or the mask_gather op's slots M (fill-mask); k is
-# the entries' "k" (the same on every top-k or span result entry), or S for an encoder. The span result kinds also carry
+# k). n is the last op's per-row width (classify), S (span), H (encoder), the mask_gather op's slots M (fill-mask) or the
+# vocabulary (next-token); k is the entries' "k" (the same on every top-k or span result entry), or S for an encoder. The span result kinds also carry
 # "max_answer_length" and optionally "sep_id" (a graph bundle with a type_ids input, ending in [S, 1, 2] start / end
-# logits); cls_embedding and mean_embedding may carry "normalize": true; classes is one int64 (2 words).
+# logits); cls_embedding and mean_embedding may carry "normalize": true; classes is one int64 (2 words) and
+# next_token_position one int32.
 OUTPUT_KIND_TABLE = {
     "logits": ("classify", "float32", "n"), "probabilities": ("classify", "float32", "n"), "classes": ("classify", "int64", ""),
     "top_k_classes": ("classify", "int32", "k"), "top_k_probabilities": ("classify", "float32", "k"),
@@ -29,9 +30,12 @@ OUTPUT_KIND_TABLE = {
     "cls_embedding": ("encoder", "float32", "n"), "mean_embedding": ("encoder", "float32", "n"),
     "masked_positions": ("fill_mask", "int32", "n"), "masked_top_k_ids": ("fill_mask", "int32", "nk"),
     "masked_top_k_probabilities": ("fill_mask", "float32", "nk"), "masked_top_k_logits": ("fill_mask", "float32", "nk"),
+    "next_token_position": ("next_token", "int32", ""), "next_token_top_k_ids": ("next_token", "int32", "k"),
+    "next_token_top_k_probabilities": ("next_token", "float32", "k"), "next_token_top_k_logits": ("next_token", "float32", "k"),
 }
-OUTPUT_KINDS, SPAN_OUTPUT_KINDS, ENCODER_OUTPUT_KINDS, MLM_OUTPUT_KINDS = (
-    tuple(k for k, v in OUTPUT_KIND_TABLE.items() if v[0] == head) for head in ("classify", "span", "encoder", "fill_mask"))
+OUTPUT_KINDS, SPAN_OUTPUT_KINDS, ENCODER_OUTPUT_KINDS, MLM_OUTPUT_KINDS, NEXT_TOKEN_OUTPUT_KINDS = (
+    tuple(k for k, v in OUTPUT_KIND_TABLE.items() if v[0] == head)
+    for head in ("classify", "span", "encoder", "fill_mask", "next_token"))
 
 
 def _signature(sig: dict, outputs):
@@ -71,8 +75,8 @@ def split_packed_rows(rows_words: np.ndarray, outputs, n, seq=None) -> dict:
     res = {}
     for name, off, width, dtype in packed_output_layout(outputs, n, seq):
         part = np.ascontiguousarray(w[:, off:off + width])
-        if dtype == "int64":
-            res[name] = part.view("<i8").reshape(-1)
+        if dtype == "int64" or not dims[name]:       # the scalar kinds: one value per row
+            res[name] = part.view("<i8" if dtype == "int64" else "<i4").reshape(-1)
         else:
             res[name] = part.view("<i4" if dtype == "int32" else "<f4")
         if len(dims[name]) == 2:
@@ -143,6 +147,9 @@ def _graph_manifest(input_shape, ops, n_buffers, input_name="x", output_name="y"
             op["b_offset"] = take(op["c"] * 4)
         elif op["op"] == "window_attention":                # relative-position bias expanded to [heads, N, N]
             op["bias_offset"] = take(op["heads"] * op["window"] ** 4 * 4)
+        elif op["op"] == "embed" and op.get("norm", True) is False:   # word and position tables only
+            op["word_offset"] = take(op["vocab"] * op["c"] * 4)
+            op["pos_offset"] = take(op["max_pos"] * op["c"] * 4)
         elif op["op"] in ("layernorm", "embed"):
             op["w_offset"] = take(op["c"] * 4)      # gamma
             op["b_offset"] = take(op["c"] * 4)      # beta
@@ -395,5 +402,44 @@ def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30
     else:
         ops.append({"op": "dense", "src": 0, "dst": 1, "h": 1, "w": 1, "c": hidden, "cout": hidden, "act": "tanh"})  # pooler on [CLS]
         ops.append({"op": "dense", "src": 1, "dst": -2, "h": 1, "w": 1, "c": hidden, "cout": labels, "act": "none"})
+    return _graph_manifest([seq], ops, 4, input_name="input_ids", output_name="logits", input_dtype="int32", inputs=inputs,
+                           outputs=outputs)
+
+
+GPT2_INPUTS = [{"name": "input_ids", "role": "ids"}, {"name": "attention_mask", "role": "mask"}]
+
+
+def gpt2_manifest(seq=1024, hidden=768, layers=12, heads=12, vocab=50257, max_pos=1024, inputs=None, outputs=None):
+    """GPT-2 (Radford et al. 2019; transformers' GPT2LMHeadModel topology) as a next-token graph bundle: token ids int32
+    [B, seq] -> the vocabulary logits of each row's last attended token, answered through NEXT_TOKEN_OUTPUT_KINDS. The
+    defaults give GPT-2 small; (1024, 16, 16), (1280, 36, 20) and (1600, 48, 25) as (hidden, layers, heads) give medium,
+    large and XL. The embedding is wte[id] + wpe[s] without LayerNorm ("norm": false). A block is ln_1, c_attn (a 1x1 conv
+    H -> 3H, packed q | k | v), causal attention, c_proj with the block input as residual, ln_2, c_fc (H -> 4H, tanh GELU)
+    and c_proj with the residual. Then a last_token op copies each row's last attended token (the highest position whose
+    mask is set, else seq - 1), ln_f runs on that one token, and the decoder, wte transposed and zero-padded to Vp = vocab
+    rounded up to a multiple of 32 with a zero bias, writes [B, 1, 1, Vp] logits (columns from vocab on are padding).
+    With inputs=None the bundle takes the ids only and attends to every position; inputs=GPT2_INPUTS adds an
+    "attention_mask" that hides keys whose mask is 0 and picks the last attended token. Positions are 0..seq-1 whatever
+    the padding, as transformers' default position ids. Every LayerNorm has eps 1e-5.
+    Buffers: 0 residual stream, 1 normed / attention context, 2 qkv / MLP hidden, 3 post-attention residual."""
+    ops = [{"op": "embed", "src": -1, "dst": 0, "h": seq, "w": 1, "c": hidden, "vocab": vocab, "max_pos": max_pos, "norm": False}]
+
+    def ln(src, dst, n):
+        return {"op": "layernorm", "src": src, "dst": dst, "h": n, "w": 1, "c": hidden, "eps": 1e-5}
+
+    def conv(src, dst, n, cin, cout, act="none", res=None):
+        o = {"op": "conv", "src": src, "dst": dst, "h": n, "w": 1, "c": cin, "kh": 1, "kw": 1, "stride": 1, "pad": 0,
+             "cout": cout, "act": act}
+        if res is not None:
+            o["res"] = res
+        return o
+
+    for _ in range(layers):
+        ops += [ln(0, 1, seq), conv(1, 2, seq, hidden, 3 * hidden),
+                {"op": "attention", "src": 2, "dst": 1, "h": seq, "w": 1, "c": 3 * hidden, "heads": heads, "causal": True},
+                conv(1, 3, seq, hidden, hidden, res=0), ln(3, 1, seq), conv(1, 2, seq, hidden, 4 * hidden, act="gelu_tanh"),
+                conv(2, 0, seq, 4 * hidden, hidden, res=3)]
+    vp = (vocab + 31) // 32 * 32
+    ops += [{"op": "last_token", "src": 0, "dst": 1, "h": seq, "w": 1, "c": hidden}, ln(1, 2, 1), conv(2, -2, 1, hidden, vp)]
     return _graph_manifest([seq], ops, 4, input_name="input_ids", output_name="logits", input_dtype="int32", inputs=inputs,
                            outputs=outputs)
