@@ -463,6 +463,29 @@ int tfsc_k_last_token(const float* hidden, const int32_t* mask, int stride, int 
  * given. */
 int tfsc_k_next_token_head(const float* logits, int64_t ld, const int32_t* positions, int rows, int vocab, int k, int32_t* top_ids,
                            float* top_probs, float* top_logits, void* stream);
+/* Greedy generation. KV cache write: kc[r, s, :] = qkv[r, s, H:2H] and vc[r, s, :] = qkv[r, s, 2H:3H] for s < S, of a packed
+ * qkv [rows, S, 3H] into caches [rows, T, H] (bit-exact copies). TFSC_E_INVALID for T < S or a NULL pointer. */
+int tfsc_k_kv_cache_write(const float* qkv, float* kc, float* vc, int rows, int S, int T, int H, void* stream);
+/* Decode attention of one query per row: qkv [rows, 3H] holds the q | k | v of the token at slot q_r = pos[r] + 1 + t
+ * (pos[r] in -1..S-1). The query sees the cached keys j < q_r of kc / vc [rows, T, H] and its own key; a key j <= pos[r]
+ * whose mask[r * mask_stride + j] is 0 gets the additive -10000 (mask may be NULL). Writes ctx [rows, H] and appends the
+ * token's k and v at slot q_r. `work` holds work_bytes >= tfsc_k_decode_attention_work_bytes(rows, S + t + 1, H, heads)
+ * bytes; it must be zero before the first launch and each launch leaves it so.
+ * TFSC_E_INVALID unless 1 <= S + t + 1 <= min(T, 16384), the head width is d % 4 == 0, d <= 128, and mask_stride >= S with
+ * a mask. */
+int tfsc_k_decode_attention(const float* qkv, float* kc, float* vc, const int32_t* pos, int t, const int32_t* mask, int mask_stride,
+                            int S, int T, float* ctx, int rows, int H, int heads, void* work, int64_t work_bytes, void* stream);
+/* Bytes of the work buffer tfsc_k_decode_attention needs for rows over L = S + t + 1 keys. */
+int64_t tfsc_k_decode_attention_work_bytes(int rows, int L, int H, int heads);
+/* One greedy step: for row r, g = the argmax of logits[r * ld, +vocab) (ties to the lower id) and its log-probability
+ * logit[g] - logsumexp. A row is live at t = 0 when pos[r] >= 0 and later while done[r] == 0; a live row writes
+ * ids[r * ids_ld + t] = g, log_probs[r * lp_ld + t] and length[r * length_ld] = t + 1 and is done after g == eos (eos < 0:
+ * none); any other row writes -1 and 0 (length 0 at t = 0). Unless last, y[r, :] = word[g] + pos_table[pos[r] + 1 + t]
+ * (the bits of tfsc_k_embed_positions). Output pointers may be NULL. TFSC_E_INVALID unless 1 <= vocab <= 57344 and
+ * ld >= vocab. */
+int tfsc_k_generate_select(const float* logits, int64_t ld, int vocab, const int32_t* pos, int t, int last, int eos, int32_t* done,
+                           int32_t* ids, int64_t ids_ld, float* log_probs, int64_t lp_ld, int32_t* length, int64_t length_ld,
+                           const float* word, const float* pos_table, float* y, int rows, int H, void* stream);
 
 #ifdef __cplusplus
 }

@@ -152,6 +152,12 @@ _sig("tfsc_k_attention_causal", C.c_int, vp, vp, C.c_int, vp, C.c_int, C.c_int, 
 _sig("tfsc_k_embed_positions", C.c_int, vp, C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp)
 _sig("tfsc_k_last_token", C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp)
 _sig("tfsc_k_next_token_head", C.c_int, vp, C.c_int64, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp)
+_sig("tfsc_k_kv_cache_write", C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp)
+_sig("tfsc_k_decode_attention", C.c_int, vp, vp, vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp,
+     C.c_int64, vp)
+_sig("tfsc_k_decode_attention_work_bytes", C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int)
+_sig("tfsc_k_generate_select", C.c_int, vp, C.c_int64, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int64, vp, C.c_int64, vp,
+     C.c_int64, vp, vp, vp, C.c_int, C.c_int, vp)
 
 
 class TfscError(RuntimeError):

@@ -103,9 +103,9 @@ __device__ __forceinline__ float head_stage_select(const float* __restrict__ x, 
   return m;
 }
 
-// 1 / sum_j expf(xs[j] - m) over the staged row: fp32 exponentials summed in fp64 (a 32768-wide row keeps its sum to ~1 ulp
-// of fp32). wsum: kHeadThreadsMax / 32 per-warp slots, s_sum: the total (shared memory).
-__device__ __forceinline__ float head_softmax_inv(const float* xs, int n, float m, double* wsum, double* s_sum) {
+// sum_j expf(xs[j] - m) over the staged row: fp32 exponentials summed in fp64 (a 32768-wide row keeps its sum to ~1 ulp of
+// fp32). wsum: kHeadThreadsMax / 32 per-warp slots, s_sum: the total (shared memory).
+__device__ __forceinline__ double head_exp_sum(const float* xs, int n, float m, double* wsum, double* s_sum) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   double acc = 0.0;
   for (int j = threadIdx.x; j < n; j += blockDim.x) acc += (double)expf(xs[j] - m);
@@ -120,7 +120,12 @@ __device__ __forceinline__ float head_softmax_inv(const float* xs, int n, float 
     if (lane == 0) *s_sum = a;
   }
   __syncthreads();
-  return (float)(1.0 / *s_sum);
+  return *s_sum;
+}
+
+// 1 / head_exp_sum, the softmax's normaliser
+__device__ __forceinline__ float head_softmax_inv(const float* xs, int n, float m, double* wsum, double* s_sum) {
+  return (float)(1.0 / head_exp_sum(xs, n, m, wsum, s_sum));
 }
 
 }  // namespace tfsc

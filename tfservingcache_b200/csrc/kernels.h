@@ -185,6 +185,36 @@ cudaError_t launch_embed_positions(const int* ids, int64_t stride, const float* 
 cudaError_t launch_last_token(const float* hidden, const int* mask, int64_t stride, int rows, int S, int H, int* positions,
                               float* gathered, cudaStream_t s);
 
+// Greedy generation (generate.cu). KV cache write: kc[r, s, :] = qkv[r, s, H:2H] and vc[r, s, :] = qkv[r, s, 2H:3H] for
+// s < S, caches [rows, T, H] (bit-exact copies).
+cudaError_t launch_kv_cache_write(const float* qkv, float* kc, float* vc, int rows, int S, int T, int H, cudaStream_t s);
+// Decode attention of one query per row: qkv [rows, 3H] is the step's q | k | v of the token at slot
+// q_r = pos[r] + 1 + t. The query sees the cached keys j < q_r and its own key, except that a key j <= pos[r] whose prompt mask
+// mask[r * mask_stride + j] is 0 gets the additive -10000 (mask may be nullptr). Writes ctx [rows, H] and appends this k and
+// v at slot q_r of kc / vc [rows, T, H]. The keys are split over decode_attention_splits(S + t + 1) blocks, a function of S
+// and t only, and combined in block order, so a row's bits do not depend on its batch. `work` holds
+// decode_attention_work_bytes(rows, S + t + 1, H, heads) (nn_limits.h). cudaErrorInvalidValue outside
+// decode_attention_supported(S + t + 1, H, heads), for S + t + 1 > T or mask_stride < S.
+cudaError_t launch_decode_attention(const float* qkv, float* kc, float* vc, const int* pos, int t, const int* mask,
+                                    int64_t mask_stride, int S, int T, float* ctx, int rows, int H, int heads, void* work,
+                                    cudaStream_t s);
+// One greedy step per row: from logits[r, :vocab] (ld >= vocab) the argmax g (ties to the lower id) and its log-probability
+// logit[g] - logsumexp(logits[:vocab]). A row is live at t = 0 when pos[r] >= 0, later while done[r] == 0. A live row
+// writes ids[t] = g, log_probs[t] and length = t + 1, and is done after g == eos (eos < 0: none); any other row writes
+// -1 and 0 (and length 0 at t = 0). Unless `last`, every row writes the next step's input y[r, :] = word[g] + pos_table[
+// pos[r] + 1 + t] (one fp32 add, as launch_embed_positions). Any output pointer may be nullptr; lds count 32-bit words.
+struct GenerateOutputs {
+  int* ids = nullptr;
+  int64_t ids_ld = 0;
+  float* log_probs = nullptr;
+  int64_t log_probs_ld = 0;
+  int* length = nullptr;
+  int64_t length_ld = 0;
+};
+cudaError_t launch_generate_select(const float* logits, int64_t ld, int vocab, const int* pos, int t, bool last, int eos,
+                                   int* done, const GenerateOutputs& o, const float* word, const float* pos_table, float* y,
+                                   int rows, int H, cudaStream_t s);
+
 // wgmma 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
 bool gemm_tc_supported(const float* A, const float* B, const float* bias, const float* R, const float* C, int M, int N, int K,
                        int lda);

@@ -14,6 +14,7 @@ size_t ModelDesc::scratch_bytes(int64_t rows) const {
   // classify head, 2S per-token start / end logits for a span head)
   if (tmpl == Template::Mlp) return 2 * (((size_t)rows * (size_t)(max_width > 0 ? max_width : 1) * 4 + 255) & ~(size_t)255);
   if (tmpl == Template::Graph) {
+    if (head == HeadKind::Generate) return generate_scratch(rows).end;
     size_t last = 1;
     for (auto v : output_shape) last *= (size_t)v;
     // a fill-mask bundle's int32 [rows, M] positions follow the head's logits, a next-token bundle's [rows]
@@ -36,12 +37,35 @@ size_t ModelDesc::mlm_positions_offset(int64_t rows) const {
   return head_scratch_offset(rows) + align256((size_t)rows * last * 4);
 }
 
+ModelDesc::GenerateScratch ModelDesc::generate_scratch(int64_t rows) const {
+  // the next-token regions come first: the logits and the last_token op's positions, which are each row's p_b
+  const int T = ops.front().h + head_k - 1;
+  int attn = 0, H = 0, heads = 0;
+  size_t work = 0;
+  for (auto& o : ops)
+    if (o.kind == OpKind::Attention) {
+      ++attn;
+      H = std::max(H, o.cout);
+      heads = std::max(heads, o.heads);
+      work = std::max(work, decode_attention_work_bytes(rows, T, o.cout, o.heads));
+    }
+  GenerateScratch g;
+  g.kv = mlm_positions_offset(rows) + align256((size_t)rows * 4);
+  g.cache_bytes = align256((size_t)rows * (size_t)T * (size_t)H * 4);
+  g.work = g.kv + 2 * (size_t)attn * g.cache_bytes;
+  g.counter_bytes = align256((size_t)rows * (size_t)heads * 4);  // decode_attention_work_bytes' first region
+  g.done = g.work + align256(work);
+  g.end = g.done + align256((size_t)rows * 4);
+  return g;
+}
+
 // ------------------------------------------------------------------------------------------------ output kinds ----
 // A row of an output kind in the bundle's head_n / head_k (ModelDesc): one int64 scalar (2 words), one 32-bit scalar, a
 // vector of head_n or head_k values, or a head_k x head_n / head_n x head_k matrix
 enum class Rows { Int64, One, N, K, KxN, NxK };
-// The entry fields a kind takes besides name and kind: "k"; "k", "max_answer_length" and "sep_id"; or "normalize"
-enum class Fields { None, K, Span, Normalize };
+// The entry fields a kind takes besides name and kind: "k"; "k", "max_answer_length" and "sep_id"; "normalize"; or
+// "max_new_tokens" and "eos_token_id"
+enum class Fields { None, K, Span, Normalize, Generate };
 struct OutputKindInfo {
   const char* name;
   HeadKind head;
@@ -73,6 +97,9 @@ static constexpr OutputKindInfo kOutputKinds[] = {
     {"next_token_top_k_ids", HeadKind::NextToken, TFSC_DT_INT32, Rows::K, Fields::K},
     {"next_token_top_k_probabilities", HeadKind::NextToken, TFSC_DT_FLOAT, Rows::K, Fields::K},
     {"next_token_top_k_logits", HeadKind::NextToken, TFSC_DT_FLOAT, Rows::K, Fields::K},
+    {"generated_ids", HeadKind::Generate, TFSC_DT_INT32, Rows::K, Fields::Generate},
+    {"generated_log_probs", HeadKind::Generate, TFSC_DT_FLOAT, Rows::K, Fields::Generate},
+    {"generated_length", HeadKind::Generate, TFSC_DT_INT32, Rows::One, Fields::Generate},
 };
 static_assert(sizeof(kOutputKinds) / sizeof(kOutputKinds[0]) == (size_t)kLastOutputKind + 1, "one row per OutputKind");
 
@@ -114,6 +141,9 @@ static bool next_token_fits(int V, int k, bool with_k) { return next_token_suppo
 static std::string next_token_limits() {
   return "1 <= vocab <= " + std::to_string(kNextTokenMaxVocab) + ", 1 <= k <= min(vocab, " + std::to_string(kHeadMaxK) + ")";
 }
+static std::string generate_limits() {
+  return "1 <= vocab <= " + std::to_string(kNextTokenMaxVocab) + ", 1 <= max_new_tokens <= " + std::to_string(kDecodeMaxKeys);
+}
 static bool encoder_fits(int S, int H, std::string* err) {
   if (encoder_head_supported(S, H)) return true;
   *err = "signature.outputs: no encoder head kernel for S = " + std::to_string(S) + " and H = " + std::to_string(H) +
@@ -125,6 +155,13 @@ bool layout_outputs(ModelDesc* d, std::string* err) {
   set_head(d);
   const bool with_k = declares_k(*d);
   switch (d->head) {
+    case HeadKind::Generate:
+      if (!generate_supported(d->head_n, d->head_k)) {
+        *err = "signature.outputs: no generate head for vocab = " + std::to_string(d->head_n) + " and max_new_tokens = " +
+               std::to_string(d->head_k) + " (" + generate_limits() + ")";
+        return false;
+      }
+      break;
     case HeadKind::NextToken:
       if (!next_token_fits(d->head_n, d->head_k, with_k)) {
         *err = "signature.outputs: no next-token head for vocab = " + std::to_string(d->head_n) + " and k = " +
@@ -236,7 +273,7 @@ ModelDesc make_affine_desc() {
 // mix of heads (fill-mask, then encoder, then span: the message names the later entry's head), a 'normalize' on a kind
 // without one, and then the fields its head takes. Sets d->head.
 static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
-  int k = -1, max_len = -1, sep_id = -1;
+  int k = -1, max_len = -1, sep_id = -1, max_new = -1, eos = -1;
   bool span_seen = false;  // a span_starts / span_ends / span_scores entry set max_len and sep_id
   // an integer field of an output entry: 0 absent, 1 read into *v, -1 present but not an integer
   auto int_field = [](const Json& oj, const char* key, int* v) {
@@ -253,12 +290,18 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
     const OutputKindInfo* ki = nullptr;
     for (auto& i : kOutputKinds)
       if (kind == i.name) ki = &i;
-    if (!ki) {  // a name that starts with next_token is told the next-token kinds, any other the kinds of the other heads
-      const bool next = kind.rfind("next_token", 0) == 0;
-      *err = "signature.outputs: unknown " + std::string(next ? "next-token " : "") + "kind '" + kind + "' (";
+    if (!ki) {  // a name that starts with next_token or generated is told the kinds of that head, any other the kinds of
+      // the heads before them
+      const HeadKind told = kind.rfind("next_token", 0) == 0 ? HeadKind::NextToken
+                            : kind.rfind("generated", 0) == 0 ? HeadKind::Generate
+                                                                : HeadKind::None;
+      *err = "signature.outputs: unknown " +
+             std::string(told == HeadKind::NextToken ? "next-token " : told == HeadKind::Generate ? "generate " : "") + "kind '" +
+             kind + "' (";
       bool any = false;
       for (auto& i : kOutputKinds)
-        if ((i.head == HeadKind::NextToken) == next) *err += std::string(any ? ", " : "") + i.name, any = true;
+        if (i.head == told || (told == HeadKind::None && i.head != HeadKind::NextToken && i.head != HeadKind::Generate))
+          *err += std::string(any ? ", " : "") + i.name, any = true;
       *err += ")";
       return false;
     }
@@ -274,6 +317,11 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
       }
     const HeadKind h = ki->head, first = d->outputs.empty() ? h : kind_info(d->outputs.front().kind).head;
     const std::string is = " ('" + mo.name + "' is " + kind + ")";
+    if ((h == HeadKind::Generate) != (first == HeadKind::Generate)) {
+      *err = "signature.outputs: generate outputs (generated_ids, generated_log_probs, generated_length) cannot be mixed with"
+             " classification, span, encoder, fill-mask or next-token outputs" + is;
+      return false;
+    }
     if ((h == HeadKind::NextToken) != (first == HeadKind::NextToken)) {
       *err = "signature.outputs: next-token outputs (next_token_position, next_token_top_k_ids, next_token_top_k_probabilities,"
              " next_token_top_k_logits) cannot be mixed with classification, span, encoder or fill-mask outputs" + is;
@@ -284,7 +332,7 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
              " masked_top_k_logits) cannot be mixed with classification, span or encoder outputs" + is;
       return false;
     }
-    if (h != HeadKind::FillMask && h != HeadKind::NextToken) {
+    if (h != HeadKind::FillMask && h != HeadKind::NextToken && h != HeadKind::Generate) {
       if ((h == HeadKind::Encoder) != (first == HeadKind::Encoder)) {
         *err = "signature.outputs: encoder outputs (sequence_output, pooled_output, cls_embedding, mean_embedding) cannot be mixed"
                " with classification or span outputs" + is;
@@ -341,6 +389,24 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
         }
         if (takes_k(mo.kind)) k = v;
         break;
+      case HeadKind::Generate:
+        if (oj.get("k") || oj.get("normalize") || span_fields) {
+          *err = "signature.outputs: 'k', 'normalize', 'max_answer_length' and 'sep_id' do not apply to generate outputs" + is;
+          return false;
+        }
+        if (int_field(oj, "max_new_tokens", &v) != 1 || v < 1 || (max_new >= 0 && v != max_new)) {
+          *err = "signature.outputs: '" + mo.name + "' needs an integer 'max_new_tokens' >= 1, the same for every generate output";
+          return false;
+        }
+        max_new = v;
+        v = -1;
+        if (const int r = int_field(oj, "eos_token_id", &v); r < 0 || (r == 1 && (v < 0 || (eos >= 0 && v != eos)))) {
+          *err = "signature.outputs: '" + mo.name + "' has an 'eos_token_id' that is not a token id >= 0 or differs from the"
+                 " other generate outputs'";
+          return false;
+        }
+        if (v >= 0) eos = v;
+        break;
       case HeadKind::Encoder:
         if (oj.get("k") || span_fields) {
           *err = "signature.outputs: 'k', 'max_answer_length' and 'sep_id' do not apply to encoder outputs" + is;
@@ -387,7 +453,8 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
     }
     d->outputs.push_back(mo);
   }
-  d->head_k = span_seen ? k : k < 0 ? 0 : k;  // a span k is always given, and a negative one is refused by span_fits
+  d->head_k = span_seen ? k : max_new >= 0 ? max_new : k < 0 ? 0 : k;  // a span k is always given, and a negative one is refused by span_fits
+  d->gen_eos = eos;
   d->span_max_len = span_seen ? max_len : 0;
   d->span_sep_id = sep_id;
   set_head(d);
@@ -522,11 +589,11 @@ static bool check_fill_mask_bundle(ModelDesc* d, int gathers, std::string* err) 
 }
 
 // the next-token head: one last_token op reads the decoder's [S, 1, H] hidden states, the ops after it run on that one
-// token and the last one writes [1, 1, Vp] vocabulary logits: head_n = vocab
-static bool check_next_token_bundle(ModelDesc* d, int last_tokens, std::string* err) {
-  if (!embed_graph(*d, "next-token", "a GPT-2 decoder, a last_token op and the vocabulary projection", err)) return false;
+// token and the last one writes [1, 1, Vp] vocabulary logits: head_n = vocab. `outputs` names the head in the messages.
+static bool check_last_token_graph(ModelDesc* d, int last_tokens, const std::string& outputs, std::string* err) {
+  if (!embed_graph(*d, outputs, "a GPT-2 decoder, a last_token op and the vocabulary projection", err)) return false;
   if (last_tokens != 1) {
-    *err = "signature.outputs: next-token outputs need exactly one last_token op (the bundle has " + std::to_string(last_tokens) + ")";
+    *err = "signature.outputs: " + outputs + " outputs need exactly one last_token op (the bundle has " + std::to_string(last_tokens) + ")";
     return false;
   }
   const GraphOp& emb = d->ops.front();
@@ -542,13 +609,66 @@ static bool check_next_token_bundle(ModelDesc* d, int last_tokens, std::string* 
   }
   const GraphOp& last = d->ops.back();
   if (last.oh != 1 || last.ow != 1 || last.cout < V) {
-    *err = "signature.outputs: next-token outputs need a last op that writes [1, 1, Vp] logits, Vp >= " + std::to_string(V) +
+    *err = "signature.outputs: " + outputs + " outputs need a last op that writes [1, 1, Vp] logits, Vp >= " + std::to_string(V) +
            " (it writes [" + std::to_string(last.oh) + ", " + std::to_string(last.ow) + ", " + std::to_string(last.cout) + "])";
     return false;
   }
+  return true;
+}
+
+static bool check_next_token_bundle(ModelDesc* d, int last_tokens, std::string* err) {
+  if (!check_last_token_graph(d, last_tokens, "next-token", err)) return false;
+  const int V = d->ops.front().vocab;
   if (!next_token_fits(V, d->head_k, declares_k(*d))) {
     *err = "signature.outputs: no next-token head for vocab = " + std::to_string(V) + " and k = " + std::to_string(d->head_k) +
            " (" + next_token_limits() + ")";
+    return false;
+  }
+  d->head_n = V;
+  return true;
+}
+
+// the generate head: a next-token bundle's graph whose decoder can run one token per row against a KV cache (run_model):
+// between the embed (word + position only) and the last_token op only LayerNorms, 1x1 convs and causal attention ops
+// decode attention takes, and the S + N - 1 slots within the position table
+static bool check_generate_bundle(ModelDesc* d, int last_tokens, std::string* err) {
+  if (!check_last_token_graph(d, last_tokens, "generate", err)) return false;
+  const GraphOp& emb = d->ops.front();
+  const int S = emb.h, V = emb.vocab, N = d->head_k;
+  if (emb.norm) {
+    *err = "signature.outputs: generate outputs need an embed op with norm false (word + position embeddings)";
+    return false;
+  }
+  for (size_t i = 1; i < d->ops.size() && d->ops[i].kind != OpKind::LastToken; ++i) {
+    const GraphOp& o = d->ops[i];
+    const bool ok = o.kind == OpKind::LayerNorm || (o.kind == OpKind::Attention && o.causal) ||
+                    (o.kind == OpKind::Conv && o.kh == 1 && o.kw == 1 && o.stride == 1 && o.pad == 0);
+    if (!ok || o.h != S || o.w != 1) {
+      *err = "signature.outputs: generate outputs need a decoder of layernorm, 1x1 conv and causal attention ops on the [" +
+             std::to_string(S) + ", 1, c] tokens between the embed and the last_token op (op " + std::to_string(i) + " is not)";
+      return false;
+    }
+  }
+  if (!generate_supported(V, N)) {
+    *err = "signature.outputs: no generate head for vocab = " + std::to_string(V) + " and max_new_tokens = " + std::to_string(N) +
+           " (" + generate_limits() + ")";
+    return false;
+  }
+  const int T = S + N - 1;
+  if (T > emb.max_pos) {
+    *err = "signature.outputs: S + max_new_tokens - 1 = " + std::to_string(T) + " positions exceed the embed op's max_pos = " +
+           std::to_string(emb.max_pos);
+    return false;
+  }
+  for (auto& o : d->ops)
+    if (o.kind == OpKind::Attention && !decode_attention_supported(T, o.cout, o.heads)) {
+      *err = "signature.outputs: no decode attention kernel for " + std::to_string(T) + " keys, hidden " + std::to_string(o.cout) +
+             ", " + std::to_string(o.heads) + " heads (1 <= keys <= " + std::to_string(kDecodeMaxKeys) +
+             ", head width d % 4 == 0 and d <= 128)";
+      return false;
+    }
+  if (d->gen_eos >= V) {
+    *err = "signature.outputs: eos_token_id = " + std::to_string(d->gen_eos) + " is not below vocab = " + std::to_string(V);
     return false;
   }
   d->head_n = V;
@@ -1011,7 +1131,7 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
            "masked_top_k_probabilities, masked_top_k_logits)";
     return false;
   }
-  if (last_tokens && d->head != HeadKind::NextToken) {
+  if (last_tokens && d->head != HeadKind::NextToken && d->head != HeadKind::Generate) {
     *err = "graph manifest: a last_token op needs next-token outputs (next_token_position, next_token_top_k_ids, "
            "next_token_top_k_probabilities, next_token_top_k_logits)";
     return false;
@@ -1019,6 +1139,7 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
   if (d->outputs.empty()) return true;
   bool ok = false;
   switch (d->head) {
+    case HeadKind::Generate: ok = check_generate_bundle(d, last_tokens, err); break;
     case HeadKind::NextToken: ok = check_next_token_bundle(d, last_tokens, err); break;
     case HeadKind::FillMask: ok = check_fill_mask_bundle(d, gathers, err); break;
     case HeadKind::Encoder: ok = check_encoder_bundle(d, err); break;

@@ -66,8 +66,9 @@ struct ModelInput {
 // logits (span.cu). Encoder (embeddings): the last hidden states [S, 1, H] and the pooler's [H] (encoder_head.cu).
 // FillMask (masked-language-model prediction): the [M, 1, Vp] vocabulary logits of the M [MASK] slots a mask_gather op
 // selected (mlm.cu). NextToken (causal language-model prediction): the [1, 1, Vp] vocabulary logits of the one token a
-// last_token op selected per row (the fill-mask head's kernel with one slot).
-enum class HeadKind { None, Classify, Span, Encoder, FillMask, NextToken };
+// last_token op selected per row (the fill-mask head's kernel with one slot). Generate (greedy generation): a next-token
+// bundle's graph run once on the prompt and then once per new token on a KV cache (generate.cu).
+enum class HeadKind { None, Classify, Span, Encoder, FillMask, NextToken, Generate };
 
 // One declared output of a multi-output bundle (signature.outputs). Its name, head, dtype and per-row shape are in the
 // kind table (model.cc). New kinds go at the end: the forward hop sends the enum's numbers.
@@ -76,9 +77,10 @@ enum class OutputKind {
   StartLogits, EndLogits, SpanStarts, SpanEnds, SpanScores,
   SequenceOutput, PooledOutput, ClsEmbedding, MeanEmbedding,
   MaskedPositions, MaskedTopKIds, MaskedTopKProbabilities, MaskedTopKLogits,
-  NextTokenPosition, NextTokenTopKIds, NextTokenTopKProbabilities, NextTokenTopKLogits
+  NextTokenPosition, NextTokenTopKIds, NextTokenTopKProbabilities, NextTokenTopKLogits,
+  GeneratedIds, GeneratedLogProbs, GeneratedLength
 };
-constexpr OutputKind kLastOutputKind = OutputKind::NextTokenTopKLogits;
+constexpr OutputKind kLastOutputKind = OutputKind::GeneratedLength;
 struct ModelOutput {
   std::string name;
   OutputKind kind = OutputKind::Logits;
@@ -132,16 +134,19 @@ struct ModelDesc {
   //   Encoder:  head_n = H, head_k = S.
   //   FillMask: head_n = M (the mask_gather op's slots), head_k = k (0: masked_positions only).
   //   NextToken: head_n = vocab (the embed op's), head_k = k (0: next_token_position only).
+  //   Generate: head_n = vocab (the embed op's), head_k = N (max_new_tokens).
   // The rest is known to the owner only, the kernels' business: a span head's span_max_len = max_answer_length and
   // span_sep_id = sep_id (-1: none); an encoder head's encoder_pooler (the last op is the pooler: it writes pooled_output,
   // and the hidden states are its source buffer) and normalize_cls / normalize_mean; a fill-mask head's mlm_vocab (the
-  // embed op's vocab, the logits the head reads of each Vp-wide row) and mlm_mask_token_id.
+  // embed op's vocab, the logits the head reads of each Vp-wide row) and mlm_mask_token_id; a generate head's gen_eos
+  // (eos_token_id, -1: none).
   std::vector<ModelOutput> outputs;
   HeadKind head = HeadKind::None;
   int head_n = 0, head_k = 0;
   int span_max_len = 0, span_sep_id = -1;
   bool encoder_pooler = false, normalize_cls = false, normalize_mean = false;
   int mlm_vocab = 0, mlm_mask_token_id = 0;
+  int gen_eos = -1;
   const ModelOutput* output(OutputKind k) const {
     for (auto& o : outputs)
       if (o.kind == k) return &o;
@@ -162,6 +167,14 @@ struct ModelDesc {
   // fill-mask and next-token bundles: offset of the mask_gather op's int32 positions [rows, M] (the last_token op's
   // [rows]) in that scratch, after the head's logits
   size_t mlm_positions_offset(int64_t rows) const;
+  // generate bundles: the regions after the positions, for T = S + N - 1 cache slots. Attention op i (in op order) keeps
+  // its K cache [rows, T, H] at kv + 2 i cache_bytes and its V cache right after it; then the decode attention work buffer
+  // (decode_attention_work_bytes at T keys) and the int32 [rows] done flags.
+  // counter_bytes: the work buffer's leading int32 counters, the part that must be zero before a request's first step
+  struct GenerateScratch {
+    size_t kv = 0, cache_bytes = 0, work = 0, counter_bytes = 0, done = 0, end = 0;
+  };
+  GenerateScratch generate_scratch(int64_t rows) const;
 };
 
 // Set d->head from the first output's kind, sort d->outputs by name, set their offsets and widths from d->head_n / d->head_k

@@ -74,6 +74,29 @@ inline bool next_token_supported(int vocab, int k) {
   return vocab >= 1 && vocab <= kNextTokenMaxVocab && k >= 1 && k <= kHeadMaxK && k <= vocab;
 }
 
+// Decode attention (generate.cu): one query per row over L cached keys, split into blocks of kDecodeKeys keys, one CTA per
+// (row, head, block). A CTA stages its block's keys in shared memory (34 KB at d = 128, within the 48 KB a kernel gets
+// without opting in) and the last CTA of a (row, head) combines the blocks in order. Head width d % 4 == 0, d <= 128.
+constexpr int kDecodeKeys = 64, kDecodeMaxKeys = 16384;
+inline int decode_attention_splits(int L) { return (L + kDecodeKeys - 1) / kDecodeKeys; }
+inline bool decode_attention_supported(int L, int H, int heads) {
+  if (L < 1 || L > kDecodeMaxKeys || heads < 1 || H < heads || H % heads) return false;
+  const int d = H / heads;
+  return d % 4 == 0 && d <= 128;
+}
+// The work buffer a launch over keys [0, L) needs: an int32 counter per (row, head), which must be zero before the first
+// launch and is left zero by each, then each block's running max, sum and unnormalised context.
+inline size_t decode_attention_work_bytes(long long rows, int L, int H, int heads) {
+  const size_t rh = (size_t)rows * heads, parts = rh * decode_attention_splits(L);
+  return ((rh * 4 + 255) & ~(size_t)255) + parts * (2 + (size_t)(H / heads)) * sizeof(float);
+}
+
+// Greedy generation (generate.cu): the select step stages a row of `vocab` logits like the next-token head (vocab <= 57344)
+// and writes max_new_tokens = N ids and log-probabilities per row; the decode steps' keys are bounded by decode attention's.
+inline bool generate_supported(int vocab, int N) {
+  return vocab >= 1 && vocab <= kNextTokenMaxVocab && N >= 1 && N <= kDecodeMaxKeys;
+}
+
 // Depthwise convolution (depthwise.cu): a thread runs the kh x kw taps of one output pixel for 4 channels (1 on the scalar
 // path). Kernels up to 7 x 7, stride 1 or 2 and padding up to k / 2 cover MobileNetV2 and EfficientNet B0-B7 (3 x 3 and
 // 5 x 5, stride <= 2) with margin; offsets within an image are 32-bit (H * W * C < 2^31).

@@ -722,14 +722,14 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
     }
     // fill-mask bundles: the mask_gather op writes the [MASK] positions here, next-token bundles the last_token op its
     // positions, and the head reads them
-    int* positions = d.head == HeadKind::FillMask || d.head == HeadKind::NextToken
+    int* positions = d.head == HeadKind::FillMask || d.head == HeadKind::NextToken || d.head == HeadKind::Generate
                          ? reinterpret_cast<int*>(scratch + d.mlm_positions_offset(rows))
                          : nullptr;
     // the request's attention-mask input, or nullptr: what the causal attention and last_token ops read (GPT-2's id 0 is a
     // token, not [PAD], so they never derive a mask from the ids)
     const int* mask_input = d.input(InputRole::Mask) ? mask : nullptr;
     bool after_gather = false;
-    for (const GraphOp& o : d.ops) {
+    auto exec = [&](const GraphOp& o) -> cudaError_t {
       const float* src = (const float*)buf(o.src);
       float* dst = (float*)buf(o.dst);
       cudaError_t e = cudaSuccess;
@@ -742,26 +742,20 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
           const int K = o.kh * o.kw * o.c;
           if (o.kind == OpKind::Dense && !res && o.act <= 1 && (int)o.lda == K && B < 64) {
             // a classifier head on a handful of rows is the tenant-MLP problem (HBM-bound weight streaming), not a GEMM tile
-            e = launch_dense(src, W, bias, dst, B, K, o.cout, o.act == 1, ws, ws_cap, st);
-            if (e != cudaSuccess) return e;
-            continue;
+            return launch_dense(src, W, bias, dst, B, K, o.cout, o.act == 1, ws, ws_cap, st);
           }
           if (after_gather && o.kind == OpKind::Conv && o.dst == -2 && !res && o.act <= 1 && o.kh == 1 && o.kw == 1 &&
               o.stride == 1 && o.pad == 0 && o.cout % 32 == 0 && B * o.oh * o.ow < 64) {
             // a fill-mask vocabulary projection, padded to Vp % 32 == 0, on fewer than 64 slots (one [MASK] per row at the
             // default batch of 8): too few rows for the tensor-core GEMM, so it streams the [H, Vp] weights once (DESIGN §4);
             // an unpadded decoder keeps the GEMM path
-            e = launch_dense(src, W, bias, dst, B * o.oh * o.ow, K, o.cout, o.act == 1, ws, ws_cap, st);
-            if (e != cudaSuccess) return e;
-            continue;
+            return launch_dense(src, W, bias, dst, B * o.oh * o.ow, K, o.cout, o.act == 1, ws, ws_cap, st);
           }
           const bool direct = o.kh == 1 && o.kw == 1 && o.stride == 1 && o.pad == 0;
           if (o.kind == OpKind::Conv && !direct && conv_tc_enabled() &&
               conv_tc_supported(src, W, bias, res, dst, B, o.h, o.w, o.c, o.kh, o.kw, o.stride, o.pad, o.oh, o.ow, o.cout)) {
             // implicit GEMM: TMA im2col gathers the patch tiles straight from the NHWC activations (no col buffer)
-            e = launch_conv_tc(src, W, bias, res, dst, B, o.h, o.w, o.c, o.kh, o.kw, o.stride, o.pad, o.oh, o.ow, o.cout, o.act, st);
-            if (e != cudaSuccess) return e;
-            continue;
+            return launch_conv_tc(src, W, bias, res, dst, B, o.h, o.w, o.c, o.kh, o.kw, o.stride, o.pad, o.oh, o.ow, o.cout, o.act, st);
           }
           const float* A = src;
           int lda = o.kind == OpKind::Dense ? (int)o.lda : K;  // Dense over a [S,H] source reads token 0 of every sequence
@@ -814,7 +808,64 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
           after_gather = true;  // the vocabulary projection below 64 rows streams its weights, as fill-mask's
           break;
       }
+      return e;
+    };
+    // generate bundles: each attention op's K and V caches [rows, T, H], T = S + N - 1 slots
+    const ModelDesc::GenerateScratch gs = d.head == HeadKind::Generate ? d.generate_scratch(rows) : ModelDesc::GenerateScratch();
+    auto cache = [&](int attn, int v) { return (float*)(scratch + gs.kv + (2 * (size_t)attn + v) * gs.cache_bytes); };
+    const int T = d.ops.front().h + d.head_k - 1;
+    int attn = 0;
+    for (const GraphOp& o : d.ops) {
+      cudaError_t e = exec(o);
+      if (e == cudaSuccess && d.head == HeadKind::Generate && o.kind == OpKind::Attention) {  // the prompt's keys and values
+        e = launch_kv_cache_write((const float*)buf(o.src), cache(attn, 0), cache(attn, 1), B, o.h, T, o.cout, st);
+        ++attn;
+      }
       if (e != cudaSuccess) return e;
+    }
+    if (d.head == HeadKind::Generate) {
+      // greedy decoding: the prefill above left each row's logits at its last attended token p_b (positions); each step
+      // picks a token, embeds it at slot p_b + 1 + t into the embed op's buffer and runs the decoder on that one token
+      // per row against the caches (DESIGN §4). A fixed N - 1 steps, no host synchronisation.
+      const GraphOp& emb = d.ops.front();
+      GenerateOutputs go;
+      for (const ModelOutput& m : d.outputs) {
+        float* p = reinterpret_cast<float*>(y) + m.offset;
+        switch (m.kind) {
+          case OutputKind::GeneratedIds: go.ids = reinterpret_cast<int*>(p), go.ids_ld = d.out_dim; break;
+          case OutputKind::GeneratedLogProbs: go.log_probs = p, go.log_probs_ld = d.out_dim; break;
+          case OutputKind::GeneratedLength: go.length = reinterpret_cast<int*>(p), go.length_ld = d.out_dim; break;
+          default: break;
+        }
+      }
+      int* done = reinterpret_cast<int*>(scratch + gs.done);
+      // the decode attention counters start at zero and every launch leaves them so; the partials after them are written
+      // before they are read
+      cudaError_t e = cudaMemsetAsync(scratch + gs.work, 0, gs.counter_bytes, st);
+      for (int t = 0; e == cudaSuccess && t < d.head_k; ++t) {
+        after_gather = false;
+        attn = 0;
+        for (size_t i = 1; t > 0 && e == cudaSuccess && i < d.ops.size(); ++i) {
+          GraphOp o = d.ops[i];
+          if (o.kind == OpKind::LastToken) {  // a copy of each row's one token; the prompt's positions stay
+            e = launch_last_token((const float*)buf(o.src), nullptr, 1, B, 1, o.c, nullptr, (float*)buf(o.dst), st);
+            after_gather = true;
+          } else if (o.kind == OpKind::Attention) {
+            e = launch_decode_attention((const float*)buf(o.src), cache(attn, 0), cache(attn, 1), positions, t - 1, mask_input,
+                                        stride ? stride : emb.h, emb.h, T, (float*)buf(o.dst), B, o.cout, o.heads,
+                                        scratch + gs.work, st);
+            ++attn;
+          } else {
+            if (!after_gather) o.h = o.oh = 1;  // the decoder's LayerNorms and 1x1 convs on one token per row
+            e = exec(o);
+          }
+        }
+        if (e == cudaSuccess)
+          e = launch_generate_select((const float*)out, d.ops.back().cout, d.head_n, positions, t, t == d.head_k - 1, d.gen_eos,
+                                     done, go, (const float*)(dm.dptr + emb.word_off), (const float*)(dm.dptr + emb.pos_off),
+                                     (float*)buf(emb.dst), B, emb.c, st);
+      }
+      return e;
     }
     SpanInputs in;
     in.ids = ids;

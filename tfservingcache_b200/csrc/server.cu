@@ -1950,6 +1950,50 @@ int tfsc_k_next_token_head(const float* logits, int64_t ld, const int32_t* posit
   cudaError_t e = launch_fill_mask_head(logits, ld, positions, rows, 1, vocab, k, kNextTokenMaxVocab, o, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "next_token_head: %s", cudaGetErrorString(e));
 }
+int tfsc_k_kv_cache_write(const float* qkv, float* kc, float* vc, int rows, int S, int T, int H, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (!qkv || !kc || !vc || rows < 0 || S < 1 || T < S || H < 1)
+    return fail(TFSC_E_INVALID, "kv_cache_write: no kernel for %d rows of S = %d, T = %d, H = %d", rows, S, T, H);
+  cudaError_t e = launch_kv_cache_write(qkv, kc, vc, rows, S, T, H, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "kv_cache_write: %s", cudaGetErrorString(e));
+}
+int64_t tfsc_k_decode_attention_work_bytes(int rows, int L, int H, int heads) {
+  if (rows < 0 || !decode_attention_supported(L, H, heads)) return -1;
+  return (int64_t)decode_attention_work_bytes(rows, L, H, heads);
+}
+int tfsc_k_decode_attention(const float* qkv, float* kc, float* vc, const int32_t* pos, int t, const int32_t* mask, int mask_stride,
+                            int S, int T, float* ctx, int rows, int H, int heads, void* work, int64_t work_bytes, void* stream) {
+  if (int rc = check_device()) return rc;
+  const int L = S + t + 1;
+  if (!qkv || !kc || !vc || !pos || !ctx || !work || rows < 0 || t < 0 || S < 1 || L > T || !decode_attention_supported(L, H, heads))
+    return fail(TFSC_E_INVALID, "decode_attention: no kernel for %d rows, S = %d, t = %d, T = %d, hidden %d, heads %d (1 <= S + t + 1"
+                " <= min(T, %d), d %% 4 == 0, d <= 128)", rows, S, t, T, H, heads, kDecodeMaxKeys);
+  if (mask && mask_stride < S) return fail(TFSC_E_INVALID, "decode_attention: mask_stride %d is below S %d", mask_stride, S);
+  if (work_bytes < (int64_t)decode_attention_work_bytes(rows, L, H, heads))
+    return fail(TFSC_E_INVALID, "decode_attention: work_bytes %lld is below %lld", (long long)work_bytes,
+                (long long)decode_attention_work_bytes(rows, L, H, heads));
+  cudaError_t e = launch_decode_attention(qkv, kc, vc, pos, t, mask, mask_stride, S, T, ctx, rows, H, heads, work, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "decode_attention: %s", cudaGetErrorString(e));
+}
+int tfsc_k_generate_select(const float* logits, int64_t ld, int vocab, const int32_t* pos, int t, int last, int eos, int32_t* done,
+                           int32_t* ids, int64_t ids_ld, float* log_probs, int64_t lp_ld, int32_t* length, int64_t length_ld,
+                           const float* word, const float* pos_table, float* y, int rows, int H, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (!logits || !pos || !done || rows < 0 || t < 0 || vocab < 1 || vocab > kNextTokenMaxVocab || ld < vocab || H < 1 ||
+      (!last && (!word || !pos_table || !y)))
+    return fail(TFSC_E_INVALID, "generate_select: no kernel for %d rows of vocab = %d, ld = %lld, H = %d (1 <= vocab <= %d, ld >= vocab,"
+                " the tables and y unless last)", rows, vocab, (long long)ld, H, kNextTokenMaxVocab);
+  GenerateOutputs o;
+  o.ids = ids;
+  o.ids_ld = ids_ld;
+  o.log_probs = log_probs;
+  o.log_probs_ld = lp_ld;
+  o.length = length;
+  o.length_ld = length_ld;
+  cudaError_t e = launch_generate_select(logits, ld, vocab, pos, t, last != 0, eos, done, o, word, pos_table, y, rows, H,
+                                         (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "generate_select: %s", cudaGetErrorString(e));
+}
 int tfsc_debug_gemm_trace(long long*) {
   return fail(TFSC_E_UNIMPLEMENTED, "no GEMM clock trace: the persistent GEMM kernel it timed is not part of the sm_90a build");
 }

@@ -20,7 +20,8 @@ def _align256(x: int) -> int:
 # vocabulary (next-token); k is the entries' "k" (the same on every top-k or span result entry), or S for an encoder. The span result kinds also carry
 # "max_answer_length" and optionally "sep_id" (a graph bundle with a type_ids input, ending in [S, 1, 2] start / end
 # logits); cls_embedding and mean_embedding may carry "normalize": true; classes is one int64 (2 words) and
-# next_token_position one int32.
+# next_token_position one int32. The generate kinds (greedy generation on a GPT-2 bundle, n = the vocabulary) carry
+# "max_new_tokens" = N as their k, the same on every entry, and optionally "eos_token_id"; generated_length is one int32.
 OUTPUT_KIND_TABLE = {
     "logits": ("classify", "float32", "n"), "probabilities": ("classify", "float32", "n"), "classes": ("classify", "int64", ""),
     "top_k_classes": ("classify", "int32", "k"), "top_k_probabilities": ("classify", "float32", "k"),
@@ -32,10 +33,12 @@ OUTPUT_KIND_TABLE = {
     "masked_top_k_probabilities": ("fill_mask", "float32", "nk"), "masked_top_k_logits": ("fill_mask", "float32", "nk"),
     "next_token_position": ("next_token", "int32", ""), "next_token_top_k_ids": ("next_token", "int32", "k"),
     "next_token_top_k_probabilities": ("next_token", "float32", "k"), "next_token_top_k_logits": ("next_token", "float32", "k"),
+    "generated_ids": ("generate", "int32", "k"), "generated_log_probs": ("generate", "float32", "k"),
+    "generated_length": ("generate", "int32", ""),
 }
-OUTPUT_KINDS, SPAN_OUTPUT_KINDS, ENCODER_OUTPUT_KINDS, MLM_OUTPUT_KINDS, NEXT_TOKEN_OUTPUT_KINDS = (
+OUTPUT_KINDS, SPAN_OUTPUT_KINDS, ENCODER_OUTPUT_KINDS, MLM_OUTPUT_KINDS, NEXT_TOKEN_OUTPUT_KINDS, GENERATE_OUTPUT_KINDS = (
     tuple(k for k, v in OUTPUT_KIND_TABLE.items() if v[0] == head)
-    for head in ("classify", "span", "encoder", "fill_mask", "next_token"))
+    for head in ("classify", "span", "encoder", "fill_mask", "next_token", "generate"))
 
 
 def _signature(sig: dict, outputs):
@@ -50,12 +53,14 @@ def _signature(sig: dict, outputs):
 
 def _dims(o, n, seq):
     head, _dtype, dims = OUTPUT_KIND_TABLE[o["kind"]]
-    return [int(n if d == "n" else seq if head == "encoder" else o.get("k")) for d in dims]
+    k = o.get("max_new_tokens") if head == "generate" else o.get("k")
+    return [int(n if d == "n" else seq if head == "encoder" else k) for d in dims]
 
 
 def packed_output_layout(outputs, n, seq=None):
     """(name, element offset, width, dtype) of every output in a packed response row, in packed order (byte-wise sorted
-    names). Offsets and widths count 32-bit words: a kind's per-row dims (OUTPUT_KIND_TABLE) in n, the entry's "k" and,
+    names). Offsets and widths count 32-bit words: a kind's per-row dims (OUTPUT_KIND_TABLE) in n, the entry's "k" (or
+    "max_new_tokens") and,
     for the encoder kinds, seq = S; classes is one little-endian int64 in 2 words."""
     out, off = [], 0
     for o in sorted(outputs, key=lambda o: o["name"].encode()):
@@ -420,7 +425,9 @@ def gpt2_manifest(seq=1024, hidden=768, layers=12, heads=12, vocab=50257, max_po
     rounded up to a multiple of 32 with a zero bias, writes [B, 1, 1, Vp] logits (columns from vocab on are padding).
     With inputs=None the bundle takes the ids only and attends to every position; inputs=GPT2_INPUTS adds an
     "attention_mask" that hides keys whose mask is 0 and picks the last attended token. Positions are 0..seq-1 whatever
-    the padding, as transformers' default position ids. Every LayerNorm has eps 1e-5.
+    the padding, as transformers' default position ids. Every LayerNorm has eps 1e-5. With GENERATE_OUTPUT_KINDS outputs
+    (each entry with "max_new_tokens": N and optionally "eos_token_id") the same graph is a greedy generation bundle:
+    seq + N - 1 <= max_pos.
     Buffers: 0 residual stream, 1 normed / attention context, 2 qkv / MLP hidden, 3 post-attention residual."""
     ops = [{"op": "embed", "src": -1, "dst": 0, "h": seq, "w": 1, "c": hidden, "vocab": vocab, "max_pos": max_pos, "norm": False}]
 
