@@ -44,6 +44,7 @@ constexpr int CONSUMERS = CONS_WG * 128;
 constexpr int CONS_WARPS = CONSUMERS / 32;
 constexpr int THREADS = CONSUMERS + 32;    // warps 0..15 consumers, warp 16 TMA producer
 }  // namespace tc
+static_assert(tc::STRIP == kTcStripCols, "kernels.cu sizes the shared counter region with kTcStripCols");
 
 // smem (dynamic, 1024-aligned): NS stages of W (32 KB each, TMA target, layout [k/4][slab][k%4][32 n] with the
 // 128-byte swizzle), 2 buffers of B' = [x_hi ; x_lo] (2*RP rows x 128 B), then the mbarriers.

@@ -499,9 +499,17 @@ static DensePlan plan_dense(int k, int n) {
   return p;
 }
 
+// The arrival counters at the start of a dense workspace. One launch_dense runs its tensor-core passes (256-column strips)
+// and its <= 8-row split-K passes (512-column strips) on the same workspace, so the SIMT kernels' partials start past the
+// tensor-core plan's counters too: past 16,384 columns those take more than the first 256 bytes, and a SIMT pass would
+// otherwise leave its partial sums in the next tensor-core pass's counters.
+static size_t dense_counter_bytes(int n) {
+  return ((size_t)((n + kTcStripCols - 1) / kTcStripCols) * sizeof(unsigned int) + 255) & ~(size_t)255;
+}
+
 static size_t stream_workspace_bytes(int k, int n) {
   DensePlan p = plan_dense(k, n);
-  size_t counters = ((size_t)p.strips * sizeof(unsigned int) + 255) & ~(size_t)255;
+  size_t counters = dense_counter_bytes(n);
   size_t partials = (size_t)p.strips * p.splits * kMaxRowsPerLaunch * kStripCols * sizeof(float);
   return counters + partials;
 }
@@ -558,7 +566,7 @@ static cudaError_t launch_dense_r(const float* x, const float* w, const float* b
     attr_set[dev & 63] = true;
   }
   unsigned int* counters = static_cast<unsigned int*>(workspace);
-  size_t coff = ((size_t)p.strips * sizeof(unsigned int) + 255) & ~(size_t)255;
+  size_t coff = dense_counter_bytes(n);
   float* partials = reinterpret_cast<float*>(static_cast<char*>(workspace) + coff);
   dim3 grid(p.strips, p.splits);
   if (pdl_enabled()) {
@@ -596,7 +604,7 @@ static cudaError_t launch_dense_bulk_r(const float* x, const float* w, const flo
     attr_set[dev & 63] = true;
   }
   unsigned int* counters = static_cast<unsigned int*>(workspace);
-  size_t coff = ((size_t)p.strips * sizeof(unsigned int) + 255) & ~(size_t)255;
+  size_t coff = dense_counter_bytes(n);
   float* partials = reinterpret_cast<float*>(static_cast<char*>(workspace) + coff);
   dim3 grid(p.strips, p.splits);
   cudaError_t le = launch_maybe_pdl(dense_bulk_kernel<R, KL>, grid, kBulkColGroups * KL + 32, smem, s, x, w, bias, y, rows, k, n,

@@ -26,6 +26,8 @@ cudaError_t launch_dense(const float* x, const float* w, const float* bias, floa
 
 // X3: wgmma 3xTF32 path for 9..64 rows per pass (dense_tc.cu)
 bool dense_tc_supported(int rows, int k, int n, const float* w, const float* x, const float* bias, const float* y);
+// output columns per tensor-core strip: one arrival counter each at the start of a dense workspace (tc::STRIP)
+constexpr int kTcStripCols = 256;
 size_t dense_tc_workspace_bytes(int k, int n);
 cudaError_t launch_dense_tc(const float* x, const float* w, const float* bias, float* y, int rows, int k, int n,
                             bool relu, void* workspace, size_t workspace_bytes, cudaStream_t s);
