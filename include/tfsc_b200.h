@@ -138,6 +138,11 @@ uint32_t tfsc_crc32c(const void* data, size_t len);   /* CRC-32C (Castagnoli), t
  * tfsc_last_error(), or writes {"in_dim", "out_dim", "head_n", "head_k", "outputs": [{"name", "kind", "offset", "width",
  * "dtype"}]} (the packed response row of signature.outputs, offsets and widths in 32-bit words) and returns its strlen. */
 int tfsc_manifest_check(const char* manifest_json, char* buf, size_t cap);
+/* The packed input layout of a tfsc_model.json as its owner has it and as an ingress rank of the forward hop rebuilds it from
+ * the signature the owner sends: {"owner": L, "ingress": L}, L = {"in_dim", "out_dim", "inputs": [{"name", "role",
+ * "offset", "width"}]} (role: 0 ids, 1 mask, 2 type_ids, 3 seed). Needs no GPU; TFSC_E_INVALID for a manifest the loader
+ * refuses. */
+int tfsc_signature_roundtrip(const char* manifest_json, char* buf, size_t cap);
 
 /* ---------------------------------------------------------------- server (a6,a8,a10,X) ------
  * One server = the cache tier + proxy tier of cmd/taskhandler/main.go:45-113 for the GPUs of
@@ -486,6 +491,17 @@ int64_t tfsc_k_decode_attention_work_bytes(int rows, int L, int H, int heads);
 int tfsc_k_generate_select(const float* logits, int64_t ld, int vocab, const int32_t* pos, int t, int last, int eos, int32_t* done,
                            int32_t* ids, int64_t ids_ld, float* log_probs, int64_t lp_ld, int32_t* length, int64_t length_ld,
                            const float* word, const float* pos_table, float* y, int rows, int H, void* stream);
+/* One sampled step: tfsc_k_generate_select with g drawn instead of taken as the argmax. Of the tokens in rank order (logit
+ * descending, ties to the lower id) it keeps the first top_k (0: all), weights them exp((z - max z) / temperature), keeps the
+ * shortest prefix whose weight reaches top_p of theirs (1: all) and picks the first kept id, ascending, whose running weight
+ * exceeds u * W (W the kept weight, u = the 53-bit uniform of Philox4x32-10 with key (seeds[r * seed_stride], 0) and
+ * counter (t, 0, 0, 0)). top_k = 1 gives tfsc_k_generate_select's bits. The log-probability is logit[g] - logsumexp at
+ * temperature 1, unfiltered, the bits tfsc_k_generate_select writes for the same g. TFSC_E_INVALID outside its limits and
+ * unless temperature and its fp32 reciprocal are finite and > 0, 0 <= top_k <= vocab, 0 < top_p <= 1, seeds is given and seed_stride >= 1. */
+int tfsc_k_generate_sample(const float* logits, int64_t ld, int vocab, const int32_t* pos, int t, int last, int eos, int32_t* done,
+                           int32_t* ids, int64_t ids_ld, float* log_probs, int64_t lp_ld, int32_t* length, int64_t length_ld,
+                           const float* word, const float* pos_table, float* y, int rows, int H, const int32_t* seeds,
+                           int64_t seed_stride, float temperature, int top_k, float top_p, void* stream);
 
 #ifdef __cplusplus
 }

@@ -87,6 +87,7 @@ _sig("tfsc_disk_model_size", i64, cp, cp, i64)
 _sig("tfsc_savedmodel_convert", C.c_int, cp, cp)
 _sig("tfsc_crc32c", C.c_uint32, vp, sz)
 _sig("tfsc_manifest_check", C.c_int, cp, C.c_char_p, sz)
+_sig("tfsc_signature_roundtrip", C.c_int, cp, C.c_char_p, sz)
 _sig("tfsc_server_create", vp, cp)
 _sig("tfsc_server_destroy", None, vp)
 _sig("tfsc_server_num_nodes", C.c_int, vp)
@@ -158,6 +159,8 @@ _sig("tfsc_k_decode_attention", C.c_int, vp, vp, vp, vp, C.c_int, vp, C.c_int, C
 _sig("tfsc_k_decode_attention_work_bytes", C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int)
 _sig("tfsc_k_generate_select", C.c_int, vp, C.c_int64, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int64, vp, C.c_int64, vp,
      C.c_int64, vp, vp, vp, C.c_int, C.c_int, vp)
+_sig("tfsc_k_generate_sample", C.c_int, vp, C.c_int64, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int64, vp, C.c_int64, vp,
+     C.c_int64, vp, vp, vp, C.c_int, C.c_int, vp, C.c_int64, C.c_float, C.c_int, C.c_float, vp)
 
 
 class TfscError(RuntimeError):

@@ -236,9 +236,16 @@ void FwdSignature::to_desc(ModelDesc* d) const {
   d->input_shape = input_shape;
   d->output_shape = output_shape;
   d->inputs.clear();
-  const int64_t S = input_names.empty() ? 0 : in_dim / (int64_t)input_names.size();
-  for (size_t i = 0; i < input_names.size(); ++i)
-    d->inputs.push_back({input_names[i], (InputRole)input_roles[i], (int64_t)i * S});
+  // the widths follow from the roles (input_width): in_dim is S per token input plus 1 per seed
+  int64_t tokens = 0, seeds = 0;
+  for (size_t i = 0; i < input_names.size(); ++i) {
+    ModelInput mi;
+    mi.name = input_names[i];
+    mi.role = (InputRole)input_roles[i];
+    (mi.role == InputRole::Seed ? seeds : tokens)++;
+    d->inputs.push_back(mi);
+  }
+  place_inputs(&d->inputs, tokens ? (in_dim - seeds) / tokens : 0);
   // the ingress rank splits the packed response rows with the owner's layout rule (layout_outputs), never with its own manifest
   d->outputs.clear();
   d->head_n = head_n;
@@ -805,3 +812,32 @@ int Forwarder::forward(int peer, const std::string& name, int64_t version, const
 }
 
 }  // namespace tfsc
+
+// Offline check of the forward hop's signature (no device): the loader's packed input layout of a manifest, and the one an
+// ingress rank rebuilds from the signature the owner sends (from_desc, the wire encoding, to_desc).
+extern "C" int tfsc_signature_roundtrip(const char* manifest_json, char* buf, size_t cap) {
+  using namespace tfsc;
+  Json j;
+  ModelDesc d;
+  std::string err;
+  if (!manifest_json || !json_parse(manifest_json, &j, &err) || !parse_manifest(j, &d, &err))
+    return fail(TFSC_E_INVALID, "%s", err.empty() ? "signature_roundtrip: no manifest" : err.c_str());
+  Writer w;
+  write_sig(&w, FwdSignature::from_desc(d));
+  Reader r(w.b);
+  const FwdSignature s = read_sig(&r);
+  if (!r.ok) return fail(TFSC_E_INTERNAL, "signature_roundtrip: the signature does not decode");
+  ModelDesc f;
+  s.to_desc(&f);
+  auto layout = [](const ModelDesc& m) {
+    std::string o = "{\"in_dim\": " + std::to_string(m.in_dim) + ", \"out_dim\": " + std::to_string(m.out_dim) + ", \"inputs\": [";
+    for (size_t i = 0; i < m.inputs.size(); ++i) {
+      o += i ? ", {\"name\": " : "{\"name\": ";
+      json_escape(m.inputs[i].name, &o);
+      o += ", \"role\": " + std::to_string((int)m.inputs[i].role) + ", \"offset\": " + std::to_string(m.inputs[i].offset) +
+           ", \"width\": " + std::to_string(m.inputs[i].width) + "}";
+    }
+    return o + "]}";
+  };
+  return copy_out("{\"owner\": " + layout(d) + ", \"ingress\": " + layout(f) + "}", buf, cap);
+}

@@ -1,4 +1,4 @@
-// Greedy generation kernels of GPT-2 generate bundles, fp32, sm_90a: the copy of the prompt's keys and values into the KV
+// Generation kernels of GPT-2 generate bundles, fp32, sm_90a: the copy of the prompt's keys and values into the KV
 // cache, single-query attention over that cache, and the step that picks each row's token and embeds it for the next step.
 //
 // kv_cache_write_kernel: after each prefill attention op, copies the k | v columns of its packed qkv buffer [rows, S, 3H] to
@@ -15,6 +15,9 @@
 //
 // generate_select_kernel: one CTA per row, the next-token head's selection (head_select.cuh) with k = 1 and its fp64 sum of
 // exponentials for the log-probability, then the next step's input row wte[g] + wpe[slot] (embed_positions_kernel's add).
+//
+// generate_sample_kernel: the select step of sampling bundles. The same staging, maximum and log-probability, then a token
+// drawn from the temperature / top-k / top-p distribution with the row's seed (sample_token), written as the select step's.
 #include <cuda_runtime.h>
 
 #include <atomic>
@@ -240,6 +243,36 @@ cudaError_t launch_decode_attention(const float* qkv, float* kc, float* vc, cons
                           ctx, H, heads, counters, part);
 }
 
+// The select and sample steps' writes for row `row` and its token g (the sentinel INT_MAX of a NaN row clamped to an id): the
+// outputs, the done flag and, unless last, the next step's input word[g] + pos_table[p + 1 + t]
+template <bool kVec>
+__device__ __forceinline__ void generate_write(int64_t row, int t, int p, bool live, int g, const float* xs, int vocab, float m,
+                                               double sum, bool last, int eos, int* __restrict__ done, const GenerateOutputs& o,
+                                               const float* __restrict__ word, const float* __restrict__ pos_table,
+                                               float* __restrict__ y, int H) {
+  // g < vocab for finite logits; a NaN row can leave the sentinel INT_MAX, which must not index shared memory or a table
+  const int gc = g < 0 ? 0 : (g >= vocab ? vocab - 1 : g);
+  if (threadIdx.x == 0) {
+    if (o.ids) o.ids[row * o.ids_ld + t] = live ? g : -1;
+    if (o.log_probs) o.log_probs[row * o.log_probs_ld + t] = live ? (xs[gc] - m) - (float)log(sum) : 0.f;
+    if (o.length && (live || t == 0)) o.length[row * o.length_ld] = live ? t + 1 : 0;
+    if (live || t == 0) done[row] = !live || g == eos;
+  }
+  if (last) return;
+  const int64_t slot = p + 1 + t;  // where the token goes: its position embedding
+  if (kVec) {
+    const float4* w = reinterpret_cast<const float4*>(word + (int64_t)gc * H);
+    const float4* pe = reinterpret_cast<const float4*>(pos_table + slot * H);
+    float4* dst = reinterpret_cast<float4*>(y + row * H);
+    for (int c = threadIdx.x; c < (H >> 2); c += blockDim.x) {
+      const float4 a = __ldg(w + c), b = __ldg(pe + c);
+      dst[c] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+    }
+  } else {
+    for (int c = threadIdx.x; c < H; c += blockDim.x) y[row * H + c] = __ldg(word + (int64_t)gc * H + c) + __ldg(pos_table + slot * H + c);
+  }
+}
+
 template <bool kVec>
 __global__ void __launch_bounds__(kHeadThreadsMax) generate_select_kernel(const float* __restrict__ logits, int64_t ld, int vocab,
                                                                           const int* __restrict__ pos, int t, bool last, int eos,
@@ -262,27 +295,7 @@ __global__ void __launch_bounds__(kHeadThreadsMax) generate_select_kernel(const 
   const bool live = t == 0 ? p >= 0 : done[row] == 0;
   const float m = head_stage_select(logits + row * ld, vocab, 1, xs, wv, wi, &s_v, &s_i, sel);
   const double sum = head_exp_sum(xs, vocab, m, wsum, &s_sum);
-  // g < vocab for finite logits; a NaN row can leave the sentinel INT_MAX, which must not index shared memory or a table
-  const int g = sel[0], gc = g < 0 ? 0 : (g >= vocab ? vocab - 1 : g);
-  if (threadIdx.x == 0) {
-    if (o.ids) o.ids[row * o.ids_ld + t] = live ? g : -1;
-    if (o.log_probs) o.log_probs[row * o.log_probs_ld + t] = live ? (xs[gc] - m) - (float)log(sum) : 0.f;
-    if (o.length && (live || t == 0)) o.length[row * o.length_ld] = live ? t + 1 : 0;
-    if (live || t == 0) done[row] = !live || g == eos;
-  }
-  if (last) return;
-  const int64_t slot = p + 1 + t;  // where the token goes: its position embedding
-  if (kVec) {
-    const float4* w = reinterpret_cast<const float4*>(word + (int64_t)gc * H);
-    const float4* pe = reinterpret_cast<const float4*>(pos_table + slot * H);
-    float4* dst = reinterpret_cast<float4*>(y + row * H);
-    for (int c = threadIdx.x; c < (H >> 2); c += blockDim.x) {
-      const float4 a = __ldg(w + c), b = __ldg(pe + c);
-      dst[c] = make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
-    }
-  } else {
-    for (int c = threadIdx.x; c < H; c += blockDim.x) y[row * H + c] = __ldg(word + (int64_t)gc * H + c) + __ldg(pos_table + slot * H + c);
-  }
+  generate_write<kVec>(row, t, p, live, sel[0], xs, vocab, m, sum, last, eos, done, o, word, pos_table, y, H);
 }
 
 cudaError_t launch_generate_select(const float* logits, int64_t ld, int vocab, const int* pos, int t, bool last, int eos,
@@ -311,6 +324,269 @@ cudaError_t launch_generate_select(const float* logits, int64_t ld, int vocab, c
                           done, o, word, pos_table, y, H)
              : launch_pdl(generate_select_kernel<false>, dim3((unsigned)rows), threads, smem, s, logits, ld, vocab, pos, t, last, eos,
                           done, o, word, pos_table, y, H);
+}
+
+// ------------------------------------------------------------------------------------------------- sampling ----
+typedef unsigned long long u64;
+
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC 2011) of counter c under key (k0, k1)
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r) k0 += 0x9E3779B9u, k1 += 0xBB67AE85u;
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+  }
+  return c;
+}
+
+// An order-preserving key of a logit: larger logits have larger keys and -0 ranks as +0, so (key descending, id ascending)
+// is the next-token head's rank order for every non-NaN logit
+__device__ __forceinline__ uint32_t rank_key(float z) {
+  uint32_t u = __float_as_uint(z);
+  if (u == 0x80000000u) u = 0;
+  return (u & 0x80000000u) ? ~u : u | 0x80000000u;
+}
+
+// A token's sampling weight exp((z - m) / temperature) in [0, 1] as a fixed-point integer of 2^-46 units, so that every sum
+// of weights is exact and does not depend on its order: 57344 of them stay below 2^62. NaN and inf give 0. inv_t is
+// 1 / temperature in fp32, rounded once on the host: a division here would call fp32 division's slow path.
+__device__ __forceinline__ u64 weight_q(float z, float m, float inv_t) {
+  const float w = expf((z - m) * inv_t);
+  return w > 0.f ? __float2ull_rz(fminf(w, 1.f) * 0x1p46f) : 0ull;
+}
+
+// hist[b] = the sum of val(key, j) over the staged logits whose key agrees with `prefix` above bit shift + 8, b the key's
+// byte at `shift`. Lanes with the same bin add their values first (integers: exact), then one shared atomic per bin.
+template <typename Val>
+__device__ __forceinline__ void radix_hist(const float* xs, int n, int shift, uint32_t prefix, Val val, u64* hist) {
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0;
+  __syncthreads();
+  const uint32_t above = shift == 24 ? 0u : ~0u << (shift + 8);
+  const int lane = threadIdx.x & 31;
+  for (int j = threadIdx.x; j - lane < n; j += blockDim.x) {  // warp-uniform trip count: every lane reaches the match
+    int bin = 256;
+    u64 v = 0;
+    if (j < n) {
+      const uint32_t key = rank_key(xs[j]);
+      if (((key ^ prefix) & above) == 0) v = val(key, j);
+      if (v) bin = (key >> shift) & 255;
+    }
+    if (!__any_sync(0xffffffffu, bin < 256)) continue;  // past the first pass most warps hold no element of the prefix
+    const unsigned peers = __match_any_sync(0xffffffffu, bin);
+    // v < 2^47: two 23-bit halves, each summed over at most 32 lanes without overflow
+    const unsigned lo = __reduce_add_sync(peers, (unsigned)(v & 0x7fffff)), hi = __reduce_add_sync(peers, (unsigned)(v >> 23));
+    if (bin < 256 && lane == __ffs(peers) - 1) atomicAdd(&hist[bin], ((u64)hi << 23) + lo);
+  }
+  __syncthreads();
+}
+
+struct RadixPick {
+  int bin;     // -1: the histogram holds less than need
+  u64 before;  // the sum of the bins above it
+  u64 count;   // its own
+  u64 need;
+};
+
+// Warp 0 finds the highest bin b whose suffix sum hist[b..255] reaches need; frac > 0 sets need = ceil(frac * total), at
+// least 1. Lane l sums bins 255 - 8l down to 248 - 8l, the lanes scan in that order. Every thread gets the result.
+__device__ __forceinline__ RadixPick radix_pick(const u64* hist, u64 need, double frac, RadixPick* s_pick) {
+  if (threadIdx.x < 32) {
+    const int lane = threadIdx.x;
+    u64 mine = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) mine += hist[255 - 8 * lane - i];
+    u64 incl = mine;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const u64 u = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += u;
+    }
+    const u64 total = __shfl_sync(0xffffffffu, incl, 31);
+    if (frac > 0.0) need = total ? min(total, max(1ull, (u64)ceil(frac * (double)total))) : 0;
+    if (lane == 0) s_pick->bin = -1, s_pick->need = need;
+    __syncwarp();
+    if (need >= 1 && incl >= need && incl - mine < need) {
+      u64 acc = incl - mine;
+      for (int i = 0; i < 8; ++i) {
+        const int b = 255 - 8 * lane - i;
+        if (acc + hist[b] >= need) {
+          s_pick->bin = b, s_pick->before = acc, s_pick->count = hist[b];
+          break;
+        }
+        acc += hist[b];
+      }
+    }
+  }
+  __syncthreads();
+  const RadixPick r = *s_pick;
+  __syncthreads();
+  return r;
+}
+
+// The first j in [0, n) at which the running sum of v(j) over ascending j exceeds target(total), total the sum over all of
+// [0, n); -1 when none does. Each thread sums a contiguous chunk of ids, the chunk sums are scanned in thread order and the
+// thread whose chunk holds the crossing walks it. scan: kHeadThreadsMax / 32 words of shared memory.
+template <typename V, typename Target>
+__device__ __forceinline__ int chunk_find(int n, V v, Target target, u64* scan, int* s_res) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  const int c = (n + blockDim.x - 1) / blockDim.x, lo = min(n, (int)threadIdx.x * c), hi = min(n, lo + c);
+  u64 mine = 0;
+  for (int j = lo; j < hi; ++j) mine += v(j);
+  u64 incl = mine;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const u64 u = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += u;
+  }
+  if (lane == 31) scan[warp] = incl;
+  if (threadIdx.x == 0) *s_res = -1;
+  __syncthreads();
+  if (warp == 0) {
+    u64 w = lane < nwarps ? scan[lane] : 0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const u64 u = __shfl_up_sync(0xffffffffu, w, o);
+      if (lane >= o) w += u;
+    }
+    if (lane < nwarps) scan[lane] = w;
+  }
+  __syncthreads();
+  const u64 total = scan[nwarps - 1], tg = target(total), before = (warp ? scan[warp - 1] : 0) + incl - mine;
+  if (tg < total && before <= tg && tg < before + mine) {
+    u64 acc = before;
+    for (int j = lo; j < hi; ++j)
+      if ((acc += v(j)) > tg) {
+        *s_res = j;
+        break;
+      }
+  }
+  __syncthreads();
+  const int r = *s_res;
+  __syncthreads();
+  return r;
+}
+
+// The sampled token of the staged row (DESIGN §3): the rank-order top_k (0: all) and the shortest rank-order prefix of those
+// whose weight reaches top_p of theirs (1: all), then the first kept id, ascending, whose running weight exceeds u * W, W
+// the kept weight and u the 53-bit uniform of Philox4x32-10 with key (seed, 0) and counter (t, 0, 0, 0). The kept set is
+// a rank threshold: key > kt, or key == kt and id <= it. Top-k and top-p boundaries are radix selections over the keys,
+// their ties cut in id order; every sum is an integer, so the token is a function of the logits' bits, seed and t.
+__device__ __forceinline__ int sample_token(const float* xs, int vocab, float m, float inv_t, int top_k, float top_p,
+                                            uint32_t seed, int t, u64* hist, RadixPick* s_pick, int* s_res) {
+  uint32_t kt = 0;
+  int it = INT_MAX;
+  auto kept = [&](uint32_t key, int j) { return key > kt || (key == kt && j <= it); };
+  if (top_k > 0 && top_k < vocab) {
+    uint32_t prefix = 0;
+    RadixPick r = {};
+    u64 need = (u64)top_k;
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      radix_hist(xs, vocab, shift, prefix, [](uint32_t, int) { return 1ull; }, hist);
+      r = radix_pick(hist, need, 0.0, s_pick);
+      prefix |= (uint32_t)r.bin << shift;
+      need -= r.before;
+    }
+    kt = prefix;
+    if (r.count != need) {  // the need-th lowest id among the ties at the boundary
+      const uint32_t k = prefix;
+      it = chunk_find(vocab, [&](int j) { return (u64)(rank_key(xs[j]) == k); }, [&](u64) { return need - 1; }, hist, s_res);
+    }
+  }
+  if (top_p < 1.f) {
+    uint32_t prefix = 0;
+    RadixPick r = {};
+    u64 need = 0;
+    bool none = false;
+    for (int shift = 24; shift >= 0 && !none; shift -= 8) {
+      radix_hist(xs, vocab, shift, prefix, [&](uint32_t key, int j) { return kept(key, j) ? weight_q(xs[j], m, inv_t) : 0ull; },
+                 hist);
+      r = radix_pick(hist, need, shift == 24 ? (double)top_p : 0.0, s_pick);
+      none = r.bin < 0;  // no kept weight at all (NaN or inf logits): top-p keeps the top-k set
+      if (shift == 24) need = r.need;
+      prefix |= (uint32_t)(r.bin & 255) << shift;
+      need -= none ? 0 : r.before;
+    }
+    if (!none) {
+      const uint32_t k = prefix;
+      const int cut = chunk_find(
+          vocab, [&](int j) { return rank_key(xs[j]) == k && kept(k, j) ? weight_q(xs[j], m, inv_t) : 0ull; },
+          [&](u64) { return need - 1; }, hist, s_res);
+      kt = k, it = cut < 0 ? it : cut;
+    }
+  }
+  const uint4 x = philox4x32_10(make_uint4((uint32_t)t, 0, 0, 0), seed, 0);
+  const u64 U = ((u64)(x.x >> 5) << 26) | (x.y >> 6);  // u = U * 2^-53
+  int g = chunk_find(
+      vocab, [&](int j) { return kept(rank_key(xs[j]), j) ? weight_q(xs[j], m, inv_t) : 0ull; },
+      [&](u64 W) { return (__umul64hi(U, W) << 11) | ((U * W) >> 53); }, hist, s_res);  // floor(u * W)
+  if (g < 0)  // no kept weight: the last kept id
+    g = chunk_find(vocab, [&](int j) { return (u64)kept(rank_key(xs[j]), j); }, [](u64 n) { return n - 1; }, hist, s_res);
+  return g;
+}
+
+template <bool kVec>
+__global__ void __launch_bounds__(kHeadThreadsMax) generate_sample_kernel(const float* __restrict__ logits, int64_t ld, int vocab,
+                                                                          const int* __restrict__ pos, int t, bool last, int eos,
+                                                                          int* __restrict__ done, GenerateOutputs o,
+                                                                          const float* __restrict__ word,
+                                                                          const float* __restrict__ pos_table, float* __restrict__ y,
+                                                                          int H, const int* __restrict__ seeds, int64_t seed_stride,
+                                                                          float inv_t, int top_k, float top_p) {
+  extern __shared__ float xs[];  // the row's vocab logits
+  __shared__ float wv[kHeadThreadsMax / 32];
+  __shared__ int wi[kHeadThreadsMax / 32];
+  __shared__ double wsum[kHeadThreadsMax / 32];
+  __shared__ float s_v;
+  __shared__ int s_i;
+  __shared__ double s_sum;
+  __shared__ int sel[1];
+  __shared__ u64 hist[256];  // the radix histograms and the id-order scans, one at a time: 2 KB beside 224 KB of logits
+  __shared__ RadixPick s_pick;
+  __shared__ int s_res;
+  const int64_t row = blockIdx.x;
+  // launched after the vocabulary projection; done comes from the previous step's launch
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  const int p = __ldg(pos + row);
+  const bool live = t == 0 ? p >= 0 : done[row] == 0;
+  const float m = head_stage_select(logits + row * ld, vocab, 1, xs, wv, wi, &s_v, &s_i, sel);
+  const double sum = head_exp_sum(xs, vocab, m, wsum, &s_sum);
+  // top_k = 1 is the greedy token; the log-probability is the model's, at temperature 1 and unfiltered, as greedy's
+  const int g = top_k == 1 ? sel[0]
+                           : sample_token(xs, vocab, m, inv_t, top_k, top_p, (uint32_t)__ldg(seeds + row * seed_stride), t,
+                                          hist, &s_pick, &s_res);
+  generate_write<kVec>(row, t, p, live, g, xs, vocab, m, sum, last, eos, done, o, word, pos_table, y, H);
+}
+
+cudaError_t launch_generate_sample(const float* logits, int64_t ld, int vocab, const int* pos, int t, bool last, int eos,
+                                   int* done, const GenerateOutputs& o, const float* word, const float* pos_table, float* y,
+                                   int rows, int H, const int* seeds, int64_t seed_stride, float temperature, int top_k,
+                                   float top_p, cudaStream_t s) {
+  if (rows < 0 || t < 0 || vocab < 1 || vocab > kNextTokenMaxVocab || ld < vocab || H < 1 || !logits || !pos || !done ||
+      (!last && (!word || !pos_table || !y)) || !seeds || seed_stride < 1 || !sampling_supported(vocab, temperature, top_k, top_p))
+    return cudaErrorInvalidValue;
+  if (rows == 0) return cudaSuccess;
+  static bool attr[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (!attr[dev & 63]) {
+    for (cudaError_t e : {cudaFuncSetAttribute(generate_sample_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               kNextTokenMaxVocab * (int)sizeof(float)),
+                          cudaFuncSetAttribute(generate_sample_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               kNextTokenMaxVocab * (int)sizeof(float))})
+      if (e != cudaSuccess) return e;
+    attr[dev & 63] = true;
+  }
+  const bool vec = H % 4 == 0 && (((uintptr_t)word | (uintptr_t)pos_table | (uintptr_t)y) & 15) == 0;
+  const size_t smem = (size_t)vocab * sizeof(float);
+  // the select step's block size: its maximum and sum of exponentials, so its log-probabilities, are the same bits
+  const int threads = head_threads(vocab);
+  const float inv_t = 1.f / temperature;
+  return vec ? launch_pdl(generate_sample_kernel<true>, dim3((unsigned)rows), threads, smem, s, logits, ld, vocab, pos, t, last, eos,
+                          done, o, word, pos_table, y, H, seeds, seed_stride, inv_t, top_k, top_p)
+             : launch_pdl(generate_sample_kernel<false>, dim3((unsigned)rows), threads, smem, s, logits, ld, vocab, pos, t, last, eos,
+                          done, o, word, pos_table, y, H, seeds, seed_stride, inv_t, top_k, top_p);
 }
 
 }  // namespace tfsc

@@ -43,9 +43,15 @@ std::string expected_inputs(const ModelDesc& d) {
 }
 
 bool check_layout(const ModelDesc& d, const InputLayout& l, std::string* err) {
+  // every input but a seed holds S values per row (input_width); a seed's [batch, 1] is named after the rest
+  const ModelInput* tokens = nullptr;
+  std::string seeds;
+  for (auto& mi : d.inputs)
+    if (mi.role == InputRole::Seed) seeds += ", '" + mi.name + "' DT_INT32 [batch, 1]";
+    else tokens = &mi;
   auto bad = [&](const std::string& why) {
     *err = why + "; model expects input" + (d.inputs.size() > 1 ? "s " : " ") + expected_inputs(d) +
-           (d.inputs.empty() ? "" : ", DT_INT32 [batch, " + std::to_string(d.in_dim / (int64_t)d.inputs.size()) + "] each");
+           (d.inputs.empty() ? "" : ", DT_INT32 [batch, " + std::to_string(tokens ? tokens->width : 0) + "] each" + seeds);
     return false;
   };
   if (!l.error.empty()) return bad(l.error);
@@ -53,7 +59,6 @@ bool check_layout(const ModelDesc& d, const InputLayout& l, std::string* err) {
     if (l.multi()) return bad("the request names " + std::to_string(l.names.size()) + " inputs");
     return true;  // one tensor for one input: the single-input checks of Node::prepare and the front-ends apply
   }
-  const int64_t S = d.in_dim / (int64_t)d.inputs.size();
   for (auto& mi : d.inputs)
     if (std::find(l.names.begin(), l.names.end(), mi.name) == l.names.end()) return bad("input '" + mi.name + "' is missing");
   for (auto& n : l.names) {
@@ -62,9 +67,10 @@ bool check_layout(const ModelDesc& d, const InputLayout& l, std::string* err) {
     if (!known) return bad(n.empty() ? std::string("an unnamed input") : "input '" + n + "' is not in the model signature");
   }
   if (l.dtype != TFSC_DT_INT32) return bad("the inputs must be DT_INT32");
-  for (size_t i = 0; i < l.names.size(); ++i)
-    if (l.row_elems[i] != S)
-      return bad("input '" + l.names[i] + "' has " + std::to_string(l.row_elems[i]) + " values per row, not " + std::to_string(S));
+  for (size_t i = 0; i < l.names.size(); ++i)  // the names are the declared ones, both in sorted order
+    if (l.row_elems[i] != d.inputs[i].width)
+      return bad("input '" + l.names[i] + "' has " + std::to_string(l.row_elems[i]) + " values per row, not " +
+                 std::to_string(d.inputs[i].width));
   if (l.rows <= 0) return bad("the request has no rows");
   return true;
 }

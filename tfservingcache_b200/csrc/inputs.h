@@ -1,7 +1,7 @@
 // Request inputs -> the packed request row. A single-input model takes one tensor whose rows are in_dim values each, as
 // always. A multi-input model (signature.inputs, e.g. BERT's input_ids / input_mask / segment_ids) takes one int32 tensor
-// per declared input, [B, S] (or [S] for one row), and its request row is the concatenation of the inputs' rows in
-// byte-wise sorted NAME order. The order depends on the names only, so the ingress rank of a forward hop packs a request
+// per declared input, [B, S] (or [S] for one row; a seed [B, 1] or [1]: input_width), and its request row is the
+// concatenation of the inputs' rows in byte-wise sorted NAME order. The order depends on the names only, so the ingress rank of a forward hop packs a request
 // without the owner's manifest; the owner checks the layout against its manifest (check_layout) before anything runs.
 #pragma once
 #include <string>
@@ -36,7 +36,8 @@ struct InputLayout {
 InputLayout layout_inputs(std::vector<InTensor>* ts);
 
 // The owner's check of a layout against the model: for a multi-input model the names must be exactly the declared ones
-// and every row S values; a single-input model takes one tensor. Messages list the expected input names.
+// and every row its input's width values (S, 1 for a seed); a single-input model takes one tensor. Messages list the
+// expected input names.
 bool check_layout(const ModelDesc& d, const InputLayout& l, std::string* err);
 
 // "'input_ids', 'input_mask', 'segment_ids'" (or the single input's name)

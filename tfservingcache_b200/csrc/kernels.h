@@ -216,6 +216,14 @@ struct GenerateOutputs {
 cudaError_t launch_generate_select(const float* logits, int64_t ld, int vocab, const int* pos, int t, bool last, int eos,
                                    int* done, const GenerateOutputs& o, const float* word, const float* pos_table, float* y,
                                    int rows, int H, cudaStream_t s);
+// One sampled step per row: launch_generate_select with g drawn from the row's logits at temperature, top_k and top_p with
+// the seed seeds[r * seed_stride] (DESIGN §3); top_k = 1 is the greedy token. The log-probability is the model's,
+// logit[g] - logsumexp(logits[:vocab]), the bits launch_generate_select gives for the same g. A row's token depends on its
+// logits' bits, seed and t only. cudaErrorInvalidValue outside sampling_supported (nn_limits.h) or for seed_stride < 1.
+cudaError_t launch_generate_sample(const float* logits, int64_t ld, int vocab, const int* pos, int t, bool last, int eos,
+                                   int* done, const GenerateOutputs& o, const float* word, const float* pos_table, float* y,
+                                   int rows, int H, const int* seeds, int64_t seed_stride, float temperature, int top_k,
+                                   float top_p, cudaStream_t s);
 
 // wgmma 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
 bool gemm_tc_supported(const float* A, const float* B, const float* bias, const float* R, const float* C, int M, int N, int K,

@@ -1,12 +1,23 @@
 #include "model.h"
 
 #include <algorithm>
+#include <cmath>
 
 #include "nn_limits.h"
 
 namespace tfsc {
 
 static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+int64_t place_inputs(std::vector<ModelInput>* inputs, int64_t S) {
+  int64_t off = 0;
+  for (auto& i : *inputs) {
+    i.offset = off;
+    i.width = input_width(i.role, S);
+    off += i.width;
+  }
+  return off;
+}
 
 size_t ModelDesc::scratch_bytes(int64_t rows) const {
   // an mlp's head reads the last layer's logits from the activation buffer that layer would have used, so only graph
@@ -220,7 +231,7 @@ static void finish(ModelDesc* d) {
   if (d->tmpl == Template::Graph) {
     d->in_dim = 1;
     for (auto v : d->input_shape) d->in_dim *= v;
-    if (!d->inputs.empty()) d->in_dim *= (int64_t)d->inputs.size();  // the packed row: S values per declared input
+    if (!d->inputs.empty()) d->in_dim = place_inputs(&d->inputs, d->in_dim);  // the packed row: the inputs' rows of S (or 1)
     d->out_dim = 1;
     for (auto v : d->output_shape) d->out_dim *= v;
     return;
@@ -269,12 +280,50 @@ ModelDesc make_affine_desc() {
   return d;
 }
 
+// A generate entry's "temperature" (finite, > 0), "top_k" (an integer >= 0; <= vocab is checked with the bundle) and "top_p"
+// (in (0, 1]), each the same on every entry that gives it: *temperature / *top_p NaN and *top_k -1 until one does
+static bool parse_sampling(const Json& oj, const std::string& name, double* temperature, int* top_k, double* top_p, std::string* err) {
+  const std::string at = "signature.outputs: '" + name + "' has a ";
+  auto differs = [&](const char* field) {
+    *err = at + "'" + field + "' that differs from the other generate outputs'";
+    return false;
+  };
+  if (const Json* f = oj.get("temperature")) {
+    if (f->type != Json::Num || !sampling_temperature_ok(f->num)) {
+      *err = at + "'temperature' that is not a finite number > 0 with a finite fp32 reciprocal";
+      return false;
+    }
+    if (!std::isnan(*temperature) && f->num != *temperature) return differs("temperature");
+    *temperature = f->num;
+  }
+  if (const Json* f = oj.get("top_k")) {
+    if (f->type != Json::Num || f->num != std::floor(f->num) || f->num < 0 || f->num > 0x7fffffff) {
+      *err = at + "'top_k' that is not an integer >= 0 (0: off)";
+      return false;
+    }
+    if (*top_k >= 0 && (int)f->num != *top_k) return differs("top_k");
+    *top_k = (int)f->num;
+  }
+  if (const Json* f = oj.get("top_p")) {
+    if (f->type != Json::Num || !(f->num > 0 && f->num <= 1) || !((float)f->num > 0)) {
+      *err = at + "'top_p' outside (0, 1] (1: off)";
+      return false;
+    }
+    if (!std::isnan(*top_p) && f->num != *top_p) return differs("top_p");
+    *top_p = f->num;
+  }
+  return true;
+}
+
 // signature.outputs, one entry at a time. An entry is refused for, in this order: an unknown kind, no name, a duplicate, a
 // mix of heads (fill-mask, then encoder, then span: the message names the later entry's head), a 'normalize' on a kind
 // without one, and then the fields its head takes. Sets d->head.
 static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
   int k = -1, max_len = -1, sep_id = -1, max_new = -1, eos = -1;
   bool span_seen = false;  // a span_starts / span_ends / span_scores entry set max_len and sep_id
+  // a generate bundle's sampling fields, NaN / -1 until an entry gives them
+  double temperature = NAN, top_p = NAN;
+  int top_k = -1;
   // an integer field of an output entry: 0 absent, 1 read into *v, -1 present but not an integer
   auto int_field = [](const Json& oj, const char* key, int* v) {
     const Json* f = oj.get(key);
@@ -406,6 +455,7 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
           return false;
         }
         if (v >= 0) eos = v;
+        if (!parse_sampling(oj, mo.name, &temperature, &top_k, &top_p, err)) return false;
         break;
       case HeadKind::Encoder:
         if (oj.get("k") || span_fields) {
@@ -455,6 +505,10 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
   }
   d->head_k = span_seen ? k : max_new >= 0 ? max_new : k < 0 ? 0 : k;  // a span k is always given, and a negative one is refused by span_fits
   d->gen_eos = eos;
+  d->gen_sampling = !std::isnan(temperature) || top_k >= 0 || !std::isnan(top_p);
+  d->gen_temperature = std::isnan(temperature) ? 1.f : (float)temperature;
+  d->gen_top_k = top_k < 0 ? 0 : top_k;
+  d->gen_top_p = std::isnan(top_p) ? 1.f : (float)top_p;
   d->span_max_len = span_seen ? max_len : 0;
   d->span_sep_id = sep_id;
   set_head(d);
@@ -671,6 +725,15 @@ static bool check_generate_bundle(ModelDesc* d, int last_tokens, std::string* er
     *err = "signature.outputs: eos_token_id = " + std::to_string(d->gen_eos) + " is not below vocab = " + std::to_string(V);
     return false;
   }
+  if (d->gen_top_k > V) {
+    *err = "signature.outputs: top_k = " + std::to_string(d->gen_top_k) + " exceeds vocab = " + std::to_string(V);
+    return false;
+  }
+  if (d->gen_sampling && !d->input(InputRole::Seed)) {
+    *err = "signature.outputs: a sampling generate bundle (temperature, top_k or top_p) needs an input with the role 'seed'"
+           " (int32 [batch, 1])";
+    return false;
+  }
   d->head_n = V;
   return true;
 }
@@ -863,6 +926,7 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
         if (role == "ids") mi.role = InputRole::Ids;
         else if (role == "mask") mi.role = InputRole::Mask;
         else if (role == "type_ids") mi.role = InputRole::TypeIds;
+        else if (role == "seed") mi.role = InputRole::Seed;
         else {
           *err = "signature.inputs: unknown role '" + role + "' (ids, mask, type_ids)";
           return false;
@@ -1120,8 +1184,6 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
       *err = "signature.inputs: an embed op with norm false reads no type_ids input";
       return false;
     }
-    const int64_t S = d->ops.front().h;
-    for (size_t i = 0; i < d->inputs.size(); ++i) d->inputs[i].offset = (int64_t)i * S;
   }
   finish(d);
   int gathers = 0, last_tokens = 0;
@@ -1136,7 +1198,14 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
            "next_token_top_k_probabilities, next_token_top_k_logits)";
     return false;
   }
-  if (d->outputs.empty()) return true;
+  // a seed feeds the sampling step only, after the head's own checks (the generate head's refuse a sampling bundle without one)
+  auto seed_ok = [&] {
+    if (!d->input(InputRole::Seed) || (d->head == HeadKind::Generate && d->gen_sampling)) return true;
+    *err = "signature.inputs: a 'seed' input belongs to sampling generate bundles (generate outputs with temperature, top_k"
+           " or top_p)";
+    return false;
+  };
+  if (d->outputs.empty()) return seed_ok();
   bool ok = false;
   switch (d->head) {
     case HeadKind::Generate: ok = check_generate_bundle(d, last_tokens, err); break;
@@ -1146,7 +1215,7 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
     case HeadKind::Span: ok = check_span_bundle(d, err); break;
     default: ok = check_classify_bundle(d, err);
   }
-  if (!ok) return false;
+  if (!ok || !seed_ok()) return false;
   for (auto& o : d->outputs) {
     bool clash = d->inputs.empty() && o.name == d->input_name;
     for (auto& i : d->inputs) clash = clash || o.name == i.name;

@@ -53,13 +53,19 @@ struct ExtraSignature {
   std::string feature;
 };
 
-// One declared input of a multi-input graph bundle (signature.inputs): BERT's input_ids / input_mask / segment_ids.
-enum class InputRole { Ids, Mask, TypeIds };
+// One declared input of a multi-input graph bundle (signature.inputs): BERT's input_ids / input_mask / segment_ids, and a
+// sampling generate bundle's per-request seed. New roles go at the end: the forward hop sends the enum's numbers.
+enum class InputRole { Ids, Mask, TypeIds, Seed };
 struct ModelInput {
   std::string name;
   InputRole role = InputRole::Ids;
-  int64_t offset = 0;  // elements into the packed request row (inputs in byte-wise sorted name order, S values each)
+  int64_t offset = 0;  // elements into the packed request row (inputs in byte-wise sorted name order, `width` values each)
+  int64_t width = 0;   // values per row: input_width
 };
+// The one rule for how many int32 values per row an input of `role` holds in a bundle of S tokens: S, or 1 for a seed
+inline int64_t input_width(InputRole role, int64_t S) { return role == InputRole::Seed ? 1 : S; }
+// Sets the width (input_width) and offset of every input, in packed order, and returns the packed row's width
+int64_t place_inputs(std::vector<ModelInput>* inputs, int64_t S);
 
 // The head that computes a bundle's signature.outputs; every output of a bundle belongs to the same one (None: no outputs).
 // Classify: the last op's N logits (head.cu). Span (question answering): the last op's [S, 1, 2] per-token start / end
@@ -139,7 +145,8 @@ struct ModelDesc {
   // span_sep_id = sep_id (-1: none); an encoder head's encoder_pooler (the last op is the pooler: it writes pooled_output,
   // and the hidden states are its source buffer) and normalize_cls / normalize_mean; a fill-mask head's mlm_vocab (the
   // embed op's vocab, the logits the head reads of each Vp-wide row) and mlm_mask_token_id; a generate head's gen_eos
-  // (eos_token_id, -1: none).
+  // (eos_token_id, -1: none) and, on a sampling bundle (gen_sampling: a generate entry gave temperature, top_k or top_p),
+  // gen_temperature (1), gen_top_k (0: off) and gen_top_p (1: off).
   std::vector<ModelOutput> outputs;
   HeadKind head = HeadKind::None;
   int head_n = 0, head_k = 0;
@@ -147,6 +154,9 @@ struct ModelDesc {
   bool encoder_pooler = false, normalize_cls = false, normalize_mean = false;
   int mlm_vocab = 0, mlm_mask_token_id = 0;
   int gen_eos = -1;
+  bool gen_sampling = false;
+  float gen_temperature = 1.f, gen_top_p = 1.f;
+  int gen_top_k = 0;
   const ModelOutput* output(OutputKind k) const {
     for (auto& o : outputs)
       if (o.kind == k) return &o;

@@ -1,6 +1,7 @@
 // Shapes the transformer kernels of nn_kernels.cu can run. Host-only (no CUDA headers): the manifest loader (model.cc)
 // rejects a bundle with the same rule the launchers apply, so a model that pages in can always be served.
 #pragma once
+#include <cfloat>
 #include <cstddef>
 
 namespace tfsc {
@@ -95,6 +96,16 @@ inline size_t decode_attention_work_bytes(long long rows, int L, int H, int head
 // and writes max_new_tokens = N ids and log-probabilities per row; the decode steps' keys are bounded by decode attention's.
 inline bool generate_supported(int vocab, int N) {
   return vocab >= 1 && vocab <= kNextTokenMaxVocab && N >= 1 && N <= kDecodeMaxKeys;
+}
+// Sampled generation (generate.cu): a temperature whose fp32 value and fp32 reciprocal are finite and > 0 (the kernel
+// weighs (z - m) * (1 / temperature): a subnormal temperature's reciprocal is inf), 0 <= top_k <= vocab (0: off) and
+// 0 < top_p <= 1 (1: off).
+inline bool sampling_temperature_ok(double temperature) {
+  const float t = (float)temperature;
+  return temperature > 0 && temperature <= FLT_MAX && t > 0.f && 1.f / t <= FLT_MAX;
+}
+inline bool sampling_supported(int vocab, double temperature, int top_k, double top_p) {
+  return sampling_temperature_ok(temperature) && top_k >= 0 && top_k <= vocab && top_p > 0 && top_p <= 1;
 }
 
 // Depthwise convolution (depthwise.cu): a thread runs the kh x kw taps of one output pixel for 4 channels (1 on the scalar

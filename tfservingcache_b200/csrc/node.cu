@@ -824,9 +824,9 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
       if (e != cudaSuccess) return e;
     }
     if (d.head == HeadKind::Generate) {
-      // greedy decoding: the prefill above left each row's logits at its last attended token p_b (positions); each step
-      // picks a token, embeds it at slot p_b + 1 + t into the embed op's buffer and runs the decoder on that one token
-      // per row against the caches (DESIGN §4). A fixed N - 1 steps, no host synchronisation.
+      // decoding: the prefill above left each row's logits at its last attended token p_b (positions); each step picks
+      // (greedy) or draws (sampling) a token, embeds it at slot p_b + 1 + t into the embed op's buffer and runs the decoder
+      // on that one token per row against the caches (DESIGN §4). A fixed N - 1 steps, no host synchronisation.
       const GraphOp& emb = d.ops.front();
       GenerateOutputs go;
       for (const ModelOutput& m : d.outputs) {
@@ -860,7 +860,12 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
             e = exec(o);
           }
         }
-        if (e == cudaSuccess)
+        if (e == cudaSuccess && d.gen_sampling)  // a sampling bundle draws each row's token with its seed (the loader's checks)
+          e = launch_generate_sample((const float*)out, d.ops.back().cout, d.head_n, positions, t, t == d.head_k - 1, d.gen_eos,
+                                     done, go, (const float*)(dm.dptr + emb.word_off), (const float*)(dm.dptr + emb.pos_off),
+                                     (float*)buf(emb.dst), B, emb.c, (const int*)x + d.input(InputRole::Seed)->offset, d.in_dim,
+                                     d.gen_temperature, d.gen_top_k, d.gen_top_p, st);
+        else if (e == cudaSuccess)
           e = launch_generate_select((const float*)out, d.ops.back().cout, d.head_n, positions, t, t == d.head_k - 1, d.gen_eos,
                                      done, go, (const float*)(dm.dptr + emb.word_off), (const float*)(dm.dptr + emb.pos_off),
                                      (float*)buf(emb.dst), B, emb.c, st);

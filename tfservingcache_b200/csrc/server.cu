@@ -1277,10 +1277,9 @@ static int rest_handle_impl(tfsc_server* s, const char* method, const char* url,
       t += "], \"unknown_rank\": false}, \"name\": \"" + key + ":0\"}";
       return t;
     };
-    // every declared input of a multi-input model is DT_INT32 [-1, S]
+    // every declared input of a multi-input model is DT_INT32 [-1, width]: [-1, S], a seed [-1, 1]
     std::string ins;
-    for (auto& mi : d.inputs)
-      ins += (ins.empty() ? "" : ", ") + tensor_info(mi.name, {std::to_string(d.in_dim / (int64_t)d.inputs.size())}, "DT_INT32");
+    for (auto& mi : d.inputs) ins += (ins.empty() ? "" : ", ") + tensor_info(mi.name, {std::to_string(mi.width)}, "DT_INT32");
     if (d.inputs.empty())
       ins = tensor_info(d.input_name, dim.empty() ? std::vector<std::string>{} : std::vector<std::string>{dim},
                         d.input_dtype == TFSC_DT_INT32 ? "DT_INT32" : "DT_FLOAT");
@@ -1993,6 +1992,30 @@ int tfsc_k_generate_select(const float* logits, int64_t ld, int vocab, const int
   cudaError_t e = launch_generate_select(logits, ld, vocab, pos, t, last != 0, eos, done, o, word, pos_table, y, rows, H,
                                          (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "generate_select: %s", cudaGetErrorString(e));
+}
+int tfsc_k_generate_sample(const float* logits, int64_t ld, int vocab, const int32_t* pos, int t, int last, int eos, int32_t* done,
+                           int32_t* ids, int64_t ids_ld, float* log_probs, int64_t lp_ld, int32_t* length, int64_t length_ld,
+                           const float* word, const float* pos_table, float* y, int rows, int H, const int32_t* seeds,
+                           int64_t seed_stride, float temperature, int top_k, float top_p, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (!logits || !pos || !done || rows < 0 || t < 0 || vocab < 1 || vocab > kNextTokenMaxVocab || ld < vocab || H < 1 ||
+      (!last && (!word || !pos_table || !y)) || !seeds || seed_stride < 1)
+    return fail(TFSC_E_INVALID, "generate_sample: no kernel for %d rows of vocab = %d, ld = %lld, H = %d, seed_stride = %lld (1 <="
+                " vocab <= %d, ld >= vocab, seeds and seed_stride >= 1, the tables and y unless last)", rows, vocab, (long long)ld, H,
+                (long long)seed_stride, kNextTokenMaxVocab);
+  if (!sampling_supported(vocab, temperature, top_k, top_p))
+    return fail(TFSC_E_INVALID, "generate_sample: temperature = %g, top_k = %d, top_p = %g (a finite temperature > 0 with a finite"
+                " reciprocal, 0 <= top_k <= vocab = %d, 0 < top_p <= 1)", (double)temperature, top_k, (double)top_p, vocab);
+  GenerateOutputs o;
+  o.ids = ids;
+  o.ids_ld = ids_ld;
+  o.log_probs = log_probs;
+  o.log_probs_ld = lp_ld;
+  o.length = length;
+  o.length_ld = length_ld;
+  cudaError_t e = launch_generate_sample(logits, ld, vocab, pos, t, last != 0, eos, done, o, word, pos_table, y, rows, H, seeds,
+                                         seed_stride, temperature, top_k, top_p, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "generate_sample: %s", cudaGetErrorString(e));
 }
 int tfsc_debug_gemm_trace(long long*) {
   return fail(TFSC_E_UNIMPLEMENTED, "no GEMM clock trace: the persistent GEMM kernel it timed is not part of the sm_90a build");

@@ -412,6 +412,8 @@ def bert_manifest(seq=128, hidden=768, layers=12, heads=12, inter=3072, vocab=30
 
 
 GPT2_INPUTS = [{"name": "input_ids", "role": "ids"}, {"name": "attention_mask", "role": "mask"}]
+# a sampling generate bundle's inputs: GPT2_INPUTS and the per-request seed, int32 [B, 1] (one value per row)
+GPT2_SAMPLING_INPUTS = GPT2_INPUTS + [{"name": "seed", "role": "seed"}]
 
 
 def gpt2_manifest(seq=1024, hidden=768, layers=12, heads=12, vocab=50257, max_pos=1024, inputs=None, outputs=None):
@@ -427,7 +429,11 @@ def gpt2_manifest(seq=1024, hidden=768, layers=12, heads=12, vocab=50257, max_po
     "attention_mask" that hides keys whose mask is 0 and picks the last attended token. Positions are 0..seq-1 whatever
     the padding, as transformers' default position ids. Every LayerNorm has eps 1e-5. With GENERATE_OUTPUT_KINDS outputs
     (each entry with "max_new_tokens": N and optionally "eos_token_id") the same graph is a greedy generation bundle:
-    seq + N - 1 <= max_pos.
+    seq + N - 1 <= max_pos. Entries that also give "temperature" (a finite number > 0, default 1), "top_k" (an integer
+    0 <= top_k <= vocab, 0 = off) or "top_p" (0 < top_p <= 1, 1 = off), the same on every entry that gives one, make it a
+    sampling bundle: each token is drawn from the temperature / top-k / top-p distribution with the row's seed, so its
+    inputs need a "seed" role (GPT2_SAMPLING_INPUTS: an int32 [B, 1] "seed" beside the ids and mask, or
+    [{"name": "input_ids", "role": "ids"}, {"name": "seed", "role": "seed"}] without a mask).
     Buffers: 0 residual stream, 1 normed / attention context, 2 qkv / MLP hidden, 3 post-attention residual."""
     ops = [{"op": "embed", "src": -1, "dst": 0, "h": seq, "w": 1, "c": hidden, "vocab": vocab, "max_pos": max_pos, "norm": False}]
 

@@ -1,6 +1,6 @@
-"""Time of greedy generation on GPT-2 small on cuda:0, from CUDA events.
+"""Time of greedy and sampled generation on GPT-2 small on cuda:0, from CUDA events.
 
-    python -m tools.time_generate [--launches 200] [--repeats 5] [--new 64] [--model-repeats 3] [--profile] [--parent PKGDIR]
+    python -m tools.time_generate [--launches 200] [--repeats 5] [--new 64] [--model-repeats 3] [--profile] [--sampling] [--parent PKGDIR]
 
 1. tfsc_k_decode_attention at rows in {1, 8, 64} and L in {128, 1024} keys, 12 heads of width 64: median of `repeats`
    windows of `launches` back-to-back launches, microseconds per launch, and the GB/s of K and V cache read (2 * rows * L * H
@@ -11,9 +11,13 @@
    prompt + N - 1 tokens, right-padded, which is what a client without generation sends for the same tokens.
 3. --profile: in a run of its own, torch.profiler's split of the decode steps' kernel time by kernel family at 8 rows and
    prompt 960 (the batch minus a prefill-only batch).
-4. --parent PKGDIR: ResNet-50, BERT-base and the tenant MLP (tools/time_convnets.py's comparison) and GPT-2 small
-   next-token at 8 x 128 (every next-token output, half the rows right-padded) against a package built from another
-   commit, alternating the two in child processes: ms per batch over windows of --steps calls, and bit-for-bit outputs.
+4. --parent PKGDIR: ResNet-50, BERT-base and the tenant MLP (tools/time_convnets.py's comparison), GPT-2 small
+   next-token at 8 x 128 (every next-token output, half the rows right-padded) and greedy generation of 32 tokens there,
+   against a package built from another commit, alternating the two in child processes: ms per batch over windows of --steps calls, and bit-for-bit outputs.
+5. --sampling: tfsc_k_generate_sample against tfsc_k_generate_select at rows in {1, 8, 64}, vocab 50257, for temperature
+   only, top_k 50, top_p 0.9 and top_k 200 with top_p 0.95 (microseconds per launch, the two alternating), and a sampling
+   bundle (top_k 50, top_p 0.9) against the greedy bundle end to end at prompt {128, 960} x rows {1, 8, 64}, N = --new:
+   ms per batch and generated tokens/s, alternating.
 Prints one JSON object with the card name and power limit. Bundles go to a temporary directory, removed at the end."""
 import argparse
 import json
@@ -114,6 +118,86 @@ def model_table(torch, t, args):
     return res
 
 
+SAMPLING = {"temperature_0.8": (0.8, 0, 1.0), "top_k_50": (1.0, 50, 1.0), "top_p_0.9": (1.0, 0, 0.9),
+            "top_k_200_top_p_0.95": (1.0, 200, 0.95)}
+
+
+def sample_kernel_table(torch, t, args):
+    """us per launch of the select step and of the sampling step on the same GPT-2-sized logits, alternating"""
+    lib = t._lib.lib
+    res = {}
+    gen = torch.Generator(device="cuda").manual_seed(0)
+    for rows in (1, 8, 64):
+        ld = (V + 31) // 32 * 32
+        x = torch.randn(rows, ld, device="cuda", generator=gen) * 3
+        pos = torch.full((rows,), 10, dtype=torch.int32, device="cuda")
+        done = torch.zeros(rows, dtype=torch.int32, device="cuda")
+        seeds = torch.arange(rows, dtype=torch.int32, device="cuda")
+        ids = torch.empty(rows, 2, dtype=torch.int32, device="cuda")
+        lp = torch.empty(rows, 2, device="cuda")
+        word, ptab, y = torch.randn(V, H, device="cuda"), torch.randn(64, H, device="cuda"), torch.empty(rows, H, device="cuda")
+        common = lambda: (x.data_ptr(), ld, V, pos.data_ptr(), 1, 0, -1, done.data_ptr(), ids.data_ptr(), 2, lp.data_ptr(), 2,  # noqa: E731
+                          None, 0, word.data_ptr(), ptab.data_ptr(), y.data_ptr(), rows, H)
+        select = lambda: t._lib.check(lib.tfsc_k_generate_select(*common(), None), "select")  # noqa: E731
+        row = {}
+        for name, (temperature, k, p) in SAMPLING.items():
+            def sample():
+                t._lib.check(lib.tfsc_k_generate_sample(*common(), seeds.data_ptr(), 1, temperature, k, p, None), "sample")
+            us = {"select": [], "sample": []}
+            for _ in range(args.repeats):                                 # alternating windows
+                us["select"].append(_median_us(torch, select, args.launches, 1))
+                us["sample"].append(_median_us(torch, sample, args.launches, 1))
+            row[name] = {"select_us": round(float(np.median(us["select"])), 2), "sample_us": round(float(np.median(us["sample"])), 2)}
+        res[f"rows{rows}"] = row
+    return res
+
+
+def sampling_model_table(torch, t, args):
+    """a sampling bundle against the greedy bundle of the same seeded GPT-2 small, end to end, alternating"""
+    mf = t.modelformat
+    tmp = tempfile.mkdtemp(prefix="tfsc_samp_")
+    res, N = {}, args.new
+    try:
+        for S in (128, 960):
+            for name, outs, inputs in ((f"greedy_s{S}", _outs(N), mf.GPT2_INPUTS),
+                                       (f"sample_s{S}", [dict(o, top_k=50, top_p=0.9) for o in _outs(N)], mf.GPT2_SAMPLING_INPUTS)):
+                man = mf.gpt2_manifest(seq=S, inputs=inputs, outputs=outs)
+                mf.write_graph_bundle(f"{tmp}/{name}/1", man, seeded_gpt2_blob(man, 0))
+        width = sum(w for _n, _o, w, _d in mf.packed_output_layout(_outs(N), V))
+        cfg = {"modelProvider.type": "diskProvider", "modelProvider.diskProvider.baseDir": tmp, "gpu.devices": [0],
+               "gpu.arenaBytes": 4 << 30, "modelCache.size": 8 << 30, "serving.maxConcurrentModels": 8, "gpu.maxBatch": 64}
+        gen = torch.Generator(device="cuda").manual_seed(0)
+        with t.Server(cfg) as srv:
+            stream = torch.cuda.Stream()
+            for S in (128, 960):
+                for rows in (1, 8, 64):
+                    ids = torch.randint(0, V, (rows, S), device="cuda", generator=gen, dtype=torch.int32)
+                    mask = torch.ones(rows, S, dtype=torch.int32, device="cuda")
+                    seed = torch.arange(rows, dtype=torch.int32, device="cuda")[:, None]
+                    xs = {"greedy": torch.cat([mask, ids], 1).contiguous(), "sample": torch.cat([mask, ids, seed], 1).contiguous()}
+                    y = torch.empty(rows, width, device="cuda")
+                    fns = {}
+                    for kind in ("greedy", "sample"):
+                        name = f"{kind}_s{S}"
+                        srv.ensure(0, name, 1)
+                        fns[kind] = (lambda name=name, x=xs[kind]: srv.predict_device(0, name, 1, x.data_ptr(), rows, y.data_ptr(),
+                                                                                       stream.cuda_stream))
+                        fns[kind]()
+                    srv.sync(0)
+                    ms = {"greedy": [], "sample": []}
+                    for _ in range(args.model_repeats):
+                        for kind in ("greedy", "sample"):
+                            ms[kind].append(_events(torch, fns[kind], 1, stream))
+                    g, s_ = float(np.median(ms["greedy"])), float(np.median(ms["sample"]))
+                    res[f"prompt{S}_rows{rows}"] = {"new_tokens": N, "greedy_ms": round(g, 3), "sample_ms": round(s_, 3),
+                                                    "greedy_tokens_per_s": round(rows * N / g * 1e3, 1),
+                                                    "sample_tokens_per_s": round(rows * N / s_ * 1e3, 1)}
+                    torch.cuda.empty_cache()
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
+    return res
+
+
 def profile_table(torch, t, args):
     """kernel time of one batch at 8 rows, prompt 960, minus that of the prefill-only bundle, by family"""
     from torch.profiler import ProfilerActivity, profile
@@ -155,8 +239,8 @@ def profile_table(torch, t, args):
 
 
 def gpt2_child(out_path, steps, repeats):
-    """this process's library: GPT-2 small next-token at 8 x 128, ms per batch, and its outputs on seeded inputs saved to
-    out_path"""
+    """this process's library: GPT-2 small next-token at 8 x 128 and greedy generation of 32 tokens at 8 x 128, ms per
+    batch, and their outputs on seeded inputs saved to out_path"""
     import torch
 
     import tfservingcache_b200 as t
@@ -168,6 +252,8 @@ def gpt2_child(out_path, steps, repeats):
     try:
         man = mf.gpt2_manifest(seq=S, inputs=mf.GPT2_INPUTS, outputs=outs)
         mf.write_graph_bundle(f"{tmp}/gpt2/1", man, seeded_gpt2_blob(man, 0))
+        gman = mf.gpt2_manifest(seq=S, inputs=mf.GPT2_INPUTS, outputs=_outs(32))
+        mf.write_graph_bundle(f"{tmp}/gen/1", gman, seeded_gpt2_blob(gman, 0))
         rng = np.random.default_rng(0)
         ids = rng.integers(0, V, (B, S)).astype(np.int32)
         mask = np.ones((B, S), np.int32)
@@ -176,7 +262,10 @@ def gpt2_child(out_path, steps, repeats):
                "gpu.arenaBytes": 2 << 30, "modelCache.size": 4 << 30, "serving.maxConcurrentModels": 2, "gpu.maxBatch": B}
         with t.Server(cfg) as srv:
             out = srv.predict("gpt2", "1", {"input_ids": ids, "attention_mask": mask}, outputs=[o["name"] for o in outs])
+            gen = srv.predict("gen", "1", {"input_ids": ids, "attention_mask": mask}, outputs=[o["name"] for o in _outs(32)])
+            out.update({f"greedy_{k}": v for k, v in gen.items()})
             srv.ensure(0, "gpt2", 1)
+            srv.ensure(0, "gen", 1)
             stream = torch.cuda.Stream()
             x = torch.from_numpy(np.ascontiguousarray(np.concatenate([mask, ids], axis=1))).cuda()  # attention_mask | input_ids
             y = torch.empty(B, sum(w for _n, _o, w, _d in mf.packed_output_layout(outs, V)), device="cuda")
@@ -187,10 +276,17 @@ def gpt2_child(out_path, steps, repeats):
                 fn()
             torch.cuda.synchronize()
             ms = float(np.median([_events(torch, fn, steps, stream) for _ in range(repeats)]))
+            yg = torch.empty(B, sum(w for _n, _o, w, _d in mf.packed_output_layout(_outs(32), V)), device="cuda")
+
+            def gfn():
+                srv.predict_device(0, "gen", 1, x.data_ptr(), B, yg.data_ptr(), stream.cuda_stream)
+            gfn()
+            torch.cuda.synchronize()
+            gms = float(np.median([_events(torch, gfn, 1, stream) for _ in range(repeats)]))
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
     np.savez(out_path, **out)
-    print(json.dumps({"gpt2_next_token_b8_s128": ms, "lib": t._lib.LIB_PATH}))
+    print(json.dumps({"gpt2_next_token_b8_s128": ms, "gpt2_greedy_generate_b8_s128_n32": gms, "lib": t._lib.LIB_PATH}))
 
 
 def gpt2_ab_table(args):
@@ -210,11 +306,13 @@ def gpt2_ab_table(args):
         same = {k: bool(a[k].tobytes() == b[k].tobytes()) for k in sorted(a)} if sorted(a) == sorted(b) else {"keys": False}
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
-    this = [r["gpt2_next_token_b8_s128"] for r in runs["this"]]
-    par = [r["gpt2_next_token_b8_s128"] for r in runs["parent"]]
-    return {"bit_identical_to_parent": same,
-            "ms": {"this": round(float(np.median(this)), 4), "parent": round(float(np.median(par)), 4),
-                   "this_runs": [round(v, 4) for v in this], "parent_runs": [round(v, 4) for v in par]}}
+    res = {"bit_identical_to_parent": same}
+    for key in ("gpt2_next_token_b8_s128", "gpt2_greedy_generate_b8_s128_n32"):
+        this = [r[key] for r in runs["this"]]
+        par = [r[key] for r in runs["parent"]]
+        res[key + "_ms"] = {"this": round(float(np.median(this)), 4), "parent": round(float(np.median(par)), 4),
+                            "this_runs": [round(v, 4) for v in this], "parent_runs": [round(v, 4) for v in par]}
+    return res
 
 
 def main():
@@ -227,6 +325,7 @@ def main():
     ap.add_argument("--ab-repeats", type=int, default=2)
     ap.add_argument("--profile", action="store_true")
     ap.add_argument("--skip-models", action="store_true")
+    ap.add_argument("--sampling", action="store_true")
     ap.add_argument("--parent", default=None, help="a tfservingcache_b200 package built from the commit to compare against")
     ap.add_argument("--gpt2-child", default=None, help=argparse.SUPPRESS)
     args = ap.parse_args()
@@ -240,11 +339,14 @@ def main():
     res["decode_attention"] = decode_table(torch, t, args)
     if not args.skip_models:
         res["models"] = model_table(torch, t, args)
+    if args.sampling:
+        res["sample_step"] = sample_kernel_table(torch, t, args)
+        res["sampling_models"] = sampling_model_table(torch, t, args)
     if args.profile:
         res["decode_step_profile"] = profile_table(torch, t, args)
     if args.parent:
         res["vs_parent"] = ab_table(args)
-        res["vs_parent"]["gpt2_next_token_b8_s128"] = gpt2_ab_table(args)
+        res["vs_parent"]["gpt2_b8_s128"] = gpt2_ab_table(args)
     res.update({"card_after": _card()})
     print(json.dumps(res))
 
