@@ -419,7 +419,7 @@ GPT2_SAMPLING_INPUTS = GPT2_INPUTS + [{"name": "seed", "role": "seed"}]
 def gpt2_manifest(seq=1024, hidden=768, layers=12, heads=12, vocab=50257, max_pos=1024, inputs=None, outputs=None):
     """GPT-2 (Radford et al. 2019; transformers' GPT2LMHeadModel topology) as a next-token graph bundle: token ids int32
     [B, seq] -> the vocabulary logits of each row's last attended token, answered through NEXT_TOKEN_OUTPUT_KINDS. The
-    defaults give GPT-2 small; (1024, 16, 16), (1280, 36, 20) and (1600, 48, 25) as (hidden, layers, heads) give medium,
+    defaults give GPT-2 small; (1024, 24, 16), (1280, 36, 20) and (1600, 48, 25) as (hidden, layers, heads) give medium,
     large and XL. The embedding is wte[id] + wpe[s] without LayerNorm ("norm": false). A block is ln_1, c_attn (a 1x1 conv
     H -> 3H, packed q | k | v), causal attention, c_proj with the block input as residual, ln_2, c_fc (H -> 4H, tanh GELU)
     and c_proj with the residual. Then a last_token op copies each row's last attended token (the highest position whose
