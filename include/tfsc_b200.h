@@ -502,6 +502,23 @@ int tfsc_k_generate_sample(const float* logits, int64_t ld, int vocab, const int
                            int32_t* ids, int64_t ids_ld, float* log_probs, int64_t lp_ld, int32_t* length, int64_t length_ld,
                            const float* word, const float* pos_table, float* y, int rows, int H, const int32_t* seeds,
                            int64_t seed_stride, float temperature, int top_k, float top_p, void* stream);
+/* One step of a generate bundle with repetition control: tfsc_k_generate_select (seeds NULL) or tfsc_k_generate_sample (seeds
+ * given, with temperature, top_k and top_p) with g chosen from the row's logits z after, in transformers' order: the
+ * repetition penalty (z < 0 ? z * p : z / p in fp32, once per id of the row's history), the ban of every token that would
+ * repeat an n-gram of the history (no_repeat_ngram_size = n, 0: off) and the ban of eos while t < min_new_tokens (0: off).
+ * All banned: g = 0, no draw. The history is the row's attended prompt ids in position order, prompt_ids[r * stride + j] for
+ * j <= pos[r] whose mask[r * stride + j] != 0 (mask NULL: all), each clamped to [0, vocab); the t = 0 step writes them to
+ * hist[r * hist_ld ..] and their count to hist_len0[r], and every step appends g at hist[r * hist_ld + hist_len0[r] + t]
+ * (pos[r] + N <= hist_ld). The log-probability is the raw row's, the bits tfsc_k_generate_select writes for the same g.
+ * TFSC_E_INVALID outside tfsc_k_generate_select's limits, unless p's fp32 value is finite, > 0 and normal, n >= 0, m >= 0
+ * with 0 <= eos < vocab when m > 0, prompt_ids, hist and hist_len0 are given, stride >= 1 and hist_ld > t, and with seeds
+ * outside tfsc_k_generate_sample's. */
+int tfsc_k_generate_process(const float* logits, int64_t ld, int vocab, const int32_t* pos, int t, int last, int eos, int32_t* done,
+                            int32_t* ids, int64_t ids_ld, float* log_probs, int64_t lp_ld, int32_t* length, int64_t length_ld,
+                            const float* word, const float* pos_table, float* y, int rows, int H, const int32_t* prompt_ids,
+                            const int32_t* mask, int64_t stride, int32_t* hist, int64_t hist_ld, int32_t* hist_len0,
+                            float repetition_penalty, int no_repeat_ngram_size, int min_new_tokens, const int32_t* seeds,
+                            int64_t seed_stride, float temperature, int top_k, float top_p, void* stream);
 
 #ifdef __cplusplus
 }

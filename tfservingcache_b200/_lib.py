@@ -161,6 +161,9 @@ _sig("tfsc_k_generate_select", C.c_int, vp, C.c_int64, C.c_int, vp, C.c_int, C.c
      C.c_int64, vp, vp, vp, C.c_int, C.c_int, vp)
 _sig("tfsc_k_generate_sample", C.c_int, vp, C.c_int64, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int64, vp, C.c_int64, vp,
      C.c_int64, vp, vp, vp, C.c_int, C.c_int, vp, C.c_int64, C.c_float, C.c_int, C.c_float, vp)
+_sig("tfsc_k_generate_process", C.c_int, vp, C.c_int64, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int64, vp, C.c_int64, vp,
+     C.c_int64, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int64, vp, C.c_int64, vp, C.c_float, C.c_int, C.c_int, vp, C.c_int64,
+     C.c_float, C.c_int, C.c_float, vp)
 
 
 class TfscError(RuntimeError):

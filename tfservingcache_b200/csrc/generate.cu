@@ -18,6 +18,10 @@
 //
 // generate_sample_kernel: the select step of sampling bundles. The same staging, maximum and log-probability, then a token
 // drawn from the temperature / top-k / top-p distribution with the row's seed (sample_token), written as the select step's.
+//
+// generate_process_kernel: the step of processing bundles (repetition penalty, no-repeat n-grams, minimum length). The same
+// staging, maximum and log-probability, then the row's history of prompt and generated ids (kept in scratch across steps)
+// processes the staged row in place, and the token is the processed row's argmax or draw (sample_token).
 #include <cuda_runtime.h>
 
 #include <atomic>
@@ -587,6 +591,160 @@ cudaError_t launch_generate_sample(const float* logits, int64_t ld, int vocab, c
                           done, o, word, pos_table, y, H, seeds, seed_stride, inv_t, top_k, top_p)
              : launch_pdl(generate_sample_kernel<false>, dim3((unsigned)rows), threads, smem, s, logits, ld, vocab, pos, t, last, eos,
                           done, o, word, pos_table, y, H, seeds, seed_stride, inv_t, top_k, top_p);
+}
+
+// --------------------------------------------------------------------------------------- repetition control ----
+// The argmax of the staged row in the next-token head's rank order (value descending, ties to the lower id; all -inf: id 0):
+// head_stage_select's first round without the staging. Every thread gets the id, and *v its value.
+__device__ __forceinline__ int staged_argmax(const float* xs, int n, float* wv, int* wi, float* s_v, int* s_i, float* v) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  float bv;
+  int bi;
+  local_best(xs, n, INFINITY, -1, &bv, &bi);
+  warp_best(bv, bi);
+  if (lane == 0) {
+    wv[warp] = bv;
+    wi[warp] = bi;
+  }
+  __syncthreads();
+  if (warp == 0) {
+    bv = lane < nwarps ? wv[lane] : -INFINITY;
+    bi = lane < nwarps ? wi[lane] : INT_MAX;
+    warp_best(bv, bi);
+    if (lane == 0) {
+      *s_v = bv;
+      *s_i = bi;
+    }
+  }
+  __syncthreads();
+  *v = *s_v;
+  return *s_i;
+}
+
+// The step of processing bundles (DESIGN §3): the select step's staging, maximum and sum of the raw logits, then in shared
+// memory the repetition penalty over the row's history, the no-repeat n-gram bans and the EOS ban below min_new steps, and
+// the argmax (seeds null) or the sampled token (sample_token) of the processed row. At t = 0 the CTA writes the history's
+// prompt part, the attended prompt ids in position order, to hist and its length to hist_len0; every step appends its token
+// at hist[hist_len0 + t]. hist is ordered across steps as done is: every launch of the chain waits for the one before.
+template <bool kVec>
+__global__ void __launch_bounds__(kHeadThreadsMax) generate_process_kernel(
+    const float* __restrict__ logits, int64_t ld, int vocab, const int* __restrict__ pos, int t, bool last, int eos,
+    int* __restrict__ done, GenerateOutputs o, const float* __restrict__ word, const float* __restrict__ pos_table,
+    float* __restrict__ y, int H, const int* __restrict__ ids, const int* __restrict__ mask, int64_t stride, int* hist,
+    int64_t hist_ld, int* hist_len0, float penalty, int ngram, int min_new, const int* __restrict__ seeds, int64_t seed_stride,
+    float inv_t, int top_k, float top_p) {
+  extern __shared__ float xs[];  // the row's vocab logits, processed in place
+  __shared__ float wv[kHeadThreadsMax / 32];
+  __shared__ int wi[kHeadThreadsMax / 32];
+  __shared__ double wsum[kHeadThreadsMax / 32];
+  __shared__ float s_v;
+  __shared__ int s_i;
+  __shared__ double s_sum;
+  __shared__ int sel[1];
+  __shared__ int wcnt[kHeadThreadsMax / 32];
+  __shared__ u64 rhist[256];  // sample_token's radix histograms and scans
+  __shared__ RadixPick s_pick;
+  __shared__ int s_res;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  const int64_t row = blockIdx.x;
+  // launched after the vocabulary projection; done, hist and hist_len0 come from the previous steps' launches
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  const int p = __ldg(pos + row);
+  const bool live = t == 0 ? p >= 0 : done[row] == 0;
+  const float* raw = logits + row * ld;
+  const float m = head_stage_select(raw, vocab, 1, xs, wv, wi, &s_v, &s_i, sel);
+  const double sum = head_exp_sum(xs, vocab, m, wsum, &s_sum);
+  int* h = hist + row * hist_ld;
+  int L0 = 0;
+  if (t == 0) {
+    // positions 0..p whose mask is set (all of them without a mask), compacted in order a block of positions at a time:
+    // a ballot per warp, the warps' counts in wcnt; ids clamped to [0, vocab) as the embedding clamps them
+    const int* irow = ids + row * stride;
+    const int* mrow = mask ? mask + row * stride : nullptr;
+    for (int base = 0; base <= p; base += blockDim.x) {
+      const int j = base + (int)threadIdx.x;
+      const bool att = j <= p && (!mrow || __ldg(mrow + j) != 0);
+      const unsigned ballot = __ballot_sync(0xffffffffu, att);
+      if (lane == 0) wcnt[warp] = __popc(ballot);
+      __syncthreads();
+      int before = 0, total = 0;
+      for (int w = 0; w < nwarps; ++w) {
+        const int c = wcnt[w];
+        before += w < warp ? c : 0;
+        total += c;
+      }
+      if (att) {
+        const int id = __ldg(irow + j);
+        h[L0 + before + __popc(ballot & ((1u << lane) - 1u))] = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
+      }
+      L0 += total;
+      __syncthreads();  // wcnt is rewritten by the next pass; the history is complete after the last
+    }
+    if (threadIdx.x == 0) hist_len0[row] = L0;
+  } else {
+    L0 = hist_len0[row];
+  }
+  const int L = L0 + t;  // the prompt part and g_0 .. g_{t-1}
+  // the penalty reads each logit from the unprocessed row in global memory, so an id the history holds twice gets the same
+  // value from both writes
+  if (penalty != 1.f)
+    for (int i = threadIdx.x; i < L; i += blockDim.x) {
+      const int id = h[i];
+      const float z = __ldg(raw + id);
+      xs[id] = z < 0.f ? __fmul_rn(z, penalty) : __fdiv_rn(z, penalty);
+    }
+  __syncthreads();
+  // every h[i + n - 1] whose n - 1 tokens before it are the history's last n - 1 tokens is banned
+  for (int i = threadIdx.x; ngram > 0 && i <= L - ngram; i += blockDim.x) {
+    bool match = true;
+    for (int k = 0; k < ngram - 1 && match; ++k) match = h[i + k] == h[L - ngram + 1 + k];
+    if (match) xs[h[i + ngram - 1]] = -INFINITY;
+  }
+  if (t < min_new && threadIdx.x == 0) xs[eos] = -INFINITY;
+  __syncthreads();
+  float mp;
+  int g = staged_argmax(xs, vocab, wv, wi, &s_v, &s_i, &mp);
+  // a sampling bundle draws from the processed row unless top_k = 1 (its argmax) or every logit is banned (id 0, no draw)
+  if (seeds && top_k != 1 && mp != -INFINITY)
+    g = sample_token(xs, vocab, mp, inv_t, top_k, top_p, (uint32_t)__ldg(seeds + row * seed_stride), t, rhist, &s_pick, &s_res);
+  // the log-probability is the raw row's: the select step's bits for the same g
+  generate_write<kVec>(row, t, p, live, g, raw, vocab, m, sum, last, eos, done, o, word, pos_table, y, H);
+  if (threadIdx.x == 0) h[L] = g < 0 ? 0 : (g >= vocab ? vocab - 1 : g);
+}
+
+cudaError_t launch_generate_process(const float* logits, int64_t ld, int vocab, const int* pos, int t, bool last, int eos,
+                                    int* done, const GenerateOutputs& o, const float* word, const float* pos_table, float* y,
+                                    int rows, int H, const int* ids, const int* mask, int64_t stride, int* hist, int64_t hist_ld,
+                                    int* hist_len0, float penalty, int ngram, int min_new, const int* seeds, int64_t seed_stride,
+                                    float temperature, int top_k, float top_p, cudaStream_t s) {
+  if (rows < 0 || t < 0 || vocab < 1 || vocab > kNextTokenMaxVocab || ld < vocab || H < 1 || !logits || !pos || !done ||
+      (!last && (!word || !pos_table || !y)) || !ids || stride < 1 || !hist || hist_ld <= t || !hist_len0 ||
+      !processing_supported(penalty, ngram, min_new) || (min_new > 0 && (eos < 0 || eos >= vocab)) ||
+      (seeds && (seed_stride < 1 || !sampling_supported(vocab, temperature, top_k, top_p))))
+    return cudaErrorInvalidValue;
+  if (rows == 0) return cudaSuccess;
+  static bool attr[64] = {};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (!attr[dev & 63]) {
+    for (cudaError_t e : {cudaFuncSetAttribute(generate_process_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               kNextTokenMaxVocab * (int)sizeof(float)),
+                          cudaFuncSetAttribute(generate_process_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               kNextTokenMaxVocab * (int)sizeof(float))})
+      if (e != cudaSuccess) return e;
+    attr[dev & 63] = true;
+  }
+  const bool vec = H % 4 == 0 && (((uintptr_t)word | (uintptr_t)pos_table | (uintptr_t)y) & 15) == 0;
+  const size_t smem = (size_t)vocab * sizeof(float);
+  // the select step's block size: its maximum and sum of exponentials, so its log-probabilities, are the same bits
+  const int threads = head_threads(vocab);
+  const float inv_t = seeds ? 1.f / temperature : 1.f;
+  return vec ? launch_pdl(generate_process_kernel<true>, dim3((unsigned)rows), threads, smem, s, logits, ld, vocab, pos, t, last,
+                          eos, done, o, word, pos_table, y, H, ids, mask, stride, hist, hist_ld, hist_len0, penalty, ngram, min_new,
+                          seeds, seed_stride, inv_t, top_k, top_p)
+             : launch_pdl(generate_process_kernel<false>, dim3((unsigned)rows), threads, smem, s, logits, ld, vocab, pos, t, last,
+                          eos, done, o, word, pos_table, y, H, ids, mask, stride, hist, hist_ld, hist_len0, penalty, ngram, min_new,
+                          seeds, seed_stride, inv_t, top_k, top_p);
 }
 
 }  // namespace tfsc

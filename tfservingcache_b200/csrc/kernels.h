@@ -224,6 +224,18 @@ cudaError_t launch_generate_sample(const float* logits, int64_t ld, int vocab, c
                                    int* done, const GenerateOutputs& o, const float* word, const float* pos_table, float* y,
                                    int rows, int H, const int* seeds, int64_t seed_stride, float temperature, int top_k,
                                    float top_p, cudaStream_t s);
+// One step of a processing bundle (DESIGN §3): launch_generate_select (seeds null) or launch_generate_sample with g chosen
+// from the row's logits after the repetition penalty over its history, the no-repeat n-gram bans (ngram: 0 off) and the
+// EOS ban while t < min_new. The history is the row's attended prompt ids, ids / mask [r * stride + j] for j <= pos[r]
+// (mask null: every position), written to hist [r * hist_ld ..] and its length to hist_len0[r] at t = 0, then g_0 .. g_{t-1};
+// the step appends g at hist[r * hist_ld + hist_len0[r] + t], so pos[r] + N <= hist_ld is the caller's to keep. The
+// log-probability is the raw row's, the bits launch_generate_select gives for the same g. cudaErrorInvalidValue outside
+// processing_supported (nn_limits.h), for min_new > 0 without an EOS id below vocab or, with seeds, outside sampling_supported.
+cudaError_t launch_generate_process(const float* logits, int64_t ld, int vocab, const int* pos, int t, bool last, int eos,
+                                    int* done, const GenerateOutputs& o, const float* word, const float* pos_table, float* y,
+                                    int rows, int H, const int* ids, const int* mask, int64_t stride, int* hist, int64_t hist_ld,
+                                    int* hist_len0, float penalty, int ngram, int min_new, const int* seeds, int64_t seed_stride,
+                                    float temperature, int top_k, float top_p, cudaStream_t s);
 
 // wgmma 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
 bool gemm_tc_supported(const float* A, const float* B, const float* bias, const float* R, const float* C, int M, int N, int K,

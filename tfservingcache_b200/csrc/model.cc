@@ -67,6 +67,11 @@ ModelDesc::GenerateScratch ModelDesc::generate_scratch(int64_t rows) const {
   g.counter_bytes = align256((size_t)rows * (size_t)heads * 4);  // decode_attention_work_bytes' first region
   g.done = g.work + align256(work);
   g.end = g.done + align256((size_t)rows * 4);
+  if (gen_processing) {
+    g.hist = g.end;
+    g.hist_len0 = g.hist + align256((size_t)rows * (size_t)(T + 1) * 4);
+    g.end = g.hist_len0 + align256((size_t)rows * 4);
+  }
   return g;
 }
 
@@ -315,6 +320,37 @@ static bool parse_sampling(const Json& oj, const std::string& name, double* temp
   return true;
 }
 
+// A generate entry's "repetition_penalty" (finite, > 0, a normal fp32 value), "no_repeat_ngram_size" and "min_new_tokens"
+// (integers >= 1; their upper bounds are checked with the bundle), each the same on every entry that gives it: *penalty NaN
+// and *ngram / *min_new -1 until one does
+static bool parse_processing(const Json& oj, const std::string& name, double* penalty, int* ngram, int* min_new, std::string* err) {
+  const std::string at = "signature.outputs: '" + name + "' has a ";
+  auto differs = [&](const char* field) {
+    *err = at + "'" + field + "' that differs from the other generate outputs'";
+    return false;
+  };
+  if (const Json* f = oj.get("repetition_penalty")) {
+    if (f->type != Json::Num || !repetition_penalty_ok(f->num)) {
+      *err = at + "'repetition_penalty' that is not a finite number > 0 with a finite, normal fp32 value (1: off)";
+      return false;
+    }
+    if (!std::isnan(*penalty) && f->num != *penalty) return differs("repetition_penalty");
+    *penalty = f->num;
+  }
+  auto count = [&](const char* field, int* v) {
+    const Json* f = oj.get(field);
+    if (!f) return true;
+    if (f->type != Json::Num || f->num != std::floor(f->num) || f->num < 1 || f->num > 0x7fffffff) {
+      *err = at + "'" + field + "' that is not an integer >= 1";
+      return false;
+    }
+    if (*v >= 0 && (int)f->num != *v) return differs(field);
+    *v = (int)f->num;
+    return true;
+  };
+  return count("no_repeat_ngram_size", ngram) && count("min_new_tokens", min_new);
+}
+
 // signature.outputs, one entry at a time. An entry is refused for, in this order: an unknown kind, no name, a duplicate, a
 // mix of heads (fill-mask, then encoder, then span: the message names the later entry's head), a 'normalize' on a kind
 // without one, and then the fields its head takes. Sets d->head.
@@ -324,6 +360,9 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
   // a generate bundle's sampling fields, NaN / -1 until an entry gives them
   double temperature = NAN, top_p = NAN;
   int top_k = -1;
+  // and its repetition-control fields
+  double penalty = NAN;
+  int ngram = -1, min_new = -1;
   // an integer field of an output entry: 0 absent, 1 read into *v, -1 present but not an integer
   auto int_field = [](const Json& oj, const char* key, int* v) {
     const Json* f = oj.get(key);
@@ -456,6 +495,7 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
         }
         if (v >= 0) eos = v;
         if (!parse_sampling(oj, mo.name, &temperature, &top_k, &top_p, err)) return false;
+        if (!parse_processing(oj, mo.name, &penalty, &ngram, &min_new, err)) return false;
         break;
       case HeadKind::Encoder:
         if (oj.get("k") || span_fields) {
@@ -509,6 +549,10 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
   d->gen_temperature = std::isnan(temperature) ? 1.f : (float)temperature;
   d->gen_top_k = top_k < 0 ? 0 : top_k;
   d->gen_top_p = std::isnan(top_p) ? 1.f : (float)top_p;
+  d->gen_processing = !std::isnan(penalty) || ngram >= 0 || min_new >= 0;
+  d->gen_repetition_penalty = std::isnan(penalty) ? 1.f : (float)penalty;
+  d->gen_no_repeat_ngram = ngram < 0 ? 0 : ngram;
+  d->gen_min_new_tokens = min_new < 0 ? 0 : min_new;
   d->span_max_len = span_seen ? max_len : 0;
   d->span_sep_id = sep_id;
   set_head(d);
@@ -732,6 +776,21 @@ static bool check_generate_bundle(ModelDesc* d, int last_tokens, std::string* er
   if (d->gen_sampling && !d->input(InputRole::Seed)) {
     *err = "signature.outputs: a sampling generate bundle (temperature, top_k or top_p) needs an input with the role 'seed'"
            " (int32 [batch, 1])";
+    return false;
+  }
+  // a history of L = S + N - 1 tokens at most: an n-gram of n > L never fits in it
+  if (d->gen_no_repeat_ngram > T) {
+    *err = "signature.outputs: no_repeat_ngram_size = " + std::to_string(d->gen_no_repeat_ngram) + " exceeds S + max_new_tokens - 1 = " +
+           std::to_string(T);
+    return false;
+  }
+  if (d->gen_min_new_tokens > N) {
+    *err = "signature.outputs: min_new_tokens = " + std::to_string(d->gen_min_new_tokens) + " exceeds max_new_tokens = " +
+           std::to_string(N);
+    return false;
+  }
+  if (d->gen_min_new_tokens > 0 && d->gen_eos < 0) {
+    *err = "signature.outputs: min_new_tokens needs an eos_token_id: it bans the EOS token until that many tokens are generated";
     return false;
   }
   d->head_n = V;

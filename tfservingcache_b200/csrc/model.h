@@ -146,7 +146,9 @@ struct ModelDesc {
   // and the hidden states are its source buffer) and normalize_cls / normalize_mean; a fill-mask head's mlm_vocab (the
   // embed op's vocab, the logits the head reads of each Vp-wide row) and mlm_mask_token_id; a generate head's gen_eos
   // (eos_token_id, -1: none) and, on a sampling bundle (gen_sampling: a generate entry gave temperature, top_k or top_p),
-  // gen_temperature (1), gen_top_k (0: off) and gen_top_p (1: off).
+  // gen_temperature (1), gen_top_k (0: off) and gen_top_p (1: off), and on a processing bundle (gen_processing: a generate
+  // entry gave repetition_penalty, no_repeat_ngram_size or min_new_tokens) gen_repetition_penalty (1), gen_no_repeat_ngram
+  // (0: off) and gen_min_new_tokens (0: off).
   std::vector<ModelOutput> outputs;
   HeadKind head = HeadKind::None;
   int head_n = 0, head_k = 0;
@@ -157,6 +159,9 @@ struct ModelDesc {
   bool gen_sampling = false;
   float gen_temperature = 1.f, gen_top_p = 1.f;
   int gen_top_k = 0;
+  bool gen_processing = false;
+  float gen_repetition_penalty = 1.f;
+  int gen_no_repeat_ngram = 0, gen_min_new_tokens = 0;
   const ModelOutput* output(OutputKind k) const {
     for (auto& o : outputs)
       if (o.kind == k) return &o;
@@ -179,10 +184,11 @@ struct ModelDesc {
   size_t mlm_positions_offset(int64_t rows) const;
   // generate bundles: the regions after the positions, for T = S + N - 1 cache slots. Attention op i (in op order) keeps
   // its K cache [rows, T, H] at kv + 2 i cache_bytes and its V cache right after it; then the decode attention work buffer
-  // (decode_attention_work_bytes at T keys) and the int32 [rows] done flags.
+  // (decode_attention_work_bytes at T keys) and the int32 [rows] done flags; a processing bundle's int32 token histories
+  // hist [rows, S + N] and their prompt lengths hist_len0 [rows] follow (0 on other bundles).
   // counter_bytes: the work buffer's leading int32 counters, the part that must be zero before a request's first step
   struct GenerateScratch {
-    size_t kv = 0, cache_bytes = 0, work = 0, counter_bytes = 0, done = 0, end = 0;
+    size_t kv = 0, cache_bytes = 0, work = 0, counter_bytes = 0, done = 0, hist = 0, hist_len0 = 0, end = 0;
   };
   GenerateScratch generate_scratch(int64_t rows) const;
 };

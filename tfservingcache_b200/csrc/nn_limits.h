@@ -107,6 +107,15 @@ inline bool sampling_temperature_ok(double temperature) {
 inline bool sampling_supported(int vocab, double temperature, int top_k, double top_p) {
   return sampling_temperature_ok(temperature) && top_k >= 0 && top_k <= vocab && top_p > 0 && top_p <= 1;
 }
+// Repetition control (generate.cu): a repetition penalty whose fp32 value is finite, > 0 and normal (the kernel multiplies
+// and divides by it in fp32, as torch does), a no-repeat n-gram size n >= 0 (0: off) and a minimum length m >= 0 (0: off).
+inline bool repetition_penalty_ok(double p) {
+  const float f = (float)p;
+  return p > 0 && p <= FLT_MAX && f >= FLT_MIN && f <= FLT_MAX;
+}
+inline bool processing_supported(double penalty, int ngram, int min_new) {
+  return repetition_penalty_ok(penalty) && ngram >= 0 && min_new >= 0;
+}
 
 // Depthwise convolution (depthwise.cu): a thread runs the kh x kw taps of one output pixel for 4 channels (1 on the scalar
 // path). Kernels up to 7 x 7, stride 1 or 2 and padding up to k / 2 cover MobileNetV2 and EfficientNet B0-B7 (3 x 3 and

@@ -860,11 +860,18 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
             e = exec(o);
           }
         }
-        if (e == cudaSuccess && d.gen_sampling)  // a sampling bundle draws each row's token with its seed (the loader's checks)
+        const int* seeds = d.gen_sampling ? (const int*)x + d.input(InputRole::Seed)->offset : nullptr;
+        if (e == cudaSuccess && d.gen_processing)  // repetition control over each row's history of attended prompt and generated ids
+          e = launch_generate_process((const float*)out, d.ops.back().cout, d.head_n, positions, t, t == d.head_k - 1, d.gen_eos,
+                                      done, go, (const float*)(dm.dptr + emb.word_off), (const float*)(dm.dptr + emb.pos_off),
+                                      (float*)buf(emb.dst), B, emb.c, ids, mask_input, stride ? stride : emb.h,
+                                      reinterpret_cast<int*>(scratch + gs.hist), emb.h + d.head_k,
+                                      reinterpret_cast<int*>(scratch + gs.hist_len0), d.gen_repetition_penalty, d.gen_no_repeat_ngram,
+                                      d.gen_min_new_tokens, seeds, d.in_dim, d.gen_temperature, d.gen_top_k, d.gen_top_p, st);
+        else if (e == cudaSuccess && d.gen_sampling)  // a sampling bundle draws each row's token with its seed (the loader's checks)
           e = launch_generate_sample((const float*)out, d.ops.back().cout, d.head_n, positions, t, t == d.head_k - 1, d.gen_eos,
                                      done, go, (const float*)(dm.dptr + emb.word_off), (const float*)(dm.dptr + emb.pos_off),
-                                     (float*)buf(emb.dst), B, emb.c, (const int*)x + d.input(InputRole::Seed)->offset, d.in_dim,
-                                     d.gen_temperature, d.gen_top_k, d.gen_top_p, st);
+                                     (float*)buf(emb.dst), B, emb.c, seeds, d.in_dim, d.gen_temperature, d.gen_top_k, d.gen_top_p, st);
         else if (e == cudaSuccess)
           e = launch_generate_select((const float*)out, d.ops.back().cout, d.head_n, positions, t, t == d.head_k - 1, d.gen_eos,
                                      done, go, (const float*)(dm.dptr + emb.word_off), (const float*)(dm.dptr + emb.pos_off),

@@ -2017,6 +2017,39 @@ int tfsc_k_generate_sample(const float* logits, int64_t ld, int vocab, const int
                                          seed_stride, temperature, top_k, top_p, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "generate_sample: %s", cudaGetErrorString(e));
 }
+int tfsc_k_generate_process(const float* logits, int64_t ld, int vocab, const int32_t* pos, int t, int last, int eos, int32_t* done,
+                            int32_t* ids, int64_t ids_ld, float* log_probs, int64_t lp_ld, int32_t* length, int64_t length_ld,
+                            const float* word, const float* pos_table, float* y, int rows, int H, const int32_t* prompt_ids,
+                            const int32_t* mask, int64_t stride, int32_t* hist, int64_t hist_ld, int32_t* hist_len0,
+                            float repetition_penalty, int no_repeat_ngram_size, int min_new_tokens, const int32_t* seeds,
+                            int64_t seed_stride, float temperature, int top_k, float top_p, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (!logits || !pos || !done || rows < 0 || t < 0 || vocab < 1 || vocab > kNextTokenMaxVocab || ld < vocab || H < 1 ||
+      (!last && (!word || !pos_table || !y)) || !prompt_ids || stride < 1 || !hist || hist_ld <= t || !hist_len0)
+    return fail(TFSC_E_INVALID, "generate_process: no kernel for %d rows of vocab = %d, ld = %lld, H = %d, stride = %lld, hist_ld ="
+                " %lld at t = %d (1 <= vocab <= %d, ld >= vocab, prompt ids, hist and hist_len0, stride >= 1, hist_ld > t, the tables"
+                " and y unless last)", rows, vocab, (long long)ld, H, (long long)stride, (long long)hist_ld, t, kNextTokenMaxVocab);
+  if (!processing_supported(repetition_penalty, no_repeat_ngram_size, min_new_tokens) ||
+      (min_new_tokens > 0 && (eos < 0 || eos >= vocab)))
+    return fail(TFSC_E_INVALID, "generate_process: repetition_penalty = %g, no_repeat_ngram_size = %d, min_new_tokens = %d, eos = %d"
+                " (a finite, normal fp32 penalty > 0, n >= 0, m >= 0, an eos below vocab = %d when m > 0)", (double)repetition_penalty,
+                no_repeat_ngram_size, min_new_tokens, eos, vocab);
+  if (seeds && (seed_stride < 1 || !sampling_supported(vocab, temperature, top_k, top_p)))
+    return fail(TFSC_E_INVALID, "generate_process: seed_stride = %lld, temperature = %g, top_k = %d, top_p = %g (seed_stride >= 1,"
+                " a finite temperature > 0 with a finite reciprocal, 0 <= top_k <= vocab = %d, 0 < top_p <= 1)", (long long)seed_stride,
+                (double)temperature, top_k, (double)top_p, vocab);
+  GenerateOutputs o;
+  o.ids = ids;
+  o.ids_ld = ids_ld;
+  o.log_probs = log_probs;
+  o.log_probs_ld = lp_ld;
+  o.length = length;
+  o.length_ld = length_ld;
+  cudaError_t e = launch_generate_process(logits, ld, vocab, pos, t, last != 0, eos, done, o, word, pos_table, y, rows, H, prompt_ids,
+                                          mask, stride, hist, hist_ld, hist_len0, repetition_penalty, no_repeat_ngram_size,
+                                          min_new_tokens, seeds, seed_stride, temperature, top_k, top_p, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "generate_process: %s", cudaGetErrorString(e));
+}
 int tfsc_debug_gemm_trace(long long*) {
   return fail(TFSC_E_UNIMPLEMENTED, "no GEMM clock trace: the persistent GEMM kernel it timed is not part of the sm_90a build");
 }

@@ -433,7 +433,13 @@ def gpt2_manifest(seq=1024, hidden=768, layers=12, heads=12, vocab=50257, max_po
     0 <= top_k <= vocab, 0 = off) or "top_p" (0 < top_p <= 1, 1 = off), the same on every entry that gives one, make it a
     sampling bundle: each token is drawn from the temperature / top-k / top-p distribution with the row's seed, so its
     inputs need a "seed" role (GPT2_SAMPLING_INPUTS: an int32 [B, 1] "seed" beside the ids and mask, or
-    [{"name": "input_ids", "role": "ids"}, {"name": "seed", "role": "seed"}] without a mask).
+    [{"name": "input_ids", "role": "ids"}, {"name": "seed", "role": "seed"}] without a mask). Entries that give
+    "repetition_penalty" (a finite number > 0 whose fp32 value is normal; 1 = off), "no_repeat_ngram_size" (an integer
+    1 <= n <= seq + N - 1) or "min_new_tokens" (an integer 1 <= m <= N; needs "eos_token_id"), the same on every entry that
+    gives one, make it a processing bundle, greedy or sampling: each step penalises the ids of the row's history (its
+    attended prompt ids and the tokens so far), bans every token that would repeat an n-gram of it and bans EOS before
+    step m, as transformers' processors of the same names, and picks the token from the processed logits;
+    generated_log_probs stay the model's raw log-probabilities.
     Buffers: 0 residual stream, 1 normed / attention context, 2 qkv / MLP hidden, 3 post-attention residual."""
     ops = [{"op": "embed", "src": -1, "dst": 0, "h": seq, "w": 1, "c": hidden, "vocab": vocab, "max_pos": max_pos, "norm": False}]
 

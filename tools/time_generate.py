@@ -1,6 +1,7 @@
 """Time of greedy and sampled generation on GPT-2 small on cuda:0, from CUDA events.
 
-    python -m tools.time_generate [--launches 200] [--repeats 5] [--new 64] [--model-repeats 3] [--profile] [--sampling] [--parent PKGDIR]
+    python -m tools.time_generate [--launches 200] [--repeats 5] [--new 64] [--model-repeats 3] [--profile] [--sampling]
+                                  [--processing] [--parent PKGDIR]
 
 1. tfsc_k_decode_attention at rows in {1, 8, 64} and L in {128, 1024} keys, 12 heads of width 64: median of `repeats`
    windows of `launches` back-to-back launches, microseconds per launch, and the GB/s of K and V cache read (2 * rows * L * H
@@ -12,12 +13,17 @@
 3. --profile: in a run of its own, torch.profiler's split of the decode steps' kernel time by kernel family at 8 rows and
    prompt 960 (the batch minus a prefill-only batch).
 4. --parent PKGDIR: ResNet-50, BERT-base and the tenant MLP (tools/time_convnets.py's comparison), GPT-2 small
-   next-token at 8 x 128 (every next-token output, half the rows right-padded) and greedy generation of 32 tokens there,
+   next-token at 8 x 128 (every next-token output, half the rows right-padded) and greedy and sampled (top_k 50, top_p 0.9)
+   generation of 32 tokens there,
    against a package built from another commit, alternating the two in child processes: ms per batch over windows of --steps calls, and bit-for-bit outputs.
 5. --sampling: tfsc_k_generate_sample against tfsc_k_generate_select at rows in {1, 8, 64}, vocab 50257, for temperature
    only, top_k 50, top_p 0.9 and top_k 200 with top_p 0.95 (microseconds per launch, the two alternating), and a sampling
    bundle (top_k 50, top_p 0.9) against the greedy bundle end to end at prompt {128, 960} x rows {1, 8, 64}, N = --new:
    ms per batch and generated tokens/s, alternating.
+6. --processing: tfsc_k_generate_process (repetition_penalty 1.3, no_repeat_ngram_size 0 or 3; greedy, and top_k 50 /
+   top_p 0.9 sampled) against tfsc_k_generate_select and tfsc_k_generate_sample at rows in {1, 8, 64}, vocab 50257, histories
+   of 128 and 1024 prompt tokens (a t = 1 step: the history built), alternating; and processing bundles (p 1.3, n 3) against
+   the greedy and sampling bundles end to end at prompt {128, 960} x rows {1, 8, 64}, N = --new, alternating.
 Prints one JSON object with the card name and power limit. Bundles go to a temporary directory, removed at the end."""
 import argparse
 import json
@@ -198,6 +204,98 @@ def sampling_model_table(torch, t, args):
     return res
 
 
+def process_kernel_table(torch, t, args):
+    """us per launch of the select and sample steps and of the processing step on the same GPT-2-sized logits, alternating"""
+    lib = t._lib.lib
+    res = {}
+    gen = torch.Generator(device="cuda").manual_seed(0)
+    ld = (V + 31) // 32 * 32
+    for rows in (1, 8, 64):
+        for S in (128, 1024):
+            x = torch.randn(rows, ld, device="cuda", generator=gen) * 3
+            prompt = torch.randint(0, 64, (rows, S), device="cuda", generator=gen, dtype=torch.int32)  # repeats for the n-gram ban
+            mask = torch.ones(rows, S, dtype=torch.int32, device="cuda")
+            pos = torch.full((rows,), S - 1, dtype=torch.int32, device="cuda")
+            done = torch.zeros(rows, dtype=torch.int32, device="cuda")
+            seeds = torch.arange(rows, dtype=torch.int32, device="cuda")
+            ids = torch.empty(rows, 2, dtype=torch.int32, device="cuda")
+            lp = torch.empty(rows, 2, device="cuda")
+            hist = torch.empty(rows, S + 2, dtype=torch.int32, device="cuda")
+            hl0 = torch.empty(rows, dtype=torch.int32, device="cuda")
+            word, ptab, y = torch.randn(V, H, device="cuda"), torch.randn(S + 2, H, device="cuda"), torch.empty(rows, H, device="cuda")
+            common = lambda t_: (x.data_ptr(), ld, V, pos.data_ptr(), t_, 0, -1, done.data_ptr(), ids.data_ptr(), 2, lp.data_ptr(),  # noqa: E731
+                                 2, None, 0, word.data_ptr(), ptab.data_ptr(), y.data_ptr(), rows, H)
+
+            def process(n, sampled, t_=1):
+                smp = (seeds.data_ptr(), 1, 1.0, 50, 0.9) if sampled else (None, 0, 1.0, 0, 1.0)
+                t._lib.check(lib.tfsc_k_generate_process(*common(t_), prompt.data_ptr(), mask.data_ptr(), S, hist.data_ptr(), S + 2,
+                                                         hl0.data_ptr(), 1.3, n, 0, *smp, None), "process")
+            fns = {"select": lambda: t._lib.check(lib.tfsc_k_generate_select(*common(1), None), "select"),
+                   "sample": lambda: t._lib.check(lib.tfsc_k_generate_sample(*common(1), seeds.data_ptr(), 1, 1.0, 50, 0.9, None), "sample")}
+            for n in (0, 3):
+                fns[f"process_n{n}"] = lambda n=n: process(n, False)
+                fns[f"process_sampled_n{n}"] = lambda n=n: process(n, True)
+            process(3, False, 0)                                          # t = 0: the history
+            torch.cuda.synchronize()
+            us = {k: [] for k in fns}
+            for _ in range(args.repeats):                                 # alternating windows
+                for k, fn in fns.items():
+                    us[k].append(_median_us(torch, fn, args.launches, 1))
+            res[f"rows{rows}_hist{S}"] = {f"{k}_us": round(float(np.median(v)), 2) for k, v in us.items()}
+    return res
+
+
+def processing_model_table(torch, t, args):
+    """processing bundles against the greedy and sampling bundles of the same seeded GPT-2 small, end to end, alternating"""
+    mf = t.modelformat
+    tmp = tempfile.mkdtemp(prefix="tfsc_proc_")
+    res, N = {}, args.new
+    proc = dict(repetition_penalty=1.3, no_repeat_ngram_size=3)
+    smp = dict(top_k=50, top_p=0.9)
+    kinds = {"greedy": ({}, mf.GPT2_INPUTS), "process": (proc, mf.GPT2_INPUTS), "sample": (smp, mf.GPT2_SAMPLING_INPUTS),
+             "process_sample": (dict(proc, **smp), mf.GPT2_SAMPLING_INPUTS)}
+    try:
+        for S in (128, 960):
+            for kind, (fields, inputs) in kinds.items():
+                man = mf.gpt2_manifest(seq=S, inputs=inputs, outputs=[dict(o, **fields) for o in _outs(N)])
+                mf.write_graph_bundle(f"{tmp}/{kind}_s{S}/1", man, seeded_gpt2_blob(man, 0))
+        width = sum(w for _n, _o, w, _d in mf.packed_output_layout(_outs(N), V))
+        cfg = {"modelProvider.type": "diskProvider", "modelProvider.diskProvider.baseDir": tmp, "gpu.devices": [0],
+               "gpu.arenaBytes": 4 << 30, "modelCache.size": 8 << 30, "serving.maxConcurrentModels": 8, "gpu.maxBatch": 64}
+        gen = torch.Generator(device="cuda").manual_seed(0)
+        with t.Server(cfg) as srv:
+            stream = torch.cuda.Stream()
+            for S in (128, 960):
+                for rows in (1, 8, 64):
+                    ids = torch.randint(0, V, (rows, S), device="cuda", generator=gen, dtype=torch.int32)
+                    mask = torch.ones(rows, S, dtype=torch.int32, device="cuda")
+                    seed = torch.arange(rows, dtype=torch.int32, device="cuda")[:, None]
+                    plain, seeded = torch.cat([mask, ids], 1).contiguous(), torch.cat([mask, ids, seed], 1).contiguous()
+                    y = torch.empty(rows, width, device="cuda")
+                    fns = {}
+                    for kind, (_f, inputs) in kinds.items():
+                        name = f"{kind}_s{S}"
+                        srv.ensure(0, name, 1)
+                        x = seeded if inputs is mf.GPT2_SAMPLING_INPUTS else plain
+                        fns[kind] = (lambda name=name, x=x: srv.predict_device(0, name, 1, x.data_ptr(), rows, y.data_ptr(), stream.cuda_stream))
+                        fns[kind]()
+                    srv.sync(0)
+                    ms = {k: [] for k in kinds}
+                    for _ in range(args.model_repeats):
+                        for kind in kinds:
+                            ms[kind].append(_events(torch, fns[kind], 1, stream))
+                    row = {"new_tokens": N}
+                    for kind in kinds:
+                        m_ = float(np.median(ms[kind]))
+                        row[f"{kind}_ms"] = round(m_, 3)
+                        row[f"{kind}_tokens_per_s"] = round(rows * N / m_ * 1e3, 1)
+                    res[f"prompt{S}_rows{rows}"] = row
+                    torch.cuda.empty_cache()
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
+    return res
+
+
 def profile_table(torch, t, args):
     """kernel time of one batch at 8 rows, prompt 960, minus that of the prefill-only bundle, by family"""
     from torch.profiler import ProfilerActivity, profile
@@ -254,6 +352,8 @@ def gpt2_child(out_path, steps, repeats):
         mf.write_graph_bundle(f"{tmp}/gpt2/1", man, seeded_gpt2_blob(man, 0))
         gman = mf.gpt2_manifest(seq=S, inputs=mf.GPT2_INPUTS, outputs=_outs(32))
         mf.write_graph_bundle(f"{tmp}/gen/1", gman, seeded_gpt2_blob(gman, 0))
+        sman = mf.gpt2_manifest(seq=S, inputs=mf.GPT2_SAMPLING_INPUTS, outputs=[dict(o, top_k=50, top_p=0.9) for o in _outs(32)])
+        mf.write_graph_bundle(f"{tmp}/smp/1", sman, seeded_gpt2_blob(sman, 0))
         rng = np.random.default_rng(0)
         ids = rng.integers(0, V, (B, S)).astype(np.int32)
         mask = np.ones((B, S), np.int32)
@@ -264,6 +364,9 @@ def gpt2_child(out_path, steps, repeats):
             out = srv.predict("gpt2", "1", {"input_ids": ids, "attention_mask": mask}, outputs=[o["name"] for o in outs])
             gen = srv.predict("gen", "1", {"input_ids": ids, "attention_mask": mask}, outputs=[o["name"] for o in _outs(32)])
             out.update({f"greedy_{k}": v for k, v in gen.items()})
+            seed = (np.arange(B, dtype=np.int32) * 7919)[:, None]
+            smp = srv.predict("smp", "1", {"input_ids": ids, "attention_mask": mask, "seed": seed}, outputs=[o["name"] for o in _outs(32)])
+            out.update({f"sampled_{k}": v for k, v in smp.items()})
             srv.ensure(0, "gpt2", 1)
             srv.ensure(0, "gen", 1)
             stream = torch.cuda.Stream()
@@ -326,6 +429,7 @@ def main():
     ap.add_argument("--profile", action="store_true")
     ap.add_argument("--skip-models", action="store_true")
     ap.add_argument("--sampling", action="store_true")
+    ap.add_argument("--processing", action="store_true")
     ap.add_argument("--parent", default=None, help="a tfservingcache_b200 package built from the commit to compare against")
     ap.add_argument("--gpt2-child", default=None, help=argparse.SUPPRESS)
     args = ap.parse_args()
@@ -342,6 +446,9 @@ def main():
     if args.sampling:
         res["sample_step"] = sample_kernel_table(torch, t, args)
         res["sampling_models"] = sampling_model_table(torch, t, args)
+    if args.processing:
+        res["process_step"] = process_kernel_table(torch, t, args)
+        res["processing_models"] = processing_model_table(torch, t, args)
     if args.profile:
         res["decode_step_profile"] = profile_table(torch, t, args)
     if args.parent:
