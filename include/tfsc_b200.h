@@ -519,6 +519,24 @@ int tfsc_k_generate_process(const float* logits, int64_t ld, int vocab, const in
                             const int32_t* mask, int64_t stride, int32_t* hist, int64_t hist_ld, int32_t* hist_len0,
                             float repetition_penalty, int no_repeat_ngram_size, int min_new_tokens, const int32_t* seeds,
                             int64_t seed_stride, float temperature, int top_k, float top_p, void* stream);
+/* Scoring. Token row i < n of logits[i * ld, +vocab) (ld >= vocab) is token g = first + i of a [rows, S] batch: row
+ * r = g / S, position p = g % S. When p is attended (mask[r * stride + p] != 0; mask NULL: every position) and s = the
+ * smallest attended position above p exists, it writes, with t = ids[r * stride + s] clamped to [0, vocab):
+ * log_probs[r * S + s] = (z[t] - max z) - (float)log(sum_j exp(z[j] - max z)), fp32 exponentials summed in fp64 (the bits
+ * tfsc_k_generate_select writes when t is the row's argmax), and ranks[r * S + s] = the number of j with z[j] > z[t] plus
+ * the number of j < t with z[j] == z[t] (0: t is the next-token head's top-1). It writes nothing else; the padding columns
+ * from vocab on are never read. TFSC_E_INVALID unless 1 <= S <= 16384, 1 <= vocab <= 57344, [first, first + n) lies within
+ * rows * S, ld >= vocab and stride >= S. */
+int tfsc_k_token_score(const float* logits, int64_t ld, int64_t first, int n, const int32_t* ids, const int32_t* mask, int64_t stride,
+                       int rows, int S, int vocab, float* log_probs, int32_t* ranks, void* stream);
+/* Score head: position s of row r is scored when it is attended (as above) and an attended position lies below it. Writes
+ * token_log_probs[r * lp_ld + s] = log_probs[r * S + s] (0 unscored), token_ranks[r * ranks_ld + s] = ranks[r * S + s]
+ * (-1 unscored), sum[r * sum_ld] = the scored log-probabilities summed in fp64 in an order fixed by S and rounded once
+ * (0 for none) and count[r * count_ld] = the number of scored positions. log_probs and ranks are read at scored positions
+ * only. Output pointers may be NULL. TFSC_E_INVALID unless 1 <= S <= 16384 and stride >= S. */
+int tfsc_k_score_head(const float* log_probs, const int32_t* ranks, const int32_t* mask, int64_t stride, int rows, int S,
+                      float* token_log_probs, int64_t lp_ld, int32_t* token_ranks, int64_t ranks_ld, float* sum, int64_t sum_ld,
+                      int32_t* count, int64_t count_ld, void* stream);
 
 #ifdef __cplusplus
 }

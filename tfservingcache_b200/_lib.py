@@ -164,6 +164,9 @@ _sig("tfsc_k_generate_sample", C.c_int, vp, C.c_int64, C.c_int, vp, C.c_int, C.c
 _sig("tfsc_k_generate_process", C.c_int, vp, C.c_int64, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int64, vp, C.c_int64, vp,
      C.c_int64, vp, vp, vp, C.c_int, C.c_int, vp, vp, C.c_int64, vp, C.c_int64, vp, C.c_float, C.c_int, C.c_int, vp, C.c_int64,
      C.c_float, C.c_int, C.c_float, vp)
+_sig("tfsc_k_token_score", C.c_int, vp, C.c_int64, C.c_int64, C.c_int, vp, vp, C.c_int64, C.c_int, C.c_int, C.c_int, vp, vp, vp)
+_sig("tfsc_k_score_head", C.c_int, vp, vp, vp, C.c_int64, C.c_int, C.c_int, vp, C.c_int64, vp, C.c_int64, vp, C.c_int64, vp,
+     C.c_int64, vp)
 
 
 class TfscError(RuntimeError):

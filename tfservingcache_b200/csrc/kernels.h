@@ -237,6 +237,32 @@ cudaError_t launch_generate_process(const float* logits, int64_t ld, int vocab, 
                                     int* hist_len0, float penalty, int ngram, int min_new, const int* seeds, int64_t seed_stride,
                                     float temperature, int top_k, float top_p, cudaStream_t s);
 
+// Scoring (score.cu). Token row i < n of logits[i * ld, +vocab) (ld >= vocab) is token g = first + i of a [rows, S] batch:
+// row r = g / S, position p = g % S. When p is attended (mask[r * stride + p] != 0; mask nullptr: every position) and
+// s = the smallest attended position above p exists, it writes, with t = ids[r * stride + s] clamped to [0, vocab),
+// log_probs[r * S + s] = (z[t] - max z) - (float)log(sum_j expf(z[j] - max z)) (the sum in fp64, the select step's
+// helpers and block size, so the bits of launch_generate_select's log-probability for g = t) and
+// ranks[r * S + s] = #{j : z[j] > z[t]} + #{j < t : z[j] == z[t]}; it writes nothing else. cudaErrorInvalidValue outside
+// score_supported (nn_limits.h), for stride < S or a null pointer.
+cudaError_t launch_token_score(const float* logits, int64_t ld, int64_t first, int n, const int* ids, const int* mask,
+                               int64_t stride, int S, int vocab, float* log_probs, int* ranks, cudaStream_t s);
+// Score head: for each row r and position s of [rows, S], scored when s is attended and an attended position lies below it,
+// writes at ptr + r * ld (ld in 32-bit words) token_log_probs[s] = log_probs[r * S + s] (0 unscored), token_ranks[s] =
+// ranks[r * S + s] (-1 unscored), the fp64 sum of the scored log-probabilities in an order fixed by S, rounded once to fp32,
+// and the number of scored positions. Reads log_probs / ranks at scored positions only. Any output pointer may be nullptr.
+struct ScoreOutputs {
+  float* log_probs = nullptr;
+  int64_t log_probs_ld = 0;
+  int* ranks = nullptr;
+  int64_t ranks_ld = 0;
+  float* sum = nullptr;
+  int64_t sum_ld = 0;
+  int* count = nullptr;
+  int64_t count_ld = 0;
+};
+cudaError_t launch_score_head(const float* log_probs, const int* ranks, const int* mask, int64_t stride, int rows, int S,
+                              const ScoreOutputs& o, cudaStream_t s);
+
 // wgmma 3xTF32 version of launch_gemm (gemm_tc.cu) for M >= 64, N % 32 == 0, K >= 32, lda % 4 == 0
 bool gemm_tc_supported(const float* A, const float* B, const float* bias, const float* R, const float* C, int M, int N, int K,
                        int lda);

@@ -26,6 +26,7 @@ size_t ModelDesc::scratch_bytes(int64_t rows) const {
   if (tmpl == Template::Mlp) return 2 * (((size_t)rows * (size_t)(max_width > 0 ? max_width : 1) * 4 + 255) & ~(size_t)255);
   if (tmpl == Template::Graph) {
     if (head == HeadKind::Generate) return generate_scratch(rows).end;
+    if (head == HeadKind::Score) return score_scratch(rows).end;
     size_t last = 1;
     for (auto v : output_shape) last *= (size_t)v;
     // a fill-mask bundle's int32 [rows, M] positions follow the head's logits, a next-token bundle's [rows]
@@ -75,13 +76,24 @@ ModelDesc::GenerateScratch ModelDesc::generate_scratch(int64_t rows) const {
   return g;
 }
 
+ModelDesc::ScoreScratch ModelDesc::score_scratch(int64_t rows) const {
+  const GraphOp& op = ops.back();  // the token_score op: [S, 1, H] -> Vp logits per token
+  const size_t tokens = (size_t)rows * (size_t)op.h;
+  ScoreScratch s;
+  s.logits = head_scratch_offset(rows);
+  s.log_probs = s.logits + align256(std::min(tokens, (size_t)kScoreChunkTokens) * (size_t)op.cout * 4);
+  s.ranks = s.log_probs + align256(tokens * 4);
+  s.end = s.ranks + align256(tokens * 4);
+  return s;
+}
+
 // ------------------------------------------------------------------------------------------------ output kinds ----
 // A row of an output kind in the bundle's head_n / head_k (ModelDesc): one int64 scalar (2 words), one 32-bit scalar, a
 // vector of head_n or head_k values, or a head_k x head_n / head_n x head_k matrix
 enum class Rows { Int64, One, N, K, KxN, NxK };
 // The entry fields a kind takes besides name and kind: "k"; "k", "max_answer_length" and "sep_id"; "normalize"; or
-// "max_new_tokens" and "eos_token_id"
-enum class Fields { None, K, Span, Normalize, Generate };
+// "max_new_tokens" and "eos_token_id"; or none at all (a score entry refuses every other field)
+enum class Fields { None, K, Span, Normalize, Generate, Score };
 struct OutputKindInfo {
   const char* name;
   HeadKind head;
@@ -116,6 +128,10 @@ static constexpr OutputKindInfo kOutputKinds[] = {
     {"generated_ids", HeadKind::Generate, TFSC_DT_INT32, Rows::K, Fields::Generate},
     {"generated_log_probs", HeadKind::Generate, TFSC_DT_FLOAT, Rows::K, Fields::Generate},
     {"generated_length", HeadKind::Generate, TFSC_DT_INT32, Rows::One, Fields::Generate},
+    {"token_log_probs", HeadKind::Score, TFSC_DT_FLOAT, Rows::N, Fields::Score},
+    {"token_ranks", HeadKind::Score, TFSC_DT_INT32, Rows::N, Fields::Score},
+    {"token_log_prob_sum", HeadKind::Score, TFSC_DT_FLOAT, Rows::One, Fields::Score},
+    {"token_count", HeadKind::Score, TFSC_DT_INT32, Rows::One, Fields::Score},
 };
 static_assert(sizeof(kOutputKinds) / sizeof(kOutputKinds[0]) == (size_t)kLastOutputKind + 1, "one row per OutputKind");
 
@@ -160,6 +176,9 @@ static std::string next_token_limits() {
 static std::string generate_limits() {
   return "1 <= vocab <= " + std::to_string(kNextTokenMaxVocab) + ", 1 <= max_new_tokens <= " + std::to_string(kDecodeMaxKeys);
 }
+static std::string score_limits() {
+  return "1 <= S <= " + std::to_string(kScoreMaxS) + ", 1 <= vocab <= " + std::to_string(kNextTokenMaxVocab);
+}
 static bool encoder_fits(int S, int H, std::string* err) {
   if (encoder_head_supported(S, H)) return true;
   *err = "signature.outputs: no encoder head kernel for S = " + std::to_string(S) + " and H = " + std::to_string(H) +
@@ -171,6 +190,12 @@ bool layout_outputs(ModelDesc* d, std::string* err) {
   set_head(d);
   const bool with_k = declares_k(*d);
   switch (d->head) {
+    case HeadKind::Score:  // vocab is the owner's business, so only S decides whether a row can be laid out
+      if (!score_supported(d->head_n, 1) || d->head_k != 0) {
+        *err = "signature.outputs: no score head for S = " + std::to_string(d->head_n) + " (1 <= S <= " + std::to_string(kScoreMaxS) + ")";
+        return false;
+      }
+      break;
     case HeadKind::Generate:
       if (!generate_supported(d->head_n, d->head_k)) {
         *err = "signature.outputs: no generate head for vocab = " + std::to_string(d->head_n) + " and max_new_tokens = " +
@@ -378,17 +403,20 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
     const OutputKindInfo* ki = nullptr;
     for (auto& i : kOutputKinds)
       if (kind == i.name) ki = &i;
-    if (!ki) {  // a name that starts with next_token or generated is told the kinds of that head, any other the kinds of
-      // the heads before them
+    if (!ki) {  // a name that starts with next_token, generated or token_ is told the kinds of that head, any other the kinds
+      // of the heads before them
       const HeadKind told = kind.rfind("next_token", 0) == 0 ? HeadKind::NextToken
                             : kind.rfind("generated", 0) == 0 ? HeadKind::Generate
+                            : kind.rfind("token_", 0) == 0    ? HeadKind::Score
                                                                 : HeadKind::None;
       *err = "signature.outputs: unknown " +
-             std::string(told == HeadKind::NextToken ? "next-token " : told == HeadKind::Generate ? "generate " : "") + "kind '" +
-             kind + "' (";
+             std::string(told == HeadKind::NextToken ? "next-token " : told == HeadKind::Generate ? "generate "
+                                                                   : told == HeadKind::Score  ? "score " : "") +
+             "kind '" + kind + "' (";
       bool any = false;
       for (auto& i : kOutputKinds)
-        if (i.head == told || (told == HeadKind::None && i.head != HeadKind::NextToken && i.head != HeadKind::Generate))
+        if (i.head == told || (told == HeadKind::None && i.head != HeadKind::NextToken && i.head != HeadKind::Generate &&
+                               i.head != HeadKind::Score))
           *err += std::string(any ? ", " : "") + i.name, any = true;
       *err += ")";
       return false;
@@ -405,6 +433,11 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
       }
     const HeadKind h = ki->head, first = d->outputs.empty() ? h : kind_info(d->outputs.front().kind).head;
     const std::string is = " ('" + mo.name + "' is " + kind + ")";
+    if ((h == HeadKind::Score) != (first == HeadKind::Score)) {
+      *err = "signature.outputs: score outputs (token_log_probs, token_ranks, token_log_prob_sum, token_count) cannot be mixed"
+             " with classification, span, encoder, fill-mask, next-token or generate outputs" + is;
+      return false;
+    }
     if ((h == HeadKind::Generate) != (first == HeadKind::Generate)) {
       *err = "signature.outputs: generate outputs (generated_ids, generated_log_probs, generated_length) cannot be mixed with"
              " classification, span, encoder, fill-mask or next-token outputs" + is;
@@ -420,7 +453,7 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
              " masked_top_k_logits) cannot be mixed with classification, span or encoder outputs" + is;
       return false;
     }
-    if (h != HeadKind::FillMask && h != HeadKind::NextToken && h != HeadKind::Generate) {
+    if (h != HeadKind::FillMask && h != HeadKind::NextToken && h != HeadKind::Generate && h != HeadKind::Score) {
       if ((h == HeadKind::Encoder) != (first == HeadKind::Encoder)) {
         *err = "signature.outputs: encoder outputs (sequence_output, pooled_output, cls_embedding, mean_embedding) cannot be mixed"
                " with classification or span outputs" + is;
@@ -446,6 +479,14 @@ static bool parse_outputs(const Json& outs, ModelDesc* d, std::string* err) {
     const bool span_fields = oj.get("max_answer_length") || oj.get("sep_id");
     int v = 0;
     switch (h) {
+      case HeadKind::Score:  // no field of another head's entries: a score entry has no k, length or sampling to give
+        for (const char* f : {"k", "normalize", "max_answer_length", "sep_id", "max_new_tokens", "eos_token_id", "temperature",
+                              "top_k", "top_p", "repetition_penalty", "no_repeat_ngram_size", "min_new_tokens"})
+          if (oj.get(f)) {
+            *err = "signature.outputs: '" + std::string(f) + "' does not apply to score outputs" + is;
+            return false;
+          }
+        break;
       case HeadKind::FillMask:
         if (oj.get("normalize") || span_fields) {
           *err = "signature.outputs: 'normalize', 'max_answer_length' and 'sep_id' do not apply to fill-mask outputs" + is;
@@ -797,6 +838,53 @@ static bool check_generate_bundle(ModelDesc* d, int last_tokens, std::string* er
   return true;
 }
 
+// the score head: one token_score op, the last, projects the decoder's [S, 1, H] hidden states (after ln_f) to Vp >= vocab
+// logits per token in chunks and scores each attended token under the attended position before it: head_n = S. Between the
+// embed and the token_score op the decoder is any graph of the embed's S tokens whose attention is causal, so that the
+// logits at p see no later token.
+static bool check_score_bundle(ModelDesc* d, int scores, std::string* err) {
+  if (!embed_graph(*d, "score", "a GPT-2 decoder, its ln_f and a token_score op", err)) return false;
+  if (scores != 1) {
+    *err = "signature.outputs: score outputs need exactly one token_score op (the bundle has " + std::to_string(scores) + ")";
+    return false;
+  }
+  const GraphOp& emb = d->ops.front();
+  const int S = emb.h, H = emb.c, V = emb.vocab;
+  const GraphOp& op = d->ops.back();
+  if (op.kind != OpKind::TokenScore) {
+    *err = "signature.outputs: score outputs need the token_score op to be the last op";
+    return false;
+  }
+  if (op.src < 0 || op.h != S || op.w != 1 || op.c != H) {
+    *err = "signature.outputs: the token_score op needs the [" + std::to_string(S) + ", 1, " + std::to_string(H) +
+           "] hidden states of a scratch buffer (it reads [" + std::to_string(op.h) + ", " + std::to_string(op.w) + ", " +
+           std::to_string(op.c) + "] of buffer " + std::to_string(op.src) + ")";
+    return false;
+  }
+  if (op.vocab != V) {
+    *err = "signature.outputs: the token_score op's vocab = " + std::to_string(op.vocab) + " differs from the embed op's vocab = " +
+           std::to_string(V);
+    return false;
+  }
+  if (op.cout < V) {
+    *err = "signature.outputs: the token_score op writes cout = " + std::to_string(op.cout) + " logits per token, below vocab = " +
+           std::to_string(V);
+    return false;
+  }
+  for (size_t i = 1; i < d->ops.size(); ++i)
+    if (d->ops[i].kind == OpKind::Attention && !d->ops[i].causal) {
+      *err = "signature.outputs: score outputs need causal attention (op " + std::to_string(i) + " is not causal)";
+      return false;
+    }
+  if (!score_supported(S, V)) {
+    *err = "signature.outputs: no score kernels for S = " + std::to_string(S) + " and vocab = " + std::to_string(V) + " (" +
+           score_limits() + ")";
+    return false;
+  }
+  d->head_n = S;
+  return true;
+}
+
 // ---------------------------------------------------------------------------------------------------- op kinds ----
 // How an op's [oh, ow, cout] follow from its fields: the kh x kw window at stride and pad, cout from the manifest (Pool:
 // cout = c); [h, w, c]; [h, w, c / 3] from the packed q | k | v; [1, 1, c]; [1, 1, cout] with kh = kw = 1; [slots, 1, c];
@@ -845,6 +933,10 @@ static constexpr OpKindInfo kOpKinds[] = {
     // highest position whose mask is set with a mask input, else S - 1; none: zeros) to dst [1, 1, H], and writes that
     // position (int32, -1 none) to the executor's positions scratch for the head
     {"last_token", Geometry::Point, Acts::Refused, Residual::Refused, Weights::None},
+    // score bundles: the vocabulary projection (a 1x1 conv [S, 1, c] -> [S, 1, cout = Vp]) of every token of the [S, 1, H]
+    // hidden states in src, run in chunks of kScoreChunkTokens token rows, each followed by the score kernel: the
+    // log-probability and rank of the next attended token's id under the first `vocab` logits, for the head
+    {"token_score", Geometry::Window, Acts::Refused, Residual::Refused, Weights::Kernel},
 };
 static_assert(sizeof(kOpKinds) / sizeof(kOpKinds[0]) == (size_t)kLastOpKind + 1, "one row per OpKind");
 
@@ -920,6 +1012,9 @@ static std::string kind_error(const Json& oj, GraphOp& o) {
              ", shift " + std::to_string(o.shift) + ") (window <= " + std::to_string(kWindowMaxWs) + ", head width <= " +
              std::to_string(kWindowMaxD) + ", K and V of a window within 48 KB, h * w * 3C < 2^31)";
     }
+    case OpKind::TokenScore:  // the shapes are checked with the score outputs
+      if (o.w == 1 && o.kh == 1 && o.kw == 1 && o.stride == 1 && o.pad == 0) return "";
+      return "token_score projects each of its h tokens: w = 1, kh = kw = stride = 1, pad = 0";
     case OpKind::PatchMerge:
       if (o.h % 2 || o.w % 2) return "patch_merge needs an even h and w (h x w = " + std::to_string(o.h) + " x " + std::to_string(o.w) + ")";
       if (oj.get("cout") && (int)oj.get_int("cout", o.c) != o.cout)
@@ -1245,8 +1340,17 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
     }
   }
   finish(d);
-  int gathers = 0, last_tokens = 0;
-  for (auto& o : d->ops) gathers += o.kind == OpKind::MaskGather, last_tokens += o.kind == OpKind::LastToken;
+  int gathers = 0, last_tokens = 0, scores = 0;
+  for (auto& o : d->ops)
+    gathers += o.kind == OpKind::MaskGather, last_tokens += o.kind == OpKind::LastToken, scores += o.kind == OpKind::TokenScore;
+  if (scores && d->head != HeadKind::Score) {
+    *err = "graph manifest: a token_score op needs score outputs (token_log_probs, token_ranks, token_log_prob_sum, token_count)";
+    return false;
+  }
+  if (d->head == HeadKind::Score && (gathers || last_tokens)) {
+    *err = "graph manifest: a score bundle scores every token: it has no last_token or mask_gather op";
+    return false;
+  }
   if (gathers && d->head != HeadKind::FillMask) {
     *err = "graph manifest: a mask_gather op needs fill-mask outputs (masked_positions, masked_top_k_ids, "
            "masked_top_k_probabilities, masked_top_k_logits)";
@@ -1267,6 +1371,7 @@ bool parse_manifest(const Json& j, ModelDesc* d, std::string* err) {
   if (d->outputs.empty()) return seed_ok();
   bool ok = false;
   switch (d->head) {
+    case HeadKind::Score: ok = check_score_bundle(d, scores, err); break;
     case HeadKind::Generate: ok = check_generate_bundle(d, last_tokens, err); break;
     case HeadKind::NextToken: ok = check_next_token_bundle(d, last_tokens, err); break;
     case HeadKind::FillMask: ok = check_fill_mask_bundle(d, gathers, err); break;

@@ -18,8 +18,8 @@ enum class Template { Affine, Mlp, Graph };
 // request tensor, -2 = the response tensor). What each kind computes, its manifest name, shape rule, activations,
 // residual and weights are in the op kind table (model.cc).
 enum class OpKind { Conv, MaxPool, AvgPool, Dense, Embed, LayerNorm, Attention, MaskGather, DepthwiseConv, ChannelScale,
-                    WindowAttention, PatchMerge, LastToken };
-constexpr OpKind kLastOpKind = OpKind::LastToken;
+                    WindowAttention, PatchMerge, LastToken, TokenScore };
+constexpr OpKind kLastOpKind = OpKind::TokenScore;
 struct GraphOp {
   OpKind kind = OpKind::Conv;
   int src = -1, dst = 0, res = -100;  // res = -100: no residual input
@@ -73,8 +73,10 @@ int64_t place_inputs(std::vector<ModelInput>* inputs, int64_t S);
 // FillMask (masked-language-model prediction): the [M, 1, Vp] vocabulary logits of the M [MASK] slots a mask_gather op
 // selected (mlm.cu). NextToken (causal language-model prediction): the [1, 1, Vp] vocabulary logits of the one token a
 // last_token op selected per row (the fill-mask head's kernel with one slot). Generate (greedy generation): a next-token
-// bundle's graph run once on the prompt and then once per new token on a KV cache (generate.cu).
-enum class HeadKind { None, Classify, Span, Encoder, FillMask, NextToken, Generate };
+// bundle's graph run once on the prompt and then once per new token on a KV cache (generate.cu). Score (scoring the input):
+// the log-probability and rank of every attended token under the logits of the attended position before it, which a
+// token_score op computes in chunks of the vocabulary projection over all S tokens (score.cu).
+enum class HeadKind { None, Classify, Span, Encoder, FillMask, NextToken, Generate, Score };
 
 // One declared output of a multi-output bundle (signature.outputs). Its name, head, dtype and per-row shape are in the
 // kind table (model.cc). New kinds go at the end: the forward hop sends the enum's numbers.
@@ -84,9 +86,10 @@ enum class OutputKind {
   SequenceOutput, PooledOutput, ClsEmbedding, MeanEmbedding,
   MaskedPositions, MaskedTopKIds, MaskedTopKProbabilities, MaskedTopKLogits,
   NextTokenPosition, NextTokenTopKIds, NextTokenTopKProbabilities, NextTokenTopKLogits,
-  GeneratedIds, GeneratedLogProbs, GeneratedLength
+  GeneratedIds, GeneratedLogProbs, GeneratedLength,
+  TokenLogProbs, TokenRanks, TokenLogProbSum, TokenCount
 };
-constexpr OutputKind kLastOutputKind = OutputKind::GeneratedLength;
+constexpr OutputKind kLastOutputKind = OutputKind::TokenCount;
 struct ModelOutput {
   std::string name;
   OutputKind kind = OutputKind::Logits;
@@ -141,6 +144,7 @@ struct ModelDesc {
   //   FillMask: head_n = M (the mask_gather op's slots), head_k = k (0: masked_positions only).
   //   NextToken: head_n = vocab (the embed op's), head_k = k (0: next_token_position only).
   //   Generate: head_n = vocab (the embed op's), head_k = N (max_new_tokens).
+  //   Score:    head_n = S, head_k = 0.
   // The rest is known to the owner only, the kernels' business: a span head's span_max_len = max_answer_length and
   // span_sep_id = sep_id (-1: none); an encoder head's encoder_pooler (the last op is the pooler: it writes pooled_output,
   // and the hidden states are its source buffer) and normalize_cls / normalize_mean; a fill-mask head's mlm_vocab (the
@@ -191,6 +195,12 @@ struct ModelDesc {
     size_t kv = 0, cache_bytes = 0, work = 0, counter_bytes = 0, done = 0, hist = 0, hist_len0 = 0, end = 0;
   };
   GenerateScratch generate_scratch(int64_t rows) const;
+  // score bundles: after the buffers, the token_score op's logits region for min(kScoreChunkTokens, rows * S) token rows of
+  // Vp columns, then the fp32 log-probabilities and int32 ranks [rows, S] its score kernel writes and the head reads
+  struct ScoreScratch {
+    size_t logits = 0, log_probs = 0, ranks = 0, end = 0;
+  };
+  ScoreScratch score_scratch(int64_t rows) const;
 };
 
 // Set d->head from the first output's kind, sort d->outputs by name, set their offsets and widths from d->head_n / d->head_k

@@ -75,6 +75,12 @@ inline bool next_token_supported(int vocab, int k) {
   return vocab >= 1 && vocab <= kNextTokenMaxVocab && k >= 1 && k <= kHeadMaxK && k <= vocab;
 }
 
+// Scoring (score.cu): the token_score op projects at most kScoreChunkTokens token rows of the flattened [rows x S] batch at a
+// time into one chunk-sized logits region (206 MB at Vp = 50272), and its score kernel stages a row of `vocab` logits like the
+// next-token head (vocab <= 57344). The score head walks the S positions of a row.
+constexpr int kScoreChunkTokens = 1024, kScoreMaxS = 16384;
+inline bool score_supported(int S, int vocab) { return S >= 1 && S <= kScoreMaxS && vocab >= 1 && vocab <= kNextTokenMaxVocab; }
+
 // Decode attention (generate.cu): one query per row over L cached keys, split into blocks of kDecodeKeys keys, one CTA per
 // (row, head, block). A CTA stages its block's keys in shared memory (34 KB at d = 128, within the 48 KB a kernel gets
 // without opting in) and the last CTA of a (row, head) combines the blocks in order. Head width d % 4 == 0, d <= 128.

@@ -578,8 +578,9 @@ size_t Node::model_ws_bytes(const ModelDesc& d) {
   }
   bool after_gather = false;
   for (auto& o : d.ops) {  // graph bundles: plain dense heads (ResNet fc) run on the weight-streaming dense kernels
-    // and so does a fill-mask bundle's vocabulary projection on a few rows (run_model)
-    if (o.kind == OpKind::Dense || (after_gather && o.kind == OpKind::Conv)) {
+    // and so does a fill-mask bundle's vocabulary projection on a few rows, and a score bundle's on a chunk of a few tokens
+    // (run_model)
+    if (o.kind == OpKind::Dense || o.kind == OpKind::TokenScore || (after_gather && o.kind == OpKind::Conv)) {
       size_t w = dense_workspace_bytes(kMaxRowsPerLaunch, o.c, o.cout);
       if (w > m) m = w;
     }
@@ -807,6 +808,28 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
           e = launch_last_token(src, mask_input, stride ? stride : o.h, B, o.h, o.c, positions, dst, st);
           after_gather = true;  // the vocabulary projection below 64 rows streams its weights, as fill-mask's
           break;
+        case OpKind::TokenScore: {
+          // the [B * S, Vp] logits would take B * S * Vp * 4 bytes (26 GB at 128 x 1024 tokens), so the projection runs on
+          // chunks of kScoreChunkTokens token rows, each into the same region and then scored (DESIGN §4). A chunk takes the
+          // route a next-token projection of that many rows takes: the weight-streaming dense kernels below 64 rows (the
+          // cluster kernel up to 8, dense_tc from 9), the tensor-core GEMM from 64. Every route waits for the previous
+          // chunk's score kernel (griddepcontrol.wait) before it writes the region.
+          const ModelDesc::ScoreScratch ss = d.score_scratch(rows);
+          float* logits = (float*)(scratch + ss.logits);
+          const float* W = (const float*)(dm.dptr + o.w_off);
+          const float* bias = (const float*)(dm.dptr + o.b_off);
+          const int64_t tokens = (int64_t)B * o.h;
+          for (int64_t first = 0; e == cudaSuccess && first < tokens; first += kScoreChunkTokens) {
+            const int n = (int)std::min<int64_t>(kScoreChunkTokens, tokens - first);
+            const float* xc = src + first * o.c;
+            e = n < 64 && o.cout % 32 == 0 ? launch_dense(xc, W, bias, logits, n, o.c, o.cout, false, ws, ws_cap, st)
+                                           : launch_gemm(xc, W, bias, nullptr, logits, n, o.cout, o.c, o.c, 0, st);
+            if (e == cudaSuccess)
+              e = launch_token_score(logits, o.cout, first, n, ids, mask_input, stride ? stride : o.h, o.h, o.vocab,
+                                     (float*)(scratch + ss.log_probs), (int*)(scratch + ss.ranks), st);
+          }
+          break;
+        }
       }
       return e;
     };
@@ -878,6 +901,22 @@ cudaError_t Node::run_model(const DeviceModel& dm, const char* x, int64_t rows, 
                                      (float*)buf(emb.dst), B, emb.c, st);
       }
       return e;
+    }
+    if (d.head == HeadKind::Score) {  // the token_score op left each scored token's log-probability and rank in scratch
+      const ModelDesc::ScoreScratch ss = d.score_scratch(rows);
+      ScoreOutputs so;
+      for (const ModelOutput& m : d.outputs) {
+        float* p = reinterpret_cast<float*>(y) + m.offset;
+        switch (m.kind) {
+          case OutputKind::TokenLogProbs: so.log_probs = p, so.log_probs_ld = d.out_dim; break;
+          case OutputKind::TokenRanks: so.ranks = reinterpret_cast<int*>(p), so.ranks_ld = d.out_dim; break;
+          case OutputKind::TokenLogProbSum: so.sum = p, so.sum_ld = d.out_dim; break;
+          case OutputKind::TokenCount: so.count = reinterpret_cast<int*>(p), so.count_ld = d.out_dim; break;
+          default: break;
+        }
+      }
+      return launch_score_head((const float*)(scratch + ss.log_probs), (const int*)(scratch + ss.ranks), mask_input,
+                               stride ? stride : d.head_n, B, d.head_n, so, st);
     }
     SpanInputs in;
     in.ids = ids;

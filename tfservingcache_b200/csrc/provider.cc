@@ -280,6 +280,7 @@ std::shared_ptr<HostModel> SyntheticModelProvider::load_model(const std::string&
       switch (o.kind) {
         case OpKind::Conv:
         case OpKind::Dense:
+        case OpKind::TokenScore:  // the vocabulary projection, a 1x1 conv
         case OpKind::DepthwiseConv: {  // depthwise: one kh x kw filter per channel, fan-in kh * kw, cout = c
           const bool dw = o.kind == OpKind::DepthwiseConv;
           const uint64_t fan_in = (uint64_t)o.kh * o.kw * (dw ? 1 : o.c);

@@ -2050,6 +2050,40 @@ int tfsc_k_generate_process(const float* logits, int64_t ld, int vocab, const in
                                           min_new_tokens, seeds, seed_stride, temperature, top_k, top_p, (cudaStream_t)stream);
   return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "generate_process: %s", cudaGetErrorString(e));
 }
+int tfsc_k_token_score(const float* logits, int64_t ld, int64_t first, int n, const int32_t* ids, const int32_t* mask, int64_t stride,
+                       int rows, int S, int vocab, float* log_probs, int32_t* ranks, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (n < 0 || first < 0 || rows < 0 || !score_supported(S, vocab) || first + n > (int64_t)rows * S)
+    return fail(TFSC_E_INVALID, "token_score: no kernel for tokens [%lld, %lld) of %d rows of S = %d, vocab = %d (1 <= S <= %d, 1 <="
+                " vocab <= %d, the tokens within rows * S)", (long long)first, (long long)first + n, rows, S, vocab, kScoreMaxS,
+                kNextTokenMaxVocab);
+  if (!logits || !ids || !log_probs || !ranks || ld < vocab || stride < S)
+    return fail(TFSC_E_INVALID, "token_score: needs the logits, ids and outputs, ld >= vocab and stride >= S (ld = %lld, stride = %lld)",
+                (long long)ld, (long long)stride);
+  cudaError_t e = launch_token_score(logits, ld, first, n, ids, mask, stride, S, vocab, log_probs, ranks, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "token_score: %s", cudaGetErrorString(e));
+}
+int tfsc_k_score_head(const float* log_probs, const int32_t* ranks, const int32_t* mask, int64_t stride, int rows, int S,
+                      float* token_log_probs, int64_t lp_ld, int32_t* token_ranks, int64_t ranks_ld, float* sum, int64_t sum_ld,
+                      int32_t* count, int64_t count_ld, void* stream) {
+  if (int rc = check_device()) return rc;
+  if (rows < 0 || S < 1 || S > kScoreMaxS || stride < S)
+    return fail(TFSC_E_INVALID, "score_head: no kernel for %d rows of S = %d, stride = %lld (1 <= S <= %d, stride >= S)", rows, S,
+                (long long)stride, kScoreMaxS);
+  if (((token_log_probs || sum) && !log_probs) || (token_ranks && !ranks))
+    return fail(TFSC_E_INVALID, "score_head: its outputs need the log-probabilities and ranks they copy");
+  ScoreOutputs o;
+  o.log_probs = token_log_probs;
+  o.log_probs_ld = lp_ld;
+  o.ranks = token_ranks;
+  o.ranks_ld = ranks_ld;
+  o.sum = sum;
+  o.sum_ld = sum_ld;
+  o.count = count;
+  o.count_ld = count_ld;
+  cudaError_t e = launch_score_head(log_probs, ranks, mask, stride, rows, S, o, (cudaStream_t)stream);
+  return e == cudaSuccess ? 0 : fail(TFSC_E_INTERNAL, "score_head: %s", cudaGetErrorString(e));
+}
 int tfsc_debug_gemm_trace(long long*) {
   return fail(TFSC_E_UNIMPLEMENTED, "no GEMM clock trace: the persistent GEMM kernel it timed is not part of the sm_90a build");
 }

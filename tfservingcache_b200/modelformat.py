@@ -22,6 +22,8 @@ def _align256(x: int) -> int:
 # logits); cls_embedding and mean_embedding may carry "normalize": true; classes is one int64 (2 words) and
 # next_token_position one int32. The generate kinds (greedy generation on a GPT-2 bundle, n = the vocabulary) carry
 # "max_new_tokens" = N as their k, the same on every entry, and optionally "eos_token_id"; generated_length is one int32.
+# The score kinds (scoring the input of a GPT-2 bundle, n = S) take a name and a kind only: token_log_probs and token_ranks
+# hold one value per position, token_log_prob_sum and token_count one per row.
 OUTPUT_KIND_TABLE = {
     "logits": ("classify", "float32", "n"), "probabilities": ("classify", "float32", "n"), "classes": ("classify", "int64", ""),
     "top_k_classes": ("classify", "int32", "k"), "top_k_probabilities": ("classify", "float32", "k"),
@@ -35,10 +37,12 @@ OUTPUT_KIND_TABLE = {
     "next_token_top_k_probabilities": ("next_token", "float32", "k"), "next_token_top_k_logits": ("next_token", "float32", "k"),
     "generated_ids": ("generate", "int32", "k"), "generated_log_probs": ("generate", "float32", "k"),
     "generated_length": ("generate", "int32", ""),
+    "token_log_probs": ("score", "float32", "n"), "token_ranks": ("score", "int32", "n"),
+    "token_log_prob_sum": ("score", "float32", ""), "token_count": ("score", "int32", ""),
 }
-OUTPUT_KINDS, SPAN_OUTPUT_KINDS, ENCODER_OUTPUT_KINDS, MLM_OUTPUT_KINDS, NEXT_TOKEN_OUTPUT_KINDS, GENERATE_OUTPUT_KINDS = (
-    tuple(k for k, v in OUTPUT_KIND_TABLE.items() if v[0] == head)
-    for head in ("classify", "span", "encoder", "fill_mask", "next_token", "generate"))
+(OUTPUT_KINDS, SPAN_OUTPUT_KINDS, ENCODER_OUTPUT_KINDS, MLM_OUTPUT_KINDS, NEXT_TOKEN_OUTPUT_KINDS, GENERATE_OUTPUT_KINDS,
+ SCORE_OUTPUT_KINDS) = (tuple(k for k, v in OUTPUT_KIND_TABLE.items() if v[0] == head)
+                        for head in ("classify", "span", "encoder", "fill_mask", "next_token", "generate", "score"))
 
 
 def _signature(sig: dict, outputs):
@@ -143,7 +147,7 @@ def _graph_manifest(input_shape, ops, n_buffers, input_name="x", output_name="y"
         return o
 
     for op in ops:
-        if op["op"] in ("conv", "dense"):
+        if op["op"] in ("conv", "dense", "token_score"):
             k = op.get("kh", 1) * op.get("kw", 1) * op["c"]
             op["w_offset"] = take(k * op["cout"] * 4)
             op["b_offset"] = take(op["cout"] * 4)
@@ -440,6 +444,10 @@ def gpt2_manifest(seq=1024, hidden=768, layers=12, heads=12, vocab=50257, max_po
     attended prompt ids and the tokens so far), bans every token that would repeat an n-gram of it and bans EOS before
     step m, as transformers' processors of the same names, and picks the token from the processed logits;
     generated_log_probs stay the model's raw log-probabilities.
+    With SCORE_OUTPUT_KINDS outputs the bundle scores its input instead: after the same blocks ln_f runs on all seq tokens
+    and a token_score op (the decoder's weights, [seq, 1, hidden] -> Vp logits per token, projected in chunks) gives each
+    attended token but a row's first its log-probability and rank under the logits of the attended position before it
+    (token_log_probs and token_ranks [seq], 0 and -1 at the other positions), and their sum and count per row.
     Buffers: 0 residual stream, 1 normed / attention context, 2 qkv / MLP hidden, 3 post-attention residual."""
     ops = [{"op": "embed", "src": -1, "dst": 0, "h": seq, "w": 1, "c": hidden, "vocab": vocab, "max_pos": max_pos, "norm": False}]
 
@@ -459,6 +467,9 @@ def gpt2_manifest(seq=1024, hidden=768, layers=12, heads=12, vocab=50257, max_po
                 conv(1, 3, seq, hidden, hidden, res=0), ln(3, 1, seq), conv(1, 2, seq, hidden, 4 * hidden, act="gelu_tanh"),
                 conv(2, 0, seq, 4 * hidden, hidden, res=3)]
     vp = (vocab + 31) // 32 * 32
-    ops += [{"op": "last_token", "src": 0, "dst": 1, "h": seq, "w": 1, "c": hidden}, ln(1, 2, 1), conv(2, -2, 1, hidden, vp)]
+    if outputs is not None and any(o.get("kind") in SCORE_OUTPUT_KINDS for o in outputs):
+        ops += [ln(0, 1, seq), {"op": "token_score", "src": 1, "dst": -2, "h": seq, "w": 1, "c": hidden, "cout": vp, "vocab": vocab}]
+    else:
+        ops += [{"op": "last_token", "src": 0, "dst": 1, "h": seq, "w": 1, "c": hidden}, ln(1, 2, 1), conv(2, -2, 1, hidden, vp)]
     return _graph_manifest([seq], ops, 4, input_name="input_ids", output_name="logits", input_dtype="int32", inputs=inputs,
                            outputs=outputs)
